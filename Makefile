@@ -1,4 +1,4 @@
-# Builds the product library (CUDA, sm_100a) and the CPU oracle (test infrastructure).
+# Builds the product library (CUDA, sm_90a) and the CPU oracle (test infrastructure).
 NVCC      ?= /usr/local/cuda/bin/nvcc
 CXX       ?= g++
 CC        ?= gcc
@@ -6,7 +6,7 @@ PKG       := clarabel.rs_b200
 CSRC      := $(PKG)/csrc
 LIB       := $(PKG)/libclarabel_b200.so
 ORACLE    := oracle/liboracle.so
-GENCODE   := -gencode arch=compute_100a,code=sm_100a
+GENCODE   := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := -O3 -std=c++17 -lineinfo --extended-lambda $(GENCODE) -Xcompiler -fPIC,-O3,-Wall -Xptxas -v
 CU_SRCS   := $(wildcard $(CSRC)/*.cu)
 CPP_SRCS  := $(wildcard $(CSRC)/*.cpp)

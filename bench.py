@@ -71,7 +71,7 @@ def load_workload(name, rank):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu_index):
         self.gpu = gpu_index
@@ -226,6 +226,9 @@ def run_ours(args, rank, world):
         durations.extend(take.tolist())
         launches_timed += int(per_iter_launch * len(take))
     torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"x": r["x"], "z": r["z"], "s": r["s"],
+                                         "obj": [r["obj_val"], r["obj_val_dual"]]})
     # re-solve with new data on the same handle (DefaultSolver::update_data): host buffers in, solution out,
     # symbolic analysis / plans / equilibration reused -- the parametric (MPC-style) use of the backend
     t_r0 = time.perf_counter()
@@ -252,8 +255,8 @@ def run_ours(args, rank, world):
             peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         except Exception:
             pass
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
-        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+        hbm_peak = float(peaks.get("hbm_gbs", 3350.0))
+        peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "data sheet 3350 GB/s (H100 SXM HBM3)"
         if shard:
             refactor_ms, ldl_solve_ms, kkt_solve_ms = shard_ms
         else:
@@ -281,14 +284,6 @@ def run_ours(args, rank, world):
                   "frac_stored": b_stored["solve"] / (ldl_solve_ms * 1e-3) / 1e9 / hbm_peak,
                   "accounting": acct % "24 nnzL + 96 N", "ms": ldl_solve_ms, "share_of_step_ms": share_sol,
                   "peak_source": peak_src}
-        # DRAM traffic per launch from the committed ncu --set full capture of this workload (profiles/), if any
-        try:
-            tr = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json"))).get(args.workload, {})
-            rf_ref["traffic"] = tr.get("refactor_dram_bytes")
-            rf_sol["traffic"] = tr.get("solve_dram_bytes")
-            rf_ref["traffic_source"] = rf_sol["traffic_source"] = tr.get("source")
-        except Exception:
-            pass
         # `roofline` is the triangular-solve launch sequence: the kernel the north star's roofline target names, and half
         # of the step together with the refactor (the two shares are within a few per cent of each other on C2 and C4)
         dominant, other = rf_sol, rf_ref
@@ -333,6 +328,23 @@ def run_ours(args, rank, world):
     return out
 
 
+DUMP_BUDGET = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Write what the timed path returned as <out_dir>/<name>.npy (float64), so that two builds can be compared output
+    for output.  Past DUMP_BUDGET bytes in all, every array is cut down to the same fixed, seeded sample of its
+    entries (sorted indices, seed 0)."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float64).ravel() for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    for name, a in arrays.items():
+        if total > DUMP_BUDGET:
+            keep = int(a.size * DUMP_BUDGET // total)
+            a = a[np.sort(np.random.default_rng(0).choice(a.size, keep, replace=False))]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def one_core():
     """Pin the calling process to one core for the single-thread CPU legs (BASELINE.md section 3); returns a restore function."""
     try:
@@ -347,7 +359,7 @@ def cpu_solve(pr, workload, max_iter, perm=None):
     """Reference algorithm on the host: oracle IPM + oracle qdldl (line-faithful C port, oracle/), ONE thread pinned to
     one core.  Ordering: the reference orders with AMD at dense-scale 1.5 (the `amd` crate is not vendored; the
     repo's own AMD stands in).  On C4 that ordering costs the CPU 2.7e12 flops per refactorisation (about half an
-    hour, measured once: profiles/r02_cpu_c4_amd_container.json), so the CPU leg there gets the nested-dissection
+    hour on one core), so the CPU leg there gets the nested-dissection
     ordering the GPU path uses -- 1.5e10 flops, the cheapest ordering known for the reference algorithm: a
     conservative baseline."""
     import clarabel_rs_b200 as cb
@@ -446,6 +458,9 @@ def main():
                     help="with --gpus N > 1: N independent problems (weak scaling) instead of ONE problem split over the N GPUs")
     ap.add_argument("--no-process-warmup", action="store_true",
                     help="skip the tiny warm-up problem (for ncu launch lists: keeps the capture on the workload)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the solution (x, z, s) and objective (primal, dual) of the last "
+                         "timed solve as DIR/<name>.npy, float64, 64 MB at most")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

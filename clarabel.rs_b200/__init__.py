@@ -1,6 +1,6 @@
-"""clarabel.rs_b200 -- B200-native KKT backend (host-side Python mirror).
+"""clarabel.rs_b200 -- GPU-native KKT backend (host-side Python mirror).
 
-The product is the C-ABI shared library ``libclarabel_b200.so`` (CUDA, sm_100a;
+The product is the C-ABI shared library ``libclarabel_b200.so`` (CUDA, sm_90a;
 see ``include/clarabel_b200.h``).  This module is the thin ctypes binding used
 by the tests and the bench; it mirrors the reference's plugin interface names:
 

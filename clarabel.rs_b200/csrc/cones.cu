@@ -1,4 +1,4 @@
-// Device cone kernels (sm_100a).  See cones.h.
+// Device cone kernels (sm_90a).  See cones.h.
 //
 // Per-function reference map (all under /root/reference/src/solver/core/cones):
 //   Nonnegative  nonnegativecone.rs:58-166, 177-195

@@ -1,4 +1,4 @@
-// Exponential and 3-D power cone kernels (sm_100a): one thread per cone.  See cones_nonsym.cuh for the per-cone
+// Exponential and 3-D power cone kernels (sm_90a): one thread per cone.  See cones_nonsym.cuh for the per-cone
 // arithmetic and the reference map, cones.h for the cone engine these methods belong to.
 //
 // Layout: cone k of the nns nonsymmetric cones owns rows off[id]..off[id]+2 of the m-vectors and entries

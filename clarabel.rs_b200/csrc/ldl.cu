@@ -1,4 +1,4 @@
-// Device multifrontal LDL^T for quasidefinite KKT matrices (sm_100a) + the
+// Device multifrontal LDL^T for quasidefinite KKT matrices (sm_90a) + the
 // cldl_* C-ABI (include/clarabel_b200.h).
 //
 // What it replaces in the reference (all file:line under /root/reference):
@@ -1185,10 +1185,10 @@ __device__ void dff_tile(const LDLDev& d, const DFFactor& q, const int* tk, doub
       for (int j = 0; j < 4; j++) acc[i][j] += a[i] * b[j];
   }
 #else
-  // The 64 x 64 x ns product L21_I (D L21_J)^T on the FP64 tensor path: mma.sync.aligned.m8n8k4 (SASS DMMA) -- the
-  // only FP64 MMA sm_100a has (tcgen05 has no FP64 kind).  On C5 these tiles ARE the dense Schur blocks of the PSD
+  // The 64 x 64 x ns product L21_I (D L21_J)^T on the FP64 tensor path: mma.sync.aligned.m8n8k4 (SASS DMMA) -- FP64
+  // MMA on sm_90a is mma.sync only (wgmma has no FP64 kind).  On C5 these tiles ARE the dense Schur blocks of the PSD
   // cones' Hs blocks (the north star's "tensor cores only for the dense Schur blocks arising from SDP cones").
-  // scripts/ubench/dmma_tile.cu: 24.5 TFLOP/s against 12.4 for the 4 x 4 FMA register tile on this tile shape.
+  // scripts/ubench/dmma_tile.cu compares it with the 4 x 4 FMA register tile on this tile shape.
   // Warp w owns rows 32 (w & 1) .., columns 16 (w >> 1) .. as 4 x 2 fragments of 8 x 8; the extend-add above and the store
   // below use the same ownership, so the product never leaves the registers.
   double c2[4][2][2];
@@ -1707,7 +1707,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     int nsm = 0;
     CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
     // resident CTAs per SM and the slab size that goes with it (227 KB of shared memory per SM, 1 KB reserved per CTA)
-    solve_minb = 3;      // C4 on a B200: 2 / 3 / 4 resident CTAs -> see profiles/ (r02 tuning)
+    solve_minb = 3;      // C4 on an H100 (700 W): 25.4 it/s against 25.0 with 2 and 25.1 with 4 resident CTAs
     if (const char* e = std::getenv("CB_SOLVE_MINB")) solve_minb = std::min(4, std::max(2, std::atoi(e)));
     const size_t extra2 = (size_t)2 * (2 * CB_PB_MAXNS + SV_MAXROWS + 4 * CB_PB_MAXNS) * sizeof(double);   // NR = 2 vectors
     {

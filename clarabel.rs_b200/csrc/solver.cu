@@ -1,4 +1,4 @@
-// Device-resident KKT solver and interior-point driver (sm_100a) + ckkt_* /
+// Device-resident KKT solver and interior-point driver (sm_90a) + ckkt_* /
 // ccone_* / cipm_* C-ABI (include/clarabel_b200.h).
 //
 // What it replaces in the reference (all file:line under /root/reference/src):

@@ -32,7 +32,9 @@ inline void cb_tmark(const char* label) {
 // number of kernels launched by this library (bench.py reports it as gpu_launches)
 extern std::atomic<unsigned long long> g_launches;   // bumped from several host threads (per-rank threads, helper threads)
 
-constexpr int RED_BLOCKS = 296;   // 2 x 148 SMs
+// Fixed, not derived from the SM count: the reduction order, and with it every result bit, is then the same on any
+// GPU.  On the 132 SMs of an H100 all 296 blocks of 256 threads are resident at once (up to 8 per SM).
+constexpr int RED_BLOCKS = 296;
 constexpr int RED_THREADS = 256;
 
 struct ReduceWS {

@@ -1,5 +1,5 @@
 /*
- * clarabel_b200.h -- C-ABI of the B200-native KKT backend for Clarabel-style
+ * clarabel_b200.h -- C-ABI of the GPU-native (H100, sm_90a) KKT backend for Clarabel-style
  * interior point solvers.  Plain pointers and sizes only; no C++/torch types.
  *
  * LEVEL 1  (cldl_*)  replaces the reference's `DirectLDLSolver` plugin trait

@@ -26,13 +26,15 @@ def build_flags():
 
 def _native_path():
     """ORACLE_NATIVE=1 (set by bench.py's CPU legs): compile the port for THIS host, `gcc -O3 -march=native`
-    (BASELINE.md section 3), into oracle/_native/ (git-ignored).  The portable library stays the fallback: a library
-    built with -march=native on one machine may not run on another, so it is never shipped."""
+    (BASELINE.md section 3), into a per-user directory under the system's temporary directory: the source tree may be
+    read-only.  The portable library stays the fallback: a library built with -march=native on one machine may not run
+    on another, so it is never shipped."""
     import subprocess
     import glob
+    import tempfile
     if os.environ.get("ORACLE_NATIVE", "0") != "1":
         return None
-    out_dir = os.path.join(_HERE, "_native")
+    out_dir = os.path.join(tempfile.gettempdir(), "clarabel_oracle_native_%d" % os.getuid())
     out = os.path.join(out_dir, "liboracle_native.so")
     srcs = sorted(glob.glob(os.path.join(_HERE, "*.c")))
     deps = srcs + sorted(glob.glob(os.path.join(_HERE, "*.h")))
@@ -58,7 +60,7 @@ def lib():
         native = _native_path()
         if native is not None:
             path = native
-            _build = "-O3 -march=native, compiled on this host (oracle/_native/)"
+            _build = "-O3 -march=native, compiled on this host (%s)" % native
         if not os.path.exists(path):
             raise RuntimeError("oracle/liboracle.so missing: run `make` (or __graft_entry__.build())")
         L = C.CDLL(path)

@@ -1,6 +1,6 @@
 """Task timeline of the dataflow factorisation (k_factor_df) on a C2-like KKT.
 
-Usage (GPU box): CB_DF_TRACE=/tmp/t.bin python scripts/df_trace.py 100000 200000 200 [out.txt]
+Usage (on the GPU): CB_DF_TRACE=/tmp/t.bin python scripts/df_trace.py 100000 200000 200 [out.txt]
 Prints per-task-kind busy/wait totals, SM utilisation over time and the D/R/T stages along the path that
 finishes last (the critical chain to the root)."""
 import os, sys, struct

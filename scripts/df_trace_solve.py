@@ -1,5 +1,5 @@
 """Task timeline of the dataflow triangular solves (k_solve2, ldl_solve.cuh) on the KKT matrix of a workload.
-Usage (GPU box): python scripts/df_trace_solve.py c2|c4"""
+Usage (on the GPU): python scripts/df_trace_solve.py c2|c4"""
 import os, sys, struct
 import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

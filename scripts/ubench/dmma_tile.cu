@@ -1,10 +1,10 @@
 // TC row of the north star ("tensor cores only for the dense Schur blocks arising from SDP cones"): is the FP64 tensor
-// path (mma.sync.aligned.m8n8k4.f64 -- the only FP64 MMA sm_100a has; tcgen05 has no FP64 kind) worth building for
+// path (mma.sync.aligned.m8n8k4.f64, SASS DMMA -- FP64 MMA on sm_90a is mma.sync only; wgmma has no FP64 kind) worth building for
 // the 64 x 64 x 64 tile products of the refactorisation (k_factor_df T tasks) and the skron blocks of the PSD cone?
 // Both variants compute C(64x64) -= A(64x64) * B(64x64)^T per CTA from shared memory, `iters` times, 256 threads:
 //   fma  : 4 x 4 register tile per thread (what k_factor_df does)
 //   dmma : 8 warps, each owns a 32 x 16 piece of C as 4 x 2 mma tiles of 8 x 8, k in steps of 4
-// Prints GFLOP/s over the whole chip (grid = 2 CTAs per SM).   nvcc -O3 -gencode arch=compute_100a,code=sm_100a
+// Prints GFLOP/s over the whole chip (grid = 2 CTAs per SM).   nvcc -O3 -gencode arch=compute_90a,code=sm_90a
 #include <cstdio>
 #include <cuda_runtime.h>
 #define TS 64

@@ -84,13 +84,15 @@ int main() {
            (double)cyc[0] / iters, (double)cyc[1] / iters, (double)cyc[2] / iters, (double)cyc[3] / iters, (double)cyc[4] / iters, (double)cyc[5] / iters, (double)cyc[6] / iters);
   }
   cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b);
+  int nsm = 0;
+  cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, 0);
   for (int per : {1, 2, 4}) {
-    k_tput<<<148 * per, 256>>>(out, 1000);
+    k_tput<<<nsm * per, 256>>>(out, 1000);
     cudaEventRecord(a);
-    k_tput<<<148 * per, 256>>>(out, 20000);
+    k_tput<<<nsm * per, 256>>>(out, 20000);
     cudaEventRecord(b); cudaEventSynchronize(b);
     float ms; cudaEventElapsedTime(&ms, a, b);
-    double fma_total = 148.0 * per * 256 * 8 * 20000;
+    double fma_total = (double)nsm * per * 256 * 8 * 20000;
     printf("FP64 throughput, %d CTAs/SM x 256 thr: %.1f GFMA/s = %.2f TFLOP/s\n", per, fma_total / ms / 1e6, 2 * fma_total / ms / 1e9);
   }
   return 0;

@@ -1,5 +1,5 @@
 // Micro-benchmark: aggregate load bandwidth of 8-byte loads by flavour (plain / ld.global.cg / volatile),
-// L2-resident (32 MB) and HBM-resident (1 GB) buffers, 296 CTAs x 256 threads, 32 loads in flight per thread.
+// L2-resident (32 MB) and HBM-resident (1 GB) buffers, 296 CTAs x 256 threads (2-3 per SM), 32 loads in flight per thread.
 #include <cstdio>
 #include <cuda_runtime.h>
 template <int MODE>

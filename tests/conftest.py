@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
     if os.environ.get("CLARABEL_EMU") == "1":
         # test_emu_cpu.py re-runs GPU test modules in a subprocess against the CUDA-on-CPU emulated build of the cone /
         # KKT / IPM layer (tests/emu/cuda_emu.h).  Test-side switch only: the product loader is not involved.

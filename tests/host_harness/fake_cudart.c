@@ -114,7 +114,7 @@ cudaError_t cudaFuncSetAttribute(const void *f, int a, int v) { (void)f; (void)a
 cudaError_t cudaDeviceGetAttribute(int *v, int attr, int dev)
 {
     (void)dev;
-    *v = attr == 97 ? 232448 /* max opt-in shared memory per block (B200) */ : attr == 16 ? 148 /* SMs */ : 0;
+    *v = attr == 97 ? 232448 /* max opt-in shared memory per block (H100) */ : attr == 16 ? 132 /* SMs */ : 0;
     return 0;
 }
 cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessorWithFlags(int *n, const void *f, int bs, size_t sm, unsigned fl)

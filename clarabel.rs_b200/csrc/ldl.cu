@@ -8,14 +8,16 @@
 //   adapter           src/solver/core/kktsolvers/direct/quasidef/ldlsolvers/qdldl.rs
 //
 // Design (see DESIGN.md): host symbolic analysis builds a supernodal assembly
-// tree; every tree level is a batch of independent dense fronts.  A front's
-// panel ((ns+nr) x ns, column major) lives in the compact factor storage, its
-// update matrix (nr x nr) in a lifetime-managed arena.  Per level: assemble
-// (original entries + children's update matrices through relative indices),
-// dense LDL^T of the pivot block with the reference's sign-aware dynamic
-// regularisation rule (qdldl.rs:645-651) applied pivot by pivot in elimination
-// order, panel scaling, Schur update.  No atomics on floating point data:
-// every sum has a fixed order, so refactor/solve are bit-reproducible run to run.
+// tree of dense fronts.  A front's panel ((ns+nr) x ns, column major) lives in
+// the compact factor storage, its update matrix (nr x nr) in a lifetime-managed
+// arena.  Tree level 0 (leaves, no dependencies) is factored by plain launches
+// (k_factor_leaf1, k_factor_level), everything above it by one persistent
+// dataflow kernel (k_factor_df).  Per front: assemble (original entries +
+// children's update matrices through relative indices), dense LDL^T of the
+// pivot block with the reference's sign-aware dynamic regularisation rule
+// (qdldl.rs:645-651) applied pivot by pivot in elimination order, panel
+// scaling, Schur update.  No atomics on floating point data: every sum has a
+// fixed order, so refactor/solve are bit-reproducible run to run.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 
@@ -218,327 +220,6 @@ __global__ void __launch_bounds__(256) k_factor_leaf1(LDLDev d, int task_base, i
   }
 }
 
-// ------------------------------------------------------------------------
-// Big fronts: two kernels per level.
-//   k_panel_big   : one CTA per front.  Assembles the ns panel columns (original
-//                   entries + the children's update-matrix columns that fall inside
-//                   the pivot block), factors the ns x ns pivot block in shared
-//                   memory (same pivot-by-pivot regularisation rule), then solves
-//                   the nr rows below it (one thread per row, rows independent).
-//   k_update_tiles: one CTA per 64x64 tile of the front's update matrix:
-//                   U_tile = sum_children extend-add  -  L21_I * D * L21_J^T
-//                   with 4x4 register tiles; the extend-add is fused, so U is
-//                   written exactly once and never zero-filled.
-// ------------------------------------------------------------------------
-#define PB_NT 256
-#define TS 64
-#define KC 32   /* pivots staged per chunk by k_update_tiles */
-
-__device__ __forceinline__ int lower_bound_dev(const int* __restrict__ a, int n, int key) {
-  int lo = 0, hi = n;
-  while (lo < hi) { int mid = (lo + hi) >> 1; if (a[mid] < key) lo = mid + 1; else hi = mid; }
-  return lo;
-}
-
-// Ordered compaction of the children of front s that satisfy `pred`: every thread
-// evaluates up to one child per round; the surviving child ids are appended to
-// s_list in child_list order (so sums keep a fixed order).  Returns the count.
-template <class Pred>
-__device__ __forceinline__ int compact_children(const LDLDev& d, int s, int* s_list, int cap, int* s_wcnt, Pred pred) {
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarp = blockDim.x >> 5;
-  const long long c0 = d.child_ptr[s], c1 = d.child_ptr[s + 1];
-  int total = 0;
-  for (long long base = c0; base < c1; base += blockDim.x) {
-    const long long ci = base + tid;
-    int c = -1;
-    bool ok = false;
-    if (ci < c1) { c = d.child_list[ci]; ok = pred(c); }
-    const unsigned bal = __ballot_sync(0xffffffffu, ok);
-    if (lane == 0) s_wcnt[warp] = __popc(bal);
-    __syncthreads();
-    int off = total;
-    for (int w = 0; w < warp; w++) off += s_wcnt[w];
-    int add = 0;
-    for (int w = 0; w < nwarp; w++) add += s_wcnt[w];
-    if (ok) {
-      const int p = off + __popc(bal & ((1u << lane) - 1u));
-      if (p < cap) s_list[p] = c;
-    }
-    total += add;
-    __syncthreads();
-  }
-  return total;
-}
-
-// Adds U-arena values into `dst_base` through a (src,dst) entry list sorted by dst.  Every thread takes a
-// contiguous slice; slice borders are moved forward to the next change of dst so that one destination is
-// only ever touched by one thread, in list order (deterministic, no atomics, no barriers).
-__device__ __forceinline__ void apply_sorted_entries(double* __restrict__ dst_base, const double* __restrict__ U,
-                                                     const int* __restrict__ esrc, const int* __restrict__ edst,
-                                                     int e0, int e1, int nthreads) {
-  const int cnt = e1 - e0;
-  if (cnt <= 0) return;
-  const int per = (cnt + nthreads - 1) / nthreads;
-  int b = e0 + threadIdx.x * per, e = min(e1, b + per);
-  if (b >= e1) return;
-  if (b > e0) { while (b < e1 && edst[b] == edst[b - 1]) b++; }
-  if (e < e1) { while (e < e1 && edst[e] == edst[e - 1]) e++; }
-  int i = b;
-  while (i < e) {
-    const int dd = edst[i];
-    double acc = 0.0;
-    while (i < e && edst[i] == dd) { acc += U[esrc[i]]; i++; }
-    dst_base[dd] += acc;
-  }
-}
-
-#define CB_CHILD_CAP 1024
-
-__global__ void __launch_bounds__(PB_NT) k_panel_big(LDLDev d, const int* __restrict__ tasks, int task_off) {
-  __shared__ __align__(16) double sA[CB_PB_MAXNS * CB_PB_LD];   // pivot block, column major, padded
-  __shared__ double sDinv[CB_PB_MAXNS], sDval[CB_PB_MAXNS], sSign[CB_PB_MAXNS];
-  __shared__ double s_inv;
-  __shared__ int s_list[CB_CHILD_CAP];
-  __shared__ int s_wcnt[PB_NT / 32];
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarp = PB_NT >> 5;
-  const int s = tasks[blockIdx.x];
-  const int f = d.sn_first[s];
-  const int ns = d.sn_first[s + 1] - f;
-  const long long rp = d.sn_rowptr[s];
-  const int nr = (int)(d.sn_rowptr[s + 1] - rp);
-  const int ld = ns + nr;
-  double* __restrict__ P = d.L + d.panel_off[s];
-  const long long psz = (long long)ld * ns;
-
-  for (long long i = tid; i < psz; i += PB_NT) P[i] = 0.0;
-  if (tid < ns) sSign[tid] = (double)d.dsigns[f + tid];
-  const int ncontrib = compact_children(d, s, s_list, CB_CHILD_CAP, s_wcnt, [&](int c) { return d.child_nb[c] > 0 && !d.child_small[c]; });
-  __syncthreads();
-  for (long long e = d.asm_ptr[s] + tid; e < d.asm_ptr[s + 1]; e += PB_NT) P[d.asm_dst[e]] = d.vals[d.asm_src[e]];
-  __syncthreads();
-  const bool overflow = ncontrib > CB_CHILD_CAP;
-  const int nloop = overflow ? (int)(d.child_ptr[s + 1] - d.child_ptr[s]) : ncontrib;
-  for (int q = 0; q < nloop; q++) {
-    const int c = overflow ? d.child_list[d.child_ptr[s] + q] : s_list[q];
-    const int nb = d.child_nb[c];   // child columns landing inside the pivot block (host precomputed)
-    if (nb == 0 || d.child_small[c]) continue;
-    const long long crp = d.sn_rowptr[c];
-    const int nrc = (int)(d.sn_rowptr[c + 1] - crp);
-    const double* __restrict__ Uc = d.U + d.upd_off[c];
-    const int* __restrict__ relc = d.rel + crp;
-    for (int b = warp; b < nb; b += nwarp) {
-      double* __restrict__ col = P + (long long)relc[b] * ld;
-      const double* __restrict__ ucol = Uc + (long long)b * nrc;
-      // destinations inside one child column are distinct: batch the read-modify-writes so that
-      // 8 independent global round trips are in flight per lane
-      int a = b + lane;
-      for (; a + 7 * 32 < nrc; a += 8 * 32) {
-        int r[8];
-        double u[8], pv[8];
-#pragma unroll
-        for (int q = 0; q < 8; q++) { r[q] = relc[a + q * 32]; u[q] = ucol[a + q * 32]; }
-#pragma unroll
-        for (int q = 0; q < 8; q++) pv[q] = col[r[q]];
-        asm volatile("" ::: "memory");
-#pragma unroll
-        for (int q = 0; q < 8; q++) col[r[q]] = pv[q] + u[q];
-      }
-      for (; a < nrc; a += 32) col[relc[a]] += ucol[a];
-    }
-    __syncthreads();
-  }
-  // all small children at once (sorted entry list, conflict free)
-  apply_sorted_entries(P, d.U, d.sc_panel_src, d.sc_panel_dst, d.sc_panel_ptr[blockIdx.x + task_off],
-                       d.sc_panel_ptr[blockIdx.x + task_off + 1], PB_NT);
-  __syncthreads();
-  // pivot block -> shared
-  for (int idx = tid; idx < ns * ns; idx += PB_NT) {
-    const int j = idx / ns, i = idx - j * ns;
-    sA[j * CB_PB_LD + i] = P[(long long)j * ld + i];
-  }
-  __syncthreads();
-  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0;   // thread 0 only
-  for (int j = 0; j < ns; j++) {
-    if (tid == 0) {
-      double dj = sA[j * CB_PB_LD + j];
-      if (d.reg_enable) {
-        const double sg = sSign[j];
-        if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; c_reg++; }
-      }
-      if (dj == 0.0) c_zero = 1;
-      if (dj > 0.0) c_pos++;
-      const double inv = 1.0 / dj;
-      if (!isfinite(inv)) c_nonf = 1;
-      sDval[j] = dj;
-      sA[j * CB_PB_LD + j] = dj;
-      sDinv[j] = inv;
-      s_inv = inv;
-    }
-    __syncthreads();
-    const double inv = s_inv;
-    const double* cj = sA + j * CB_PB_LD;
-    for (int k = j + 1 + warp; k < ns; k += nwarp) {
-      const double wk = cj[k] * inv;
-      double* ck = sA + k * CB_PB_LD;
-      for (int i = k + lane; i < ns; i += 32) ck[i] -= cj[i] * wk;
-    }
-    __syncthreads();
-    for (int i = j + 1 + tid; i < ns; i += PB_NT) sA[j * CB_PB_LD + i] *= inv;
-    // column j is final; the next pivot only reads column j+1
-  }
-  __syncthreads();
-  if (tid == 0) {
-    if (c_reg) atomicAdd(&d.status[ST_REGCOUNT], c_reg);
-    if (c_pos) atomicAdd(&d.status[ST_POSINERTIA], c_pos);
-    if (c_zero) atomicExch(&d.status[ST_ZEROPIV], 1);
-    if (c_nonf) atomicExch(&d.status[ST_NONFINITE], 1);
-  }
-  if (tid < ns) { d.D[f + tid] = sDval[tid]; d.Dinv[f + tid] = sDinv[tid]; }
-  // write the unit-lower pivot block back
-  for (int idx = tid; idx < ns * ns; idx += PB_NT) {
-    const int j = idx / ns, i = idx - j * ns;
-    if (i >= j) P[(long long)j * ld + i] = sA[j * CB_PB_LD + i];
-  }
-  // rows below:  W L11^T = F21,  L21 = W D^-1.  One thread per row, 16 columns at a time in
-  // registers; W of earlier column blocks is re-read from the panel (L21 * D), coalesced.
-  constexpr int JB = 16;
-  for (int r0 = 0; r0 < nr; r0 += PB_NT) {
-    const int r = r0 + tid;
-    if (r >= nr) continue;
-    double* __restrict__ prow = P + ns + r;
-    for (int jb = 0; jb < ns; jb += JB) {
-      const int nj = min(JB, ns - jb);
-      double t[JB];
-#pragma unroll
-      for (int jj = 0; jj < JB; jj++) t[jj] = jj < nj ? prow[(long long)(jb + jj) * ld] : 0.0;
-      for (int kb = 0; kb < jb; kb += JB) {
-        double wv[JB];
-#pragma unroll
-        for (int kk = 0; kk < JB; kk++) wv[kk] = prow[(long long)(kb + kk) * ld];   // 16 loads in flight
-#pragma unroll
-        for (int kk = 0; kk < JB; kk++) {
-          const double wk = wv[kk] * sDval[kb + kk];
-          const double2* lk2 = reinterpret_cast<const double2*>(sA + (kb + kk) * CB_PB_LD + jb);   // L11[jb+jj][k]
-#pragma unroll
-          for (int j2 = 0; j2 < JB / 2; j2++) {
-            const double2 l = lk2[j2];
-            t[2 * j2] -= wk * l.x;
-            t[2 * j2 + 1] -= wk * l.y;
-          }
-        }
-      }
-#pragma unroll
-      for (int jj = 0; jj < JB; jj++) {
-        if (jj < nj) {
-          const double* lk = sA + (jb + jj) * CB_PB_LD + jb;   // column jb+jj: rows jb+jj+1.. hold L11[.][jb+jj]
-#pragma unroll
-          for (int j2 = jj + 1; j2 < JB; j2++) t[j2] -= t[jj] * lk[j2];
-        }
-      }
-#pragma unroll
-      for (int jj = 0; jj < JB; jj++) if (jj < nj) prow[(long long)(jb + jj) * ld] = t[jj] * sDinv[jb + jj];
-    }
-  }
-}
-
-// tile descriptor: x = task, y = tile row, z = tile column (ti >= tj)
-__global__ void __launch_bounds__(256) k_update_tiles(LDLDev d, const int4* __restrict__ tiles, int tile_off) {
-  extern __shared__ double sm[];
-  double* sAt = sm;                 // [KC][TS]   L21 rows of tile-row I   (KC pivots at a time)
-  double* sBt = sm + KC * TS;        // [KC][TS]   L21 rows of tile-row J scaled by D
-  double* sC = sm + 2 * KC * TS;     // [TS][TS+1] children's contributions
-  const int4 td = tiles[blockIdx.x];
-  const int s = td.x, ti = td.y, tj = td.z;
-  const int tid = threadIdx.x;
-  const int f = d.sn_first[s];
-  const int ns = d.sn_first[s + 1] - f;
-  const long long rp = d.sn_rowptr[s];
-  const int nr = (int)(d.sn_rowptr[s + 1] - rp);
-  const int ld = ns + nr;
-  const double* __restrict__ P = d.L + d.panel_off[s];
-  double* __restrict__ U = d.U + d.upd_off[s];
-  const int i0 = ti * TS, j0 = tj * TS;
-  const int ni = min(TS, nr - i0), nj = min(TS, nr - j0);
-
-  for (int idx = tid; idx < TS * (TS + 1); idx += 256) sC[idx] = 0.0;
-  __syncthreads();
-  // extend-add (fixed child order; distinct destinations inside one child).  Only children whose
-  // rows can reach both tile rows are visited.
-  __shared__ int s_list[CB_CHILD_CAP];
-  __shared__ int s_wcnt[8];
-  const int ncontrib = compact_children(d, s, s_list, CB_CHILD_CAP, s_wcnt, [&](int c) {
-    const int2 tr = d.child_trange[c];
-    return !(ti < tr.x || ti > tr.y || tj < tr.x || tj > tr.y) && !d.child_small[c];
-  });
-  const bool overflow = ncontrib > CB_CHILD_CAP;
-  const int nloop = overflow ? (int)(d.child_ptr[s + 1] - d.child_ptr[s]) : ncontrib;
-  for (int q = 0; q < nloop; q++) {
-    const int c = overflow ? d.child_list[d.child_ptr[s] + q] : s_list[q];
-    if (overflow) {
-      const int2 tr = d.child_trange[c];
-      if (ti < tr.x || ti > tr.y || tj < tr.x || tj > tr.y || d.child_small[c]) continue;
-    }
-    const long long crp = d.sn_rowptr[c];
-    const int nrc = (int)(d.sn_rowptr[c + 1] - crp);
-    const int* __restrict__ relc = d.rel + crp;
-    // first child row falling into tile row t is tp[t - tlo] (host precomputed, uniform loads)
-    const int* __restrict__ tp = d.child_tptr + d.child_tptr_off[c];
-    const int tlo = d.child_trange[c].x;
-    const int a0 = tp[ti - tlo], a1 = tp[ti - tlo + 1], b0 = tp[tj - tlo], b1 = tp[tj - tlo + 1];
-    const int na = a1 - a0, nb = b1 - b0;
-    if (na > 0 && nb > 0) {
-      const double* __restrict__ Uc = d.U + d.upd_off[c];
-      for (int idx = tid; idx < na * nb; idx += 256) {
-        const int bb = idx / na, aa = idx - bb * na;
-        const int a = a0 + aa, b = b0 + bb;
-        if (a >= b) sC[(relc[a] - ns - i0) * (TS + 1) + (relc[b] - ns - j0)] += Uc[(long long)b * nrc + a];
-      }
-    }
-    __syncthreads();
-  }
-  // all small children of this tile at once
-  apply_sorted_entries(sC, d.U, d.sc_tile_src, d.sc_tile_dst, d.sc_tile_ptr[blockIdx.x + tile_off],
-                       d.sc_tile_ptr[blockIdx.x + tile_off + 1], 256);
-  // 4x4 register tile per thread
-  const int tx = tid & 15, ty = tid >> 4;
-  double acc[4][4];
-#pragma unroll
-  for (int i = 0; i < 4; i++)
-#pragma unroll
-    for (int j = 0; j < 4; j++) acc[i][j] = 0.0;
-  for (int k0 = 0; k0 < ns; k0 += KC) {
-    const int kc = min(KC, ns - k0);
-    __syncthreads();   // previous chunk fully consumed
-    for (int idx = tid; idx < kc * TS; idx += 256) {
-      const int k = idx / TS, r = idx - k * TS;
-      const long long col = (long long)(k0 + k) * ld + ns;
-      sAt[idx] = (r < ni) ? P[col + i0 + r] : 0.0;
-      sBt[idx] = (r < nj) ? P[col + j0 + r] * d.D[f + k0 + k] : 0.0;
-    }
-    __syncthreads();
-#pragma unroll 4
-    for (int k = 0; k < kc; k++) {
-      double a[4], b[4];
-#pragma unroll
-      for (int i = 0; i < 4; i++) { a[i] = sAt[k * TS + tx + 16 * i]; b[i] = sBt[k * TS + ty + 16 * i]; }
-#pragma unroll
-      for (int i = 0; i < 4; i++)
-#pragma unroll
-        for (int j = 0; j < 4; j++) acc[i][j] += a[i] * b[j];
-    }
-  }
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    const int r = tx + 16 * i;
-#pragma unroll
-    for (int j = 0; j < 4; j++) {
-      const int c = ty + 16 * j;
-      if (r < ni && c < nj && (i0 + r >= j0 + c))
-        U[(long long)(j0 + c) * nr + (i0 + r)] = sC[r * (TS + 1) + c] - acc[i][j];
-    }
-  }
-}
-
 __global__ void k_permute_in(int n, const int* __restrict__ perm, const double* __restrict__ b,
                              double* __restrict__ xp) {
   int k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -552,7 +233,7 @@ __global__ void k_permute_in(int n, const int* __restrict__ perm, const double* 
 // overlap across levels and a level never waits for its slowest front.  A task is one wide front
 // (whole CTA) or a batch of up to 8 narrow fronts (one warp each).  Data that crosses fronts is read
 // with ld.global.cg (L2), written once before its consumers are released (threadfence + atomic).
-// No floating-point atomics: results are bit-identical to the level-synchronous kernels.
+// No floating-point atomics: every sum has a fixed order, so results are bit-identical run to run.
 // ------------------------------------------------------------------------
 __device__ __forceinline__ unsigned long long df_gtime() {
 #ifdef CB_EMU   /* host build of the test suite (tests/emu): no device clock */
@@ -583,10 +264,11 @@ __device__ __forceinline__ void df_wait_set(volatile int* p) {
 //   T  big front: one 64x64 tile of the update matrix (extend-add + Schur update) waits: all R of the front
 // A front is complete when its last tile (or its F task) finishes; that releases its parent.  Data
 // produced by other CTAs inside this kernel is read with ld.global.cg (L1 is not coherent across SMs and
-// the update-matrix arena is recycled along the schedule).  Same arithmetic, same summation orders as the
-// level-synchronous kernels: results are bit-identical.
+// the update-matrix arena is recycled along the schedule).  Every sum has a fixed order, whatever the
+// schedule: results are bit-identical run to run.
 // ------------------------------------------------------------------------
 #define DF_NT 256
+#define TS 64   /* rows and columns of an update-matrix tile (T tasks) */
 #define DF_SMEM_DOUBLES (CB_PB_MAXNS * CB_PB_LD + 2 * CB_PB_MAXNS + CB_PB_MAXNS * 128)   /* 12544 doubles = 98 KB (R task); T needs 12352 */
 
 __device__ __forceinline__ double ldcg_d(const double* p) { return __ldcg(p); }
@@ -1378,11 +1060,9 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   }
 
   CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  if (std::getenv("CB_LEAF_STREAMS") == nullptr || std::atoi(std::getenv("CB_LEAF_STREAMS")) != 0) {
-    CK(cudaStreamCreateWithFlags(&stream_a, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&stream_b, cudaStreamNonBlocking));
-    for (auto& e : ev_leaf) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  }
+  CK(cudaStreamCreateWithFlags(&stream_a, cudaStreamNonBlocking));
+  CK(cudaStreamCreateWithFlags(&stream_b, cudaStreamNonBlocking));
+  for (auto& e : ev_leaf) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
   CK(cudaEventCreate(&ev0));
   CK(cudaEventCreate(&ev1));
   CK(cudaMallocHost((void**)&h_status, ST_COUNT * sizeof(int)));
@@ -1401,7 +1081,6 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   if ((rc = upload(&tmp_l, to_ll(S.asm_ptr)))) return rc; dev.asm_ptr = tmp_l;
   if ((rc = upload(&tmp_i, S.asm_src))) return rc; dev.asm_src = tmp_i;
   if ((rc = upload(&tmp_l, to_ll(S.asm_dst)))) return rc; dev.asm_dst = tmp_l;
-  if ((rc = upload(&tmp_i, S.level_tasks))) return rc; dev.level_tasks = tmp_i;
   if ((rc = upload(&tmp_i, S.perm))) return rc; dev.perm = tmp_i;
   {
     std::vector<signed char> ds(n);
@@ -1439,26 +1118,23 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   dev.reg_delta = o.regularize_delta;
 
   cb_tmark("ldl: uploads + device alloc");
-  // per-child constants for the big-front kernels and the per-destination gather lists for the solves
+  // rows of every child that land in its parent's pivot block (k_factor_df's child records) and the per-destination
+  // gather lists for the solves
   std::vector<int> h_child_nb(S.nsup, 0);
   // (runs on a host thread next to the launch plan and the small-child lists below; it only reads the symbolic
   // structure and writes its own device arrays)
   auto build_child_consts = [&]() -> int {
     int rc = 0;
     if (cudaSetDevice(device) != cudaSuccess) return CLDL_E_CUDA;
-    std::vector<int>& child_nb = h_child_nb;
-    std::vector<int2> child_tr(S.nsup, make_int2(1, 0));
     std::vector<int> gptr((size_t)n + S.sn_rows.size() + 1, 0);
     for (int c = 0; c < S.nsup; c++) {
       const int p = S.sn_parent[c];
       if (p < 0) continue;
       const int pns = S.sn_first[p + 1] - S.sn_first[p];
       const int64_t pbase = (int64_t)S.sn_first[p] + S.sn_rowptr[p];
-      const int64_t b0 = S.sn_rowptr[c], e0 = S.sn_rowptr[c + 1];
       int nb = 0;
-      for (int64_t t = b0; t < e0; t++) { if (S.rel[t] < pns) nb++; gptr[pbase + S.rel[t] + 1]++; }
-      child_nb[c] = nb;
-      if (b0 + nb < e0) child_tr[c] = make_int2((S.rel[b0 + nb] - pns) / TS, (S.rel[e0 - 1] - pns) / TS);
+      for (int64_t t = S.sn_rowptr[c]; t < S.sn_rowptr[c + 1]; t++) { if (S.rel[t] < pns) nb++; gptr[pbase + S.rel[t] + 1]++; }
+      h_child_nb[c] = nb;
     }
     for (size_t i = 0; i + 1 < gptr.size(); i++) gptr[i + 1] += gptr[i];
     std::vector<int> gsrc(S.sn_rows.size() ? S.sn_rows.size() : 1, 0), pos(gptr.begin(), gptr.end() - 1);
@@ -1470,121 +1146,72 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
         for (int64_t t = S.sn_rowptr[c]; t < S.sn_rowptr[c + 1]; t++) gsrc[pos[pbase + S.rel[t]]++] = (int)t;
       }
     }
-    std::vector<int> tptr_off(S.nsup + 1, 0), tptr;
-    for (int c = 0; c < S.nsup; c++) {
-      tptr_off[c] = (int)tptr.size();
-      const int p = S.sn_parent[c];
-      if (p < 0 || child_tr[c].x > child_tr[c].y) continue;
-      const int pns = S.sn_first[p + 1] - S.sn_first[p];
-      const int64_t b0 = S.sn_rowptr[c], e0 = S.sn_rowptr[c + 1];
-      int64_t t = b0 + child_nb[c];
-      for (int tile = child_tr[c].x; tile <= child_tr[c].y + 1; tile++) {
-        while (t < e0 && S.rel[t] < pns + tile * TS) t++;
-        tptr.push_back((int)(t - b0));
-      }
-    }
-    tptr_off[S.nsup] = (int)tptr.size();
     int* t1 = nullptr;
-    if ((rc = upload(&t1, tptr_off))) return rc; dev.child_tptr_off = t1;
-    if ((rc = upload(&t1, tptr))) return rc; dev.child_tptr = t1;
-    if ((rc = upload(&t1, child_nb))) return rc; dev.child_nb = t1;
     if ((rc = upload(&t1, gptr))) return rc; dev.gat_ptr = t1;
     if ((rc = upload(&t1, gsrc))) return rc; dev.gat_src = t1;
-    int2* t2 = nullptr;
-    CK(cudaMalloc((void**)&t2, (size_t)(S.nsup ? S.nsup : 1) * sizeof(int2)));
-    CK(cudaMemcpy(t2, child_tr.data(), (size_t)S.nsup * sizeof(int2), cudaMemcpyHostToDevice));
-    dev.child_trange = t2;
-      return rc;
+    return rc;
   };
   int rc_child = 0;
   std::thread th_child([&]() { rc_child = build_child_consts(); });
   struct ThJoin { std::thread* t; ~ThJoin() { if (t->joinable()) t->join(); } } th_child_guard{&th_child};
   cb_tmark("ldl: child consts + gather lists");
-  // per-level launch plan.  Small fronts: one fused CTA each, grouped by the shared-memory class of
-  // their panel.  Big fronts (nr >= CB_BIG_NR): panel kernel + tiled update kernel.
+  // big fronts (nr >= CB_BIG_NR: k_factor_df's D, R and T tasks) in level order, and the 64x64 tiles of their update
+  // matrices: big_pos / tile_base number them for the small-child entry lists and the factor tasks
+  std::vector<int> big_pos(S.nsup, -1), tile_base(S.nsup, -1);
+  int nbig = 0, ntiles = 0;
+  auto is_big = [&](int s) { return big_pos[s] >= 0; };
+  for (int s : S.level_tasks) {
+    const long long ns = S.sn_first[s + 1] - S.sn_first[s];
+    const long long nr = S.sn_rowptr[s + 1] - S.sn_rowptr[s];
+    if (nr < CB_BIG_NR || ns > CB_PB_MAXNS) continue;
+    const int nt = (int)((nr + TS - 1) / TS);
+    big_pos[s] = nbig++;
+    tile_base[s] = ntiles;
+    ntiles += nt * (nt + 1) / 2;
+  }
+  // launch plan of tree level 0 (leaves: no dependencies, factored by plain launches before k_factor_df).  Single-column
+  // fronts take one thread each (k_factor_leaf1), the others one fused CTA each (k_factor_level), grouped by the
+  // shared-memory class of their panel.  level_tasks is reordered into these groups.
   int max_optin = 0;
   CK(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
   const int cap_big = (max_optin - 2048) / 8;  // doubles
   CK(cudaFuncSetAttribute(k_factor_level<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap_big * 8));
-  const size_t smem_panel = 0;   // static shared memory only
-  const size_t smem_tiles = (size_t)(2 * KC * TS + TS * (TS + 1)) * 8;
-  CK(cudaFuncSetAttribute(k_update_tiles, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_tiles));
   const long long classes[3] = {1024, 5632, cap_big};  // 8 KB, 44 KB, ~225 KB panels
   plan.clear();
-  const bool leaf1_kernel = std::getenv("CB_FACTOR_LEAF1") == nullptr || std::atoi(std::getenv("CB_FACTOR_LEAF1")) != 0;
-  std::vector<int> big_tasks;
-  std::vector<int4> tiles;
-  for (int l = 0; l < S.nlevels; l++) {
-    int b = S.level_ptr[l], e = S.level_ptr[l + 1];
-    std::vector<int> order[4], order1;
-    const size_t big0 = big_tasks.size(), tile0 = tiles.size();
+  if (S.nlevels > 0) {
+    const int b = S.level_ptr[0], e = S.level_ptr[1];
+    std::vector<int> order[4], order1, big;
     std::vector<int> not_mine;       // sharded: fronts of other ranks are parked at the end of the level's range
     for (int t = b; t < e; t++) {
       const int s = S.level_tasks[t];
       const long long ns = S.sn_first[s + 1] - S.sn_first[s];
       const long long nr = S.sn_rowptr[s + 1] - S.sn_rowptr[s];
-      if (!mine(s) && !(nr >= CB_BIG_NR && ns <= CB_PB_MAXNS)) { not_mine.push_back(s); continue; }
-      if (nr >= CB_BIG_NR && ns <= CB_PB_MAXNS) {
-        big_tasks.push_back(s);
-        const int nt = (int)((nr + TS - 1) / TS);
-        for (int ti = 0; ti < nt; ti++)
-          for (int tj = 0; tj <= ti; tj++) tiles.push_back(make_int4(s, ti, tj, 0));
-        continue;
-      }
-      if (l == 0 && ns == 1 && leaf1_kernel) { order1.push_back(s); continue; }
+      if (is_big(s)) { big.push_back(s); continue; }
+      if (!mine(s)) { not_mine.push_back(s); continue; }
+      if (ns == 1) { order1.push_back(s); continue; }
       const long long p = (ns + nr) * ns;
       int c = p <= classes[0] ? 0 : p <= classes[1] ? 1 : p <= classes[2] ? 2 : 3;
       order[c].push_back(s);
     }
     int pos = b;
-    if (!order1.empty()) {      // single-column leaves: one thread each (k_factor_leaf1)
-      LaunchSeg seg;
-      seg.kind = 3; seg.level = l; seg.base = pos; seg.count = (int)order1.size(); seg.smem_doubles = 0; seg.threads = 256;
-      plan.push_back(seg);
+    if (!order1.empty()) {
+      plan.push_back(LaunchSeg{true, pos, (int)order1.size(), 0, 256});
       for (int s : order1) S.level_tasks[pos++] = s;
     }
     for (int c = 3; c >= 0; c--) {
       if (order[c].empty()) continue;
-      LaunchSeg seg;
-      seg.kind = 0;
-      seg.level = l;
-      seg.base = pos;
-      seg.count = (int)order[c].size();
-      seg.smem_doubles = c == 3 ? 0 : (int)classes[c];
-      seg.threads = c == 0 ? 64 : 256;
-      plan.push_back(seg);
+      plan.push_back(LaunchSeg{false, pos, (int)order[c].size(), c == 3 ? 0 : (int)classes[c], c == 0 ? 64 : 256});
       for (int s : order[c]) S.level_tasks[pos++] = s;
     }
-    for (size_t k = big0; k < big_tasks.size(); k++) S.level_tasks[pos++] = big_tasks[k];
+    for (int s : big) S.level_tasks[pos++] = s;
     for (int s : not_mine) S.level_tasks[pos++] = s;
-    if (big_tasks.size() > big0) {
-      LaunchSeg seg;
-      seg.kind = 1; seg.level = l; seg.base = (int)big0; seg.count = (int)(big_tasks.size() - big0);
-      seg.smem_doubles = (int)(smem_panel / 8); seg.threads = PB_NT;
-      plan.push_back(seg);
-      seg.kind = 2; seg.base = (int)tile0; seg.count = (int)(tiles.size() - tile0);
-      seg.smem_doubles = (int)(smem_tiles / 8); seg.threads = 256;
-      plan.push_back(seg);
-    }
   }
-  {
-    int* t1 = nullptr;
-    if ((rc = upload(&t1, big_tasks))) return rc;
-    d_big_tasks = t1;
-    int4* t4 = nullptr;
-    CK(cudaMalloc((void**)&t4, (tiles.size() ? tiles.size() : 1) * sizeof(int4)));
-    if (!tiles.empty()) CK(cudaMemcpy(t4, tiles.data(), tiles.size() * sizeof(int4), cudaMemcpyHostToDevice));
-    d_tiles = t4;
-    n_tiles = (int64_t)tiles.size();
-  }
-  cb_tmark("ldl: launch plan + tiles");
+  if ((rc = upload(&tmp_i, S.level_tasks))) return rc; dev.level_tasks = tmp_i;
+  cb_tmark("ldl: launch plan");
   // small children (nr <= CB_SMALL_CHILD) of big fronts: one dst-sorted (src,dst) list per panel and per tile
   std::vector<signed char> small_child;
   std::vector<int> h_sc_panel_ptr, h_sc_tile_ptr;
   {
-    std::vector<int> big_pos(S.nsup, -1), tile_base(S.nsup, -1);
-    for (size_t k = 0; k < big_tasks.size(); k++) big_pos[big_tasks[k]] = (int)k;
-    for (size_t k = 0; k < tiles.size(); k++) if (tile_base[tiles[k].x] < 0) tile_base[tiles[k].x] = (int)k;
     std::vector<signed char>& small = small_child;
     small.assign(S.nsup, 0);
     struct Ent { int key; int dst; int src; };
@@ -1678,21 +1305,17 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     std::vector<int> ptr, src, dst, tptr, tsrc, tdst;
     int* t1 = nullptr;
     {
-      std::thread tb([&]() { build(te, tiles.size(), tptr, tsrc, tdst); });
-      build(pe, big_tasks.size(), ptr, src, dst);
+      std::thread tb([&]() { build(te, ntiles, tptr, tsrc, tdst); });
+      build(pe, nbig, ptr, src, dst);
       tb.join();
     }
     cb_tmark("ldl:   small-child: panel + tile lists");
     h_sc_panel_ptr = ptr;
-    if ((rc = upload(&t1, ptr))) return rc; dev.sc_panel_ptr = t1;
     if ((rc = upload(&t1, src))) return rc; dev.sc_panel_src = t1;
     if ((rc = upload(&t1, dst))) return rc; dev.sc_panel_dst = t1;
     h_sc_tile_ptr = tptr;
-    if ((rc = upload(&t1, tptr))) return rc; dev.sc_tile_ptr = t1;
     if ((rc = upload(&t1, tsrc))) return rc; dev.sc_tile_src = t1;
     if ((rc = upload(&t1, tdst))) return rc; dev.sc_tile_dst = t1;
-    signed char* t8 = nullptr;
-    if ((rc = upload(&t8, small))) return rc; dev.child_small = t8;
   }
   th_child.join();
   if (rc_child) return rc_child;
@@ -1700,22 +1323,16 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   // solve plan (ldl_solve.cuh): level-0 narrow fronts get plain kernels, everything else becomes queue tasks in level
   // order -- batches of narrow fronts, and for every wide front a head task (pivot block + first rows) followed by row
   // tasks when the panel exceeds the shared-memory slab.
-  // level_tasks was re-ordered inside levels: re-upload
-  CK(cudaMemcpy((void*)dev.level_tasks, S.level_tasks.data(), S.level_tasks.size() * sizeof(int),
-                cudaMemcpyHostToDevice));
   {
     int nsm = 0;
     CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
-    // resident CTAs per SM and the slab size that goes with it (227 KB of shared memory per SM, 1 KB reserved per CTA)
-    solve_minb = 3;      // C4 on an H100 (700 W): 25.4 it/s against 25.0 with 2 and 25.1 with 4 resident CTAs
-    if (const char* e = std::getenv("CB_SOLVE_MINB")) solve_minb = std::min(4, std::max(2, std::atoi(e)));
+    // the slab size that goes with SV_MINB resident CTAs per SM (227 KB of shared memory per SM, 1 KB reserved per CTA)
     const size_t extra2 = (size_t)2 * (2 * CB_PB_MAXNS + SV_MAXROWS + 4 * CB_PB_MAXNS) * sizeof(double);   // NR = 2 vectors
     {
-      const size_t per_cta = ((size_t)227 * 1024) / solve_minb - 1024 - 64;
+      const size_t per_cta = ((size_t)227 * 1024) / SV_MINB - 1024 - 64;
       sv_cap = (int)((per_cta - extra2) / sizeof(double)) - 2;
       sv_cap &= ~1;
       sv_cap = std::min(sv_cap, 16384);
-      if (const char* e = std::getenv("CB_SOLVE_CAP")) sv_cap = std::max(CB_PB_MAXNS * (CB_PB_MAXNS + 9), std::atoi(e)) & ~1;
     }
     const int cap = sv_cap;
     auto wide = [&](int s) { return S.sn_first[s + 1] - S.sn_first[s] > CB_SOLVE_SMALL_NS; };
@@ -1886,8 +1503,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     if ((rc = sv_configure())) return rc;
     int occ = sv_occupancy();
     if (occ < 1) return CLDL_E_CUDA;
-    df_grid = nsm * occ;
-    if (const char* e = std::getenv("CB_DF_GRID")) df_grid = std::max(1, std::atoi(e));
+    sv_grid = nsm * occ;
     use_dataflow = true;
     if (std::getenv("CB_DF_TRACE_SOLVE") && nt > 0) {
       CK(cudaMalloc((void**)&sv.trace, (size_t)nt * 8 * sizeof(unsigned long long)));
@@ -1895,7 +1511,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
       h_sv_tasks.assign((const int*)tk.data(), (const int*)tk.data() + (size_t)nt * 24);
     }
     if (std::getenv("CB_TIMING") != nullptr) std::fprintf(stderr, "[cb timing]     solve plan: %d tasks (%d leaf columns, %d narrow leaves, %d wide leaves, %d wide fronts, %d row slabs), slab %d doubles, %d CTAs\n",
-                                     nt, sv_nleaf1, sv_nleafn, sv_nleafw, sv_nwide, nslots, cap, df_grid);
+                                     nt, sv_nleaf1, sv_nleafn, sv_nleafw, sv_nwide, nslots, cap, sv_grid);
   }
   cb_tmark("ldl:   solve plan: dataflow solve tasks");
   // dataflow factorisation plan (k_factor_df): level 0's small fronts keep their level-synchronous launch
@@ -1903,16 +1519,12 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   // record carries the front's constants and the range of its child records, so a task starts with two
   // dependent loads (record, child records) instead of walking the tree arrays.
   {
-    std::vector<int> big_pos(S.nsup, -1), tile_base(S.nsup, -1);
-    for (size_t k = 0; k < big_tasks.size(); k++) big_pos[big_tasks[k]] = (int)k;
-    for (size_t k = 0; k < tiles.size(); k++) if (tile_base[tiles[k].x] < 0) tile_base[tiles[k].x] = (int)k;
     std::vector<int> tk;       // 16 ints per task
     std::vector<int> desc;     // 12 ints per child record
     std::vector<int> cnt_init(4 * (size_t)S.nsup, 0);   // [pend | diag_done | rows_left | tiles_left]
     int* pend = cnt_init.data();
     int* rows_left = cnt_init.data() + 2 * (size_t)S.nsup;
     int* tiles_left = cnt_init.data() + 3 * (size_t)S.nsup;
-    auto is_big = [&](int s) { return big_pos[s] >= 0; };
     for (int s = 0; s < S.nsup; s++) {
       const int p = S.sn_parent[s];
       const bool presolved = (S.sn_level[s] == 0 && !is_big(s));
@@ -2049,8 +1661,8 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     }
     }
     cb_tmark("ldl:   solve plan: factor tasks built");
-    if (std::getenv("CB_TIMING")) std::fprintf(stderr, "[cb timing]     factor plan: %zu tasks, %zu child records, %zu big fronts, %zu tiles\n",
-                                                tk.size() / 16, desc.size() / 12, big_tasks.size(), tiles.size());
+    if (std::getenv("CB_TIMING")) std::fprintf(stderr, "[cb timing]     factor plan: %zu tasks, %zu child records, %d big fronts, %d tiles\n",
+                                                tk.size() / 16, desc.size() / 12, nbig, ntiles);
     dff.ntask = (int)(tk.size() / 16);
     if (!sharded()) dff_ntask_owned = dff.ntask;
     int4* t4 = nullptr;
@@ -2073,7 +1685,6 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_factor_df, DF_NT, (size_t)DF_SMEM_DOUBLES * 8));
     dff_grid = nsm * std::max(1, occ);
     dff_nsup4 = 4 * (size_t)S.nsup;
-    factor_dataflow = std::getenv("CB_FACTOR_LEVELSYNC") == nullptr;
     if (std::getenv("CB_DF_TRACE") && dff.ntask > 0) {
       h_dff_tasks = tk;
       CK(cudaMalloc((void**)&dff.trace, (size_t)dff.ntask * 10 * sizeof(unsigned long long)));
@@ -2108,7 +1719,7 @@ void LDLObject::release() {
   fr(dev.rel); fr(dev.panel_off); fr(dev.upd_off); fr(dev.asm_ptr); fr(dev.asm_src);
   fr(dev.asm_dst); fr(dev.level_tasks); fr(dev.perm); fr(dev.dsigns); fr(dev.vals); fr(dev.L);
   fr(dev.U); fr(dev.D); fr(dev.Dinv); fr(dev.u); fr(dev.status); fr(d_xp); fr(d_bx);
-  fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(d_big_tasks); fr(d_tiles); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_wide); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.desc); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.child_nb); fr(dev.child_trange); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.child_tptr); fr(dev.child_tptr_off); fr(dev.sc_panel_ptr); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_ptr); fr(dev.sc_tile_src); fr(dev.sc_tile_dst); fr(dev.child_small);
+  fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_wide); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.desc); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
   if (h_status) cudaFreeHost(h_status);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
@@ -2118,43 +1729,29 @@ void LDLObject::release() {
   if (stream) cudaStreamDestroy(stream);
 }
 
-int LDLObject::refactor_async() {
-  if (sharded()) return has_transport() ? refactor_sharded() : CLDL_E_ARG;   // without a transport: the phase entry points
-  CK(cudaSetDevice(device));
+// the start of every refactor: status, counters and queue head of k_factor_df reset, tree level 0 factored by the
+// plain launches of `plan`
+int LDLObject::refactor_level0() {
   CK(cudaMemsetAsync(dev.status, 0, ST_COUNT * sizeof(int), stream));
-  if (factor_dataflow) {
-    CK(cudaMemcpyAsync(d_dff_cnt, d_dff_init, dff_nsup4 * sizeof(int), cudaMemcpyDeviceToDevice, stream));
-    CK(cudaMemsetAsync(dff.qhead, 0, sizeof(int), stream));
-    for (const LaunchSeg& g : plan) {
-      if (g.level != 0 || (g.kind != 0 && g.kind != 3)) continue;
-      g_launches++;
-      if (g.kind == 3) k_factor_leaf1<<<(g.count + 255) / 256, 256, 0, stream>>>(dev, g.base, g.count);
-      else if (g.threads == 64)
-        k_factor_level<64><<<g.count, 64, (size_t)g.smem_doubles * 8, stream>>>(dev, g.base, g.smem_doubles);
-      else
-        k_factor_level<256><<<g.count, 256, (size_t)g.smem_doubles * 8, stream>>>(dev, g.base, g.smem_doubles);
-    }
-    g_launches++;
-    k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, dff);
-    invert_pivots();
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(h_status, dev.status, ST_COUNT * sizeof(int), cudaMemcpyDeviceToHost, stream));
-    factored = true;
-    return CLDL_OK;
-  }
+  CK(cudaMemcpyAsync(d_dff_cnt, d_dff_init, dff_nsup4 * sizeof(int), cudaMemcpyDeviceToDevice, stream));
+  CK(cudaMemsetAsync(dff.qhead, 0, sizeof(int), stream));
   g_launches += plan.size();
   for (const LaunchSeg& g : plan) {
-    if (g.kind == 3)
-      k_factor_leaf1<<<(g.count + 255) / 256, 256, 0, stream>>>(dev, g.base, g.count);
-    else if (g.kind == 1)
-      k_panel_big<<<g.count, PB_NT, (size_t)g.smem_doubles * 8, stream>>>(dev, d_big_tasks + g.base, g.base);
-    else if (g.kind == 2)
-      k_update_tiles<<<g.count, 256, (size_t)g.smem_doubles * 8, stream>>>(dev, d_tiles + g.base, g.base);
+    if (g.leaf1) k_factor_leaf1<<<(g.count + 255) / 256, 256, 0, stream>>>(dev, g.base, g.count);
     else if (g.threads == 64)
       k_factor_level<64><<<g.count, 64, (size_t)g.smem_doubles * 8, stream>>>(dev, g.base, g.smem_doubles);
     else
       k_factor_level<256><<<g.count, 256, (size_t)g.smem_doubles * 8, stream>>>(dev, g.base, g.smem_doubles);
   }
+  return CLDL_OK;
+}
+
+int LDLObject::refactor_async() {
+  if (sharded()) return has_transport() ? refactor_sharded() : CLDL_E_ARG;   // without a transport: the phase entry points
+  CK(cudaSetDevice(device));
+  if (int rc = refactor_level0()) return rc;
+  g_launches++;
+  k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, dff);
   invert_pivots();
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h_status, dev.status, ST_COUNT * sizeof(int), cudaMemcpyDeviceToHost, stream));
@@ -2178,7 +1775,7 @@ int LDLObject::sync_status() {
   CK(cudaStreamSynchronize(stream));
   regularize_count = (uint64_t)h_status[ST_REGCOUNT];
   positive_inertia = (uint64_t)h_status[ST_POSINERTIA];
-  if (dff.trace && factor_dataflow) {  // diagnostic: CB_DF_TRACE=<file> dumps the last refactor's task timeline
+  if (dff.trace) {  // diagnostic: CB_DF_TRACE=<file> dumps the last refactor's task timeline
     std::vector<unsigned long long> tr((size_t)dff.ntask * 10);
     CK(cudaMemcpy(tr.data(), dff.trace, tr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     if (FILE* fp = std::fopen(std::getenv("CB_DF_TRACE"), "wb")) {
@@ -2193,56 +1790,35 @@ int LDLObject::sync_status() {
   return h_status[ST_NONFINITE] ? 0 : 1;
 }
 
-// opt-in to the dynamic shared memory of the sweep kernels (every instantiation that can be launched)
-template <bool FWD, int NR, int MINB>
-static cudaError_t sv_attr(size_t bytes) {
-  return cudaFuncSetAttribute(k_solve2<FWD, NR, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-}
+// opt-in to the dynamic shared memory of the sweep kernels
 int LDLObject::sv_configure() {
-  for (int nr = 1; nr <= 2; nr++) {
-    const size_t b = sv_smem[nr - 1];
-    cudaError_t e = cudaSuccess;
-    if (solve_minb == 2) { e = nr == 1 ? sv_attr<true, 1, 2>(b) : sv_attr<true, 2, 2>(b); if (e == cudaSuccess) e = nr == 1 ? sv_attr<false, 1, 2>(b) : sv_attr<false, 2, 2>(b); }
-    else if (solve_minb == 3) { e = nr == 1 ? sv_attr<true, 1, 3>(b) : sv_attr<true, 2, 3>(b); if (e == cudaSuccess) e = nr == 1 ? sv_attr<false, 1, 3>(b) : sv_attr<false, 2, 3>(b); }
-    else { e = nr == 1 ? sv_attr<true, 1, 4>(b) : sv_attr<true, 2, 4>(b); if (e == cudaSuccess) e = nr == 1 ? sv_attr<false, 1, 4>(b) : sv_attr<false, 2, 4>(b); }
-    CK(e);
-  }
+  CK(cudaFuncSetAttribute(k_solve2<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem[0]));
+  CK(cudaFuncSetAttribute(k_solve2<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem[0]));
+  CK(cudaFuncSetAttribute(k_solve2<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem[1]));
+  CK(cudaFuncSetAttribute(k_solve2<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sv_smem[1]));
   return CLDL_OK;
 }
 int LDLObject::sv_occupancy() {
-  int occ = 1 << 30;
-  for (int fwd = 0; fwd < 2; fwd++) {
-    int o = 0;
-    cudaError_t e;
-    // the two-right-hand-side instantiation needs the most shared memory: it decides how many CTAs are co-resident
-    if (solve_minb == 2) e = fwd ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k_solve2<true, 2, 2>, SV_NT, sv_smem[1]) : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k_solve2<false, 2, 2>, SV_NT, sv_smem[1]);
-    else if (solve_minb == 3) e = fwd ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k_solve2<true, 2, 3>, SV_NT, sv_smem[1]) : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k_solve2<false, 2, 3>, SV_NT, sv_smem[1]);
-    else e = fwd ? cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k_solve2<true, 2, 4>, SV_NT, sv_smem[1]) : cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, k_solve2<false, 2, 4>, SV_NT, sv_smem[1]);
-    if (e != cudaSuccess) return 0;
-    occ = std::min(occ, o);
-  }
-  return occ;
-}
-
-template <bool FWD, int NR>
-static void sv_launch(int minb, int grid, size_t smem, cudaStream_t st, const LDLDev& d, const SVPlan& q, const SVRhs& r, int cap) {
-  if (minb == 2) k_solve2<FWD, NR, 2><<<grid, SV_NT, smem, st>>>(d, q, r, cap);
-  else if (minb == 3) k_solve2<FWD, NR, 3><<<grid, SV_NT, smem, st>>>(d, q, r, cap);
-  else k_solve2<FWD, NR, 4><<<grid, SV_NT, smem, st>>>(d, q, r, cap);
+  // the two-right-hand-side instantiations need the most shared memory: they decide how many CTAs are co-resident
+  int of = 0, ob = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&of, k_solve2<true, 2>, SV_NT, sv_smem[1]) != cudaSuccess ||
+      cudaOccupancyMaxActiveBlocksPerMultiprocessor(&ob, k_solve2<false, 2>, SV_NT, sv_smem[1]) != cudaSuccess)
+    return 0;
+  return std::min(of, ob);
 }
 
 // one sweep kernel over the task queue as it stands (queue heads / counters are prepared by the caller)
 void LDLObject::sv_sweep(bool fwd, int nrhs, const SVPlan& q, const SVRhs& r) {
   g_launches++;
   const size_t smem = sv_smem[nrhs - 1];
-  if (fwd) { if (nrhs == 1) sv_launch<true, 1>(solve_minb, df_grid, smem, stream, dev, q, r, sv_cap); else sv_launch<true, 2>(solve_minb, df_grid, smem, stream, dev, q, r, sv_cap); }
-  else { if (nrhs == 1) sv_launch<false, 1>(solve_minb, df_grid, smem, stream, dev, q, r, sv_cap); else sv_launch<false, 2>(solve_minb, df_grid, smem, stream, dev, q, r, sv_cap); }
+  if (fwd) { if (nrhs == 1) k_solve2<true, 1><<<sv_grid, SV_NT, smem, stream>>>(dev, q, r, sv_cap); else k_solve2<true, 2><<<sv_grid, SV_NT, smem, stream>>>(dev, q, r, sv_cap); }
+  else { if (nrhs == 1) k_solve2<false, 1><<<sv_grid, SV_NT, smem, stream>>>(dev, q, r, sv_cap); else k_solve2<false, 2><<<sv_grid, SV_NT, smem, stream>>>(dev, q, r, sv_cap); }
 }
 // the level-0 fronts: before the forward sweep, after the backward sweep.  The three kernels touch disjoint fronts and
 // none depends on another, so the two narrow-leaf kernels run on side streams next to the wide-leaf kernel
 // (C4: 24 + 48 + 186 us one after the other -> ~190 us together)
 void LDLObject::sv_leaves(bool fwd, int nrhs, const SVRhs& r) {
-  const bool side = stream_a && stream_b && ((sv_nleaf1 ? 1 : 0) + (sv_nleafn ? 1 : 0) + (sv_nleafw ? 1 : 0)) > 1;
+  const bool side = ((sv_nleaf1 ? 1 : 0) + (sv_nleafn ? 1 : 0) + (sv_nleafw ? 1 : 0)) > 1;
   cudaStream_t s1 = side ? stream_a : stream, sn = side ? stream_b : stream;
   if (side) {
     cudaEventRecord(ev_leaf[0], stream);
@@ -2324,21 +1900,10 @@ __global__ void k_scatter_idx(int n, const int* __restrict__ idx, const double* 
 }
 
 int LDLObject::refactor_phase_async(int phase) {
-  if (!sharded() || !factor_dataflow) return CLDL_E_ARG;
+  if (!sharded()) return CLDL_E_ARG;
   CK(cudaSetDevice(device));
   if (phase == 0) {
-    CK(cudaMemsetAsync(dev.status, 0, ST_COUNT * sizeof(int), stream));
-    CK(cudaMemcpyAsync(d_dff_cnt, d_dff_init, dff_nsup4 * sizeof(int), cudaMemcpyDeviceToDevice, stream));
-    CK(cudaMemsetAsync(dff.qhead, 0, sizeof(int), stream));
-    for (const LaunchSeg& g : plan) {
-      if (g.level != 0 || (g.kind != 0 && g.kind != 3) || g.count == 0) continue;
-      g_launches++;
-      if (g.kind == 3) k_factor_leaf1<<<(g.count + 255) / 256, 256, 0, stream>>>(dev, g.base, g.count);
-      else if (g.threads == 64)
-        k_factor_level<64><<<g.count, 64, (size_t)g.smem_doubles * 8, stream>>>(dev, g.base, g.smem_doubles);
-      else
-        k_factor_level<256><<<g.count, 256, (size_t)g.smem_doubles * 8, stream>>>(dev, g.base, g.smem_doubles);
-    }
+    if (int rc = refactor_level0()) return rc;
     DFFactor q = dff;
     q.ntask = dff_ntask_owned;
     g_launches++;

@@ -14,9 +14,8 @@
 #define CB_PB_MAXNS 64     /* widest panel (columns) of a front */
 #define CB_PB_LD 66        /* padded leading dimension of the pivot block in shared memory */
 #define CB_SOLVE_SMALL_NS 8 /* solves: fronts with at most this many pivots get one warp, wider ones one CTA */
-#define CB_SOLVE_STAGE 1536  /* doubles of gathered x staged in shared memory by k_bwd_big */
 #define CB_SMALL_CHILD 16  /* children of big fronts with at most this many rows go through sorted entry lists */
-#define CB_BIG_NR 96       /* fronts with at least this many rows below the pivot block use the multi-CTA path */
+#define CB_BIG_NR 96       /* fronts with at least this many rows below the pivot block are factored by D, R and T tasks */
 
 namespace cb {
 
@@ -35,14 +34,11 @@ struct LDLDev {
   const long long* asm_ptr = nullptr;
   const int* asm_src = nullptr;
   const long long* asm_dst = nullptr;
-  const int* level_tasks = nullptr;
-  const int* child_nb = nullptr;      // per front: rows that land inside its parent's pivot block
-  const int2* child_trange = nullptr; // per front: [first,last] 64-row tile of the parent's update matrix it touches
-  const int* child_tptr_off = nullptr; // per front: offset into child_tptr
-  const int* child_tptr = nullptr;     // first own row falling into each parent tile row (tlo..thi+1)
-  const signed char* child_small = nullptr;  // 1: child of a big front handled through the sorted entry lists
-  const int *sc_panel_ptr = nullptr, *sc_panel_src = nullptr, *sc_panel_dst = nullptr;  // per big front
-  const int *sc_tile_ptr = nullptr, *sc_tile_src = nullptr, *sc_tile_dst = nullptr;     // per update tile
+  const int* level_tasks = nullptr;   // fronts of tree level 0 in the order of the launch plan (LaunchSeg)
+  // small children of big fronts: (src,dst) entries sorted by dst, per big front (panel) and per update tile; a factor
+  // task's range is in its record
+  const int *sc_panel_src = nullptr, *sc_panel_dst = nullptr;
+  const int *sc_tile_src = nullptr, *sc_tile_dst = nullptr;
   const int* gat_ptr = nullptr;       // solves: per front slot, CSR of contributing child update-vector entries
   const int* gat_src = nullptr;
   const int* perm = nullptr;
@@ -58,9 +54,11 @@ struct LDLDev {
   int reg_enable = 1;
 };
 
+// one launch of the level-0 factorisation over level_tasks[base, base + count): k_factor_leaf1 (single-column fronts,
+// one thread each) or k_factor_level<threads> with smem_doubles of dynamic shared memory
 struct LaunchSeg {
-  int kind = 0;  // 0 fused small fronts, 1 big-front panels, 2 big-front update tiles
-  int level, base, count, smem_doubles, threads;
+  bool leaf1;
+  int base, count, smem_doubles, threads;
 };
 
 // dataflow factorisation plan (see k_factor_df in ldl.cu)
@@ -74,7 +72,7 @@ struct DFFactor {
   int* tiles_left = nullptr;        // [nsup]
   int* qhead = nullptr;
   const int* parent = nullptr;
-  const int* big_pos = nullptr;     // [nsup] index into sc_panel_ptr (position in the big-front list) or -1
+  const int* big_pos = nullptr;     // [nsup] position in the big-front list or -1
   const int* tile_base = nullptr;   // [nsup] first global tile id of the front or -1
   unsigned long long* trace = nullptr;  // optional [ntask][4]: grab, ready, end (globaltimer ns), smid
 };
@@ -100,9 +98,7 @@ class LDLObject {
   std::vector<int> h_dff_tasks;
   int dff_grid = 0;
   size_t dff_nsup4 = 0;
-  bool factor_dataflow = true;
-  int df_grid = 0;
-  int solve_minb = 4;
+  int sv_grid = 0;                  // CTAs of a sweep kernel (as many as can be co-resident)
   bool use_dataflow = true;
   int n = 0;
   int64_t nnzA = 0;
@@ -124,9 +120,6 @@ class LDLObject {
   double* d_tmp_val = nullptr;
   signed char* d_tmp_sgn = nullptr;
   size_t tmp_cap = 0;
-  int* d_big_tasks = nullptr;
-  int4* d_tiles = nullptr;
-  int64_t n_tiles = 0;
   std::vector<int> h_idx;
   bool factored = false;
   uint64_t regularize_count = 0, positive_inertia = 0;
@@ -167,6 +160,7 @@ class LDLObject {
   int init(int n, const int64_t* Ap, const int32_t* Ai, const double* Ax, const int8_t* dsigns,
            const cldl_opts& o, const int* perm_in);
   void release();
+  int refactor_level0();   // the start of every refactor: counters reset, tree level 0 factored
   int refactor_async();
   int sync_status();
   // one right-hand side, or two swept together (d_x1 / d_b1 non-null): the panels are read once for both

@@ -451,8 +451,8 @@ __device__ __forceinline__ void sv_stage(double* sl, int boff, const double* __r
   }
 }
 
-template <bool FWD, int NR, int MINB>
-__global__ void __launch_bounds__(SV_NT, MINB) k_solve2(LDLDev d, SVPlan q, SVRhs r, int cap) {
+template <bool FWD, int NR>
+__global__ void __launch_bounds__(SV_NT, SV_MINB) k_solve2(LDLDev d, SVPlan q, SVRhs r, int cap) {
   extern __shared__ __align__(16) double sv_smem[];
   double* slab = sv_smem;                       // cap doubles (+ 2 of slack: a bulk copy is rounded up to 16 bytes)
   double* sw = slab + cap + 2;                  // NR * 64: gathered right-hand side of the pivot block / D^-1 y - sums

@@ -268,7 +268,6 @@ __device__ __forceinline__ void df_wait_set(volatile int* p) {
 // schedule: results are bit-identical run to run.
 // ------------------------------------------------------------------------
 #define DF_NT 256
-#define TS 64   /* rows and columns of an update-matrix tile (T tasks) */
 #define DF_SMEM_DOUBLES (CB_PB_MAXNS * CB_PB_LD + 2 * CB_PB_MAXNS + CB_PB_MAXNS * 128)   /* 12544 doubles = 98 KB (R task); T needs 12352 */
 
 __device__ __forceinline__ double ldcg_d(const double* p) { return __ldcg(p); }
@@ -392,14 +391,12 @@ __device__ void dff_small(const LDLDev& d, int s, double* sm, int* s_flag) {
   if (use_sm) for (long long i = tid; i < psz; i += DF_NT) P[i] = W[i];
 }
 
-// ---- task / child records built by the host (LDLObject::init) ----
-// DFTask   (16 ints): kind, s, a, b, ns, nr, f, d0, d1, e0, e1, -, panel_off (2), upd_off (2)
-// DFChild  (12 ints): U offset (2), rel offset (2), nrc, a0, a1, b0, b1, -, -, -
-//   rows a0..a1 and columns b0..b1 (child-local indices) of the child's update matrix land in this task's
-//   target (pivot block / row block / tile); only a >= b is stored.
-struct DFChildRec { long long uoff, relp; int nrc, a0, a1, b0, b1, p0, p1, p2; };
+// ---- D, R and T tasks read their records (DFTask, DFChildRec: ldl_plan.h) by field ----
 #define DF_DCAP 32          /* child records staged per round */
-#define DF_RB 128           /* rows per R task */
+#define DF_REC_INTS ((int)(sizeof(DFChildRec) / sizeof(int)))
+// an int field of a child record in global memory, loaded on its own: read through a DFChildRec lvalue, the record's
+// 8-byte alignment lets the compiler pair neighbouring fields into 64-bit loads, which reschedules the tile task
+#define DF_REC_INT(r, field) (reinterpret_cast<const int*>(r)[offsetof(DFChildRec, field) / sizeof(int)])
 
 // One child's block added into a shared-memory target.  The 8 warps own the target COLUMNS (column & 7), so no
 // two warps ever touch the same element and a warp meets the children in list order: sums keep a fixed order
@@ -412,10 +409,10 @@ __device__ __forceinline__ void df_add_child(const LDLDev& d, const DFChildRec& 
   const int* __restrict__ relc = d.rel + ch.relp;
   const double* Uc = d.U + ch.uoff;
   __syncwarp();
-  if (ch.p0 == 3) {
+  if (ch.contig == 3) {
     // rows and columns of the block are contiguous in the target (the previous panel of the same separator,
     // dense children): no index loads, warp-wide coalesced reads down the columns this warp owns
-    const int r0 = ch.p1 - rowoff - ch.a0, c0 = ch.p2 - coloff - ch.b0;   // target row of a: r0 + a, column of b: c0 + b
+    const int r0 = ch.ra0 - rowoff - ch.a0, c0 = ch.rb0 - coloff - ch.b0;   // target row of a: r0 + a, column of b: c0 + b
     const int bfirst = ch.b0 + ((warp - (c0 + ch.b0)) & 7);
     const int a1 = ch.a1, b1 = ch.b1;
     for (int ab = ch.a0; ab < a1; ab += 32 * NH) {
@@ -556,7 +553,8 @@ template <class F>
 __device__ __forceinline__ void df_children(const DFFactor& q, int d0, int d1, int* s_desc, F f) {
   for (int base = d0; base < d1; base += DF_DCAP) {
     const int cnt = min(DF_DCAP, d1 - base);
-    for (int i = threadIdx.x; i < cnt * 12; i += DF_NT) s_desc[i] = q.desc[(size_t)base * 12 + i];
+    const int* src = reinterpret_cast<const int*>(q.recs);
+    for (int i = threadIdx.x; i < cnt * DF_REC_INTS; i += DF_NT) s_desc[i] = src[(size_t)base * DF_REC_INTS + i];
     __syncthreads();
     const DFChildRec* rec = reinterpret_cast<const DFChildRec*>(s_desc);
     for (int k = 0; k < cnt; k++) f(rec[k]);
@@ -569,17 +567,17 @@ __device__ __forceinline__ void df_children(const DFFactor& q, int d0, int d1, i
 // owns the 4x4 block (rows 4bi.., columns 4bj..) of the lower triangle; per pivot the owners of the pivot
 // column publish it through a double-buffered shared column (one barrier per pivot), the owner of the diagonal
 // element applies the sign test / regularisation and the reciprocal.
-__device__ void dff_diag(const LDLDev& d, const DFFactor& q, const int* tk, double* sm, int* s_desc, int* s_ed, double* s_ev) {
+__device__ void dff_diag(const LDLDev& d, const DFFactor& q, const DFTask& tk, double* sm, int* s_desc, int* s_ed, double* s_ev) {
   double* sA = sm;                                     // [64][CB_PB_LD]
   double* sSign = sm + CB_PB_MAXNS * CB_PB_LD;         // [64]
   double* colbuf = sSign + CB_PB_MAXNS;                // [2][72]: column, then dj, 1/dj
   const int tid = threadIdx.x;
-  const int s = tk[1], ns = tk[4], nr = tk[5], f = tk[6];
+  const int s = tk.s, ns = tk.ns, nr = tk.nr, f = tk.f;
   const int ld = ns + nr;
-  const long long poff = *reinterpret_cast<const long long*>(tk + 12);
+  const long long poff = tk.poff;
   double* P = d.L + poff;
   DFEnt pe;
-  df_ent_issue(d.U, d.sc_panel_src, d.sc_panel_dst, tk[9], tk[10], pe);
+  df_ent_issue(d.U, d.sc_panel_src, d.sc_panel_dst, tk.e0, tk.e1, pe);
   for (int i = tid; i < CB_PB_MAXNS * CB_PB_LD; i += DF_NT) sA[i] = 0.0;
   if (tid < CB_PB_MAXNS) sSign[tid] = tid < ns ? (double)d.dsigns[f + tid] : 1.0;
   __syncthreads();
@@ -588,8 +586,8 @@ __device__ void dff_diag(const LDLDev& d, const DFFactor& q, const int* tk, doub
     if (row < ns) sA[col * CB_PB_LD + row] = v;
   });
   __syncthreads();
-  df_children(q, tk[7], tk[8], s_desc, [&](const DFChildRec& ch) { df_add_child<2>(d, ch, sA, 0, 1, 0, CB_PB_LD); });
-  df_ent_apply(sA, d.U, d.sc_panel_src, d.sc_panel_dst, tk[9], tk[10], pe, s_ed, s_ev,
+  df_children(q, tk.d0, tk.d1, s_desc, [&](const DFChildRec& ch) { df_add_child<2>(d, ch, sA, 0, 1, 0, CB_PB_LD); });
+  df_ent_apply(sA, d.U, d.sc_panel_src, d.sc_panel_dst, tk.e0, tk.e1, pe, s_ed, s_ev,
                [&](int dd) -> long long { const int col = dd / ld, row = dd - col * ld; return row < ns ? (long long)col * CB_PB_LD + row : -1; });
   __syncthreads();
   DF_STAMP(q, 4);
@@ -673,19 +671,19 @@ __device__ void dff_diag(const LDLDev& d, const DFFactor& q, const int* tk, doub
 }
 
 // ---- R: DF_RB rows below the pivot block: assemble in shared memory, wait for D, triangular solve ----
-__device__ void dff_rows(const LDLDev& d, const DFFactor& q, const int* tk, double* sm, int* s_desc, int* s_ed, double* s_ev) {
+__device__ void dff_rows(const LDLDev& d, const DFFactor& q, const DFTask& tk, double* sm, int* s_desc, int* s_ed, double* s_ev) {
   double* sA = sm;                                     // [64][CB_PB_LD]  L11 (unit lower, column major)
   double* sDval = sm + CB_PB_MAXNS * CB_PB_LD;
   double* sDinv = sDval + CB_PB_MAXNS;
   double* sR = sDinv + CB_PB_MAXNS;                    // [64][DF_RB]  the rows, column major
   const int tid = threadIdx.x;
-  const int s = tk[1], blk = tk[2], ns = tk[4], nr = tk[5], f = tk[6];
+  const int s = tk.s, blk = tk.a, ns = tk.ns, nr = tk.nr, f = tk.f;
   const int ld = ns + nr;
-  double* P = d.L + *reinterpret_cast<const long long*>(tk + 12);
+  double* P = d.L + tk.poff;
   const int r0 = blk * DF_RB, r1 = min(nr, r0 + DF_RB);
   const int g0 = ns + r0, g1 = ns + r1;
   DFEnt pe;
-  df_ent_issue(d.U, d.sc_panel_src, d.sc_panel_dst, tk[9], tk[10], pe);
+  df_ent_issue(d.U, d.sc_panel_src, d.sc_panel_dst, tk.e0, tk.e1, pe);
   for (int i = tid; i < CB_PB_MAXNS * DF_RB; i += DF_NT) sR[i] = 0.0;
   __syncthreads();
   df_scatter_asm(d, s, [&](long long dst, double v) {
@@ -693,8 +691,8 @@ __device__ void dff_rows(const LDLDev& d, const DFFactor& q, const int* tk, doub
     if (row >= g0 && row < g1) sR[col * DF_RB + row - g0] = v;
   });
   __syncthreads();
-  df_children(q, tk[7], tk[8], s_desc, [&](const DFChildRec& ch) { df_add_child<4>(d, ch, sR, g0, 1, 0, DF_RB); });
-  df_ent_apply(sR, d.U, d.sc_panel_src, d.sc_panel_dst, tk[9], tk[10], pe, s_ed, s_ev,
+  df_children(q, tk.d0, tk.d1, s_desc, [&](const DFChildRec& ch) { df_add_child<4>(d, ch, sR, g0, 1, 0, DF_RB); });
+  df_ent_apply(sR, d.U, d.sc_panel_src, d.sc_panel_dst, tk.e0, tk.e1, pe, s_ed, s_ev,
                [&](int dd) -> long long { const int col = dd / ld, row = dd - col * ld; return (row >= g0 && row < g1) ? (long long)col * DF_RB + row - g0 : -1; });
   __syncthreads();
   DF_STAMP(q, 4);
@@ -746,22 +744,22 @@ __device__ void dff_rows(const LDLDev& d, const DFFactor& q, const int* tk, doub
 }
 
 // ---- T: one 64x64 tile of the update matrix ----
-__device__ void dff_tile(const LDLDev& d, const DFFactor& q, const int* tk, double* sm, int* s_desc, int* s_ed, double* s_ev) {
+__device__ void dff_tile(const LDLDev& d, const DFFactor& q, const DFTask& tk, double* sm, int* s_desc, int* s_ed, double* s_ev) {
   double* sAt = sm;                      // [ns][TS]  L21 rows of tile-row I
   double* sBt = sm + TS * TS;            // [ns][TS]  L21 rows of tile-row J, scaled by D
   double* sC = sm + 2 * TS * TS;         // [TS][TS+1] children's contributions
   double* sD = sC + TS * (TS + 1);       // [ns]
   const int tid = threadIdx.x;
-  const int ti = tk[2], tj = tk[3], ns = tk[4], nr = tk[5], f = tk[6];
+  const int ti = tk.a, tj = tk.b, ns = tk.ns, nr = tk.nr, f = tk.f;
   const int ld = ns + nr;
-  const double* P = d.L + *reinterpret_cast<const long long*>(tk + 12);
-  double* U = d.U + *reinterpret_cast<const long long*>(tk + 14);
+  const double* P = d.L + tk.poff;
+  double* U = d.U + tk.uoff;
   const int i0 = ti * TS, j0 = tj * TS;
   const int ni = min(TS, nr - i0), nj = min(TS, nr - j0);
   // every independent load of the task is issued up front (sorted entries, child records, the whole K range
   // of both panels) so that the task pays ~3 dependent memory round trips instead of one per stage
   DFEnt pe;
-  df_ent_issue(d.U, d.sc_tile_src, d.sc_tile_dst, tk[9], tk[10], pe);
+  df_ent_issue(d.U, d.sc_tile_src, d.sc_tile_dst, tk.e0, tk.e1, pe);
   {
     // finished panels are immutable for the rest of the launch and start on sector boundaries, so they may
     // travel through L1: 8-byte cp.async straight into shared memory, no registers, no issue stall
@@ -806,12 +804,12 @@ __device__ void dff_tile(const LDLDev& d, const DFFactor& q, const int* tk, doub
   for (int i = 0; i < 4; i++)
 #pragma unroll
     for (int j = 0; j < 4; j++) creg[i][j] = 0.0;
-  const int ndense = tk[11];
+  const int ndense = tk.ndense;
   for (int kd = 0; kd < ndense; kd++) {
-    const int* rec = q.desc + (size_t)(tk[7] + kd) * 12;
-    const long long uoff = *reinterpret_cast<const long long*>(rec);
-    const int nrc = rec[4], a0 = rec[5], a1 = rec[6], b0 = rec[7], b1 = rec[8];
-    const int ra = a0 - (rec[10] - (ns + i0)), rb = b0 - (rec[11] - (ns + j0));   // child index = tile index + ra / rb
+    const DFChildRec* rec = q.recs + (size_t)(tk.d0 + kd);
+    const long long uoff = rec->uoff;
+    const int nrc = DF_REC_INT(rec, nrc), a0 = DF_REC_INT(rec, a0), a1 = DF_REC_INT(rec, a1), b0 = DF_REC_INT(rec, b0), b1 = DF_REC_INT(rec, b1);
+    const int ra = a0 - (DF_REC_INT(rec, ra0) - (ns + i0)), rb = b0 - (DF_REC_INT(rec, rb0) - (ns + j0));   // child index = tile index + ra / rb
     const double* Uc = d.U + uoff;
     double v[4][4];
 #pragma unroll
@@ -828,14 +826,14 @@ __device__ void dff_tile(const LDLDev& d, const DFFactor& q, const int* tk, doub
 #pragma unroll
       for (int j = 0; j < 4; j++) creg[i][j] += v[i][j];
   }
-  const bool use_sc = (tk[8] - tk[7] > ndense) || (tk[10] > tk[9]);
+  const bool use_sc = (tk.d1 - tk.d0 > ndense) || (tk.e1 > tk.e0);
   if (use_sc) {
     for (int idx = tid; idx < TS * (TS + 1); idx += DF_NT) sC[idx] = 0.0;
     __syncthreads();
     DF_STAMP(q, 7);
-    df_children(q, tk[7] + ndense, tk[8], s_desc, [&](const DFChildRec& ch) { df_add_child<2>(d, ch, sC, ns + i0, TS + 1, ns + j0, 1); });
+    df_children(q, tk.d0 + ndense, tk.d1, s_desc, [&](const DFChildRec& ch) { df_add_child<2>(d, ch, sC, ns + i0, TS + 1, ns + j0, 1); });
     DF_STAMP(q, 8);
-    df_ent_apply(sC, d.U, d.sc_tile_src, d.sc_tile_dst, tk[9], tk[10], pe, s_ed, s_ev, [&](int dd) -> long long { return dd; });
+    df_ent_apply(sC, d.U, d.sc_tile_src, d.sc_tile_dst, tk.e0, tk.e1, pe, s_ed, s_ev, [&](int dd) -> long long { return dd; });
   }
 #ifndef CB_EMU
   asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -918,7 +916,7 @@ __device__ void dff_tile(const LDLDev& d, const DFFactor& q, const int* tk, doub
 
 __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
   extern __shared__ __align__(16) double dfsm[];
-  __shared__ __align__(16) int s_desc[DF_DCAP * 12];
+  __shared__ __align__(16) int s_desc[DF_DCAP * DF_REC_INTS];
   __shared__ __align__(16) int s_task[16];
   __shared__ int s_ed[DF_ENT_FAST];
   __shared__ double s_ev[DF_ENT_FAST];
@@ -944,7 +942,8 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
     if (qi < 0) break;
     if (tid < 4) reinterpret_cast<int4*>(s_task)[tid] = q.tasks[4 * (size_t)qi + tid];
     __syncthreads();
-    const int kind = s_task[0], s = s_task[1];
+    const DFTask& tk = *reinterpret_cast<const DFTask*>(s_task);
+    const int kind = tk.kind, s = tk.s;
     if (kind == 0) {
       if (tid == 0) { df_wait_zero(q.pend + s); __threadfence(); if (q.trace) q.trace[10 * (size_t)qi + 1] = df_gtime(); }
       __syncthreads();
@@ -954,7 +953,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
     } else if (kind == 1) {
       if (tid == 0) { df_wait_zero(q.pend + s); __threadfence(); if (q.trace) q.trace[10 * (size_t)qi + 1] = df_gtime(); }
       __syncthreads();
-      dff_diag(d, q, s_task, dfsm, s_desc, s_ed, s_ev);
+      dff_diag(d, q, tk, dfsm, s_desc, s_ed, s_ev);
       __syncthreads();
       if (tid == 0) { __threadfence(); atomicExch(q.diag_done + s, 1); }
     } else if (kind == 2) {
@@ -962,13 +961,13 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
       // first, assembles, and only then waits for the D task of the front
       if (tid == 0) { df_wait_zero(q.pend + s); __threadfence(); if (q.trace) q.trace[10 * (size_t)qi + 1] = df_gtime(); }
       __syncthreads();
-      dff_rows(d, q, s_task, dfsm, s_desc, s_ed, s_ev);
+      dff_rows(d, q, tk, dfsm, s_desc, s_ed, s_ev);
       __syncthreads();
       if (tid == 0) { __threadfence(); atomicSub(q.rows_left + s, 1); }
     } else {
       if (tid == 0) { df_wait_zero(q.rows_left + s); __threadfence(); if (q.trace) q.trace[10 * (size_t)qi + 1] = df_gtime(); }
       __syncthreads();
-      dff_tile(d, q, s_task, dfsm, s_desc, s_ed, s_ev);
+      dff_tile(d, q, tk, dfsm, s_desc, s_ed, s_ev);
       __syncthreads();
       if (tid == 0) {
         __threadfence();
@@ -1012,11 +1011,13 @@ __global__ void k_offset_values(double* __restrict__ vals, const int* __restrict
     }                                                                                \
   } while (0)
 
-template <class T>
-static int upload(T** dptr, const std::vector<T>& v) {
-  size_t bytes = (v.size() ? v.size() : 1) * sizeof(T);
-  CK(cudaMalloc((void**)dptr, bytes));
-  if (!v.empty()) CK(cudaMemcpy(*dptr, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+// a device copy of v (at least one element) in *dptr
+template <class D, class T>
+static int upload(D** dptr, const std::vector<T>& v) {
+  T* p = nullptr;
+  CK(cudaMalloc((void**)&p, (v.size() ? v.size() : 1) * sizeof(T)));
+  if (!v.empty()) CK(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
+  *dptr = reinterpret_cast<D*>(p);
   return 0;
 }
 
@@ -1067,27 +1068,23 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   CK(cudaEventCreate(&ev1));
   CK(cudaMallocHost((void**)&h_status, ST_COUNT * sizeof(int)));
 
-  int* tmp_i = nullptr;
-  long long* tmp_l = nullptr;
   auto to_ll = [](const std::vector<int64_t>& v) { return std::vector<long long>(v.begin(), v.end()); };
-  if ((rc = upload(&tmp_i, S.sn_first))) return rc; dev.sn_first = tmp_i;
-  if ((rc = upload(&tmp_l, to_ll(S.sn_rowptr)))) return rc; dev.sn_rowptr = tmp_l;
-  if ((rc = upload(&tmp_i, S.sn_rows))) return rc; dev.sn_rows = tmp_i;
-  if ((rc = upload(&tmp_l, to_ll(S.child_ptr)))) return rc; dev.child_ptr = tmp_l;
-  if ((rc = upload(&tmp_i, S.child_list))) return rc; dev.child_list = tmp_i;
-  if ((rc = upload(&tmp_i, S.rel))) return rc; dev.rel = tmp_i;
-  if ((rc = upload(&tmp_l, to_ll(S.panel_off)))) return rc; dev.panel_off = tmp_l;
-  if ((rc = upload(&tmp_l, to_ll(S.upd_off)))) return rc; dev.upd_off = tmp_l;
-  if ((rc = upload(&tmp_l, to_ll(S.asm_ptr)))) return rc; dev.asm_ptr = tmp_l;
-  if ((rc = upload(&tmp_i, S.asm_src))) return rc; dev.asm_src = tmp_i;
-  if ((rc = upload(&tmp_l, to_ll(S.asm_dst)))) return rc; dev.asm_dst = tmp_l;
-  if ((rc = upload(&tmp_i, S.perm))) return rc; dev.perm = tmp_i;
+  if ((rc = upload(&dev.sn_first, S.sn_first))) return rc;
+  if ((rc = upload(&dev.sn_rowptr, to_ll(S.sn_rowptr)))) return rc;
+  if ((rc = upload(&dev.sn_rows, S.sn_rows))) return rc;
+  if ((rc = upload(&dev.child_ptr, to_ll(S.child_ptr)))) return rc;
+  if ((rc = upload(&dev.child_list, S.child_list))) return rc;
+  if ((rc = upload(&dev.rel, S.rel))) return rc;
+  if ((rc = upload(&dev.panel_off, to_ll(S.panel_off)))) return rc;
+  if ((rc = upload(&dev.upd_off, to_ll(S.upd_off)))) return rc;
+  if ((rc = upload(&dev.asm_ptr, to_ll(S.asm_ptr)))) return rc;
+  if ((rc = upload(&dev.asm_src, S.asm_src))) return rc;
+  if ((rc = upload(&dev.asm_dst, to_ll(S.asm_dst)))) return rc;
+  if ((rc = upload(&dev.perm, S.perm))) return rc;
   {
     std::vector<signed char> ds(n);
     for (int k = 0; k < n; k++) ds[k] = dsigns ? (signed char)dsigns[S.perm[k]] : (signed char)1;
-    signed char* t = nullptr;
-    if ((rc = upload(&t, ds))) return rc;
-    dev.dsigns = t;
+    if ((rc = upload(&dev.dsigns, ds))) return rc;
   }
   nnzA = Ap[n];
   CK(cudaMalloc((void**)&dev.vals, (size_t)(nnzA ? nnzA : 1) * sizeof(double)));
@@ -1118,584 +1115,111 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   dev.reg_delta = o.regularize_delta;
 
   cb_tmark("ldl: uploads + device alloc");
-  // rows of every child that land in its parent's pivot block (k_factor_df's child records) and the per-destination
-  // gather lists for the solves
-  std::vector<int> h_child_nb(S.nsup, 0);
-  // (runs on a host thread next to the launch plan and the small-child lists below; it only reads the symbolic
-  // structure and writes its own device arrays)
-  auto build_child_consts = [&]() -> int {
-    int rc = 0;
-    if (cudaSetDevice(device) != cudaSuccess) return CLDL_E_CUDA;
-    std::vector<int> gptr((size_t)n + S.sn_rows.size() + 1, 0);
-    for (int c = 0; c < S.nsup; c++) {
-      const int p = S.sn_parent[c];
-      if (p < 0) continue;
-      const int pns = S.sn_first[p + 1] - S.sn_first[p];
-      const int64_t pbase = (int64_t)S.sn_first[p] + S.sn_rowptr[p];
-      int nb = 0;
-      for (int64_t t = S.sn_rowptr[c]; t < S.sn_rowptr[c + 1]; t++) { if (S.rel[t] < pns) nb++; gptr[pbase + S.rel[t] + 1]++; }
-      h_child_nb[c] = nb;
-    }
-    for (size_t i = 0; i + 1 < gptr.size(); i++) gptr[i + 1] += gptr[i];
-    std::vector<int> gsrc(S.sn_rows.size() ? S.sn_rows.size() : 1, 0), pos(gptr.begin(), gptr.end() - 1);
-    // children in child_list order so that every destination sums in a fixed, reproducible order
-    for (int p = 0; p < S.nsup; p++) {
-      const int64_t pbase = (int64_t)S.sn_first[p] + S.sn_rowptr[p];
-      for (int64_t ci = S.child_ptr[p]; ci < S.child_ptr[p + 1]; ci++) {
-        const int c = S.child_list[ci];
-        for (int64_t t = S.sn_rowptr[c]; t < S.sn_rowptr[c + 1]; t++) gsrc[pos[pbase + S.rel[t]]++] = (int)t;
-      }
-    }
-    int* t1 = nullptr;
-    if ((rc = upload(&t1, gptr))) return rc; dev.gat_ptr = t1;
-    if ((rc = upload(&t1, gsrc))) return rc; dev.gat_src = t1;
-    return rc;
-  };
-  int rc_child = 0;
-  std::thread th_child([&]() { rc_child = build_child_consts(); });
-  struct ThJoin { std::thread* t; ~ThJoin() { if (t->joinable()) t->join(); } } th_child_guard{&th_child};
-  cb_tmark("ldl: child consts + gather lists");
-  // big fronts (nr >= CB_BIG_NR: k_factor_df's D, R and T tasks) in level order, and the 64x64 tiles of their update
-  // matrices: big_pos / tile_base number them for the small-child entry lists and the factor tasks
-  std::vector<int> big_pos(S.nsup, -1), tile_base(S.nsup, -1);
-  int nbig = 0, ntiles = 0;
-  auto is_big = [&](int s) { return big_pos[s] >= 0; };
-  for (int s : S.level_tasks) {
-    const long long ns = S.sn_first[s + 1] - S.sn_first[s];
-    const long long nr = S.sn_rowptr[s + 1] - S.sn_rowptr[s];
-    if (nr < CB_BIG_NR || ns > CB_PB_MAXNS) continue;
-    const int nt = (int)((nr + TS - 1) / TS);
-    big_pos[s] = nbig++;
-    tile_base[s] = ntiles;
-    ntiles += nt * (nt + 1) / 2;
-  }
-  // launch plan of tree level 0 (leaves: no dependencies, factored by plain launches before k_factor_df).  Single-column
-  // fronts take one thread each (k_factor_leaf1), the others one fused CTA each (k_factor_level), grouped by the
-  // shared-memory class of their panel.  level_tasks is reordered into these groups.
-  int max_optin = 0;
+  // plans (ldl_plan.cpp): the solve plan is built on a host thread beside the level-0 and factorisation plans
+  int max_optin = 0, nsm = 0;
   CK(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device));
-  const int cap_big = (max_optin - 2048) / 8;  // doubles
-  CK(cudaFuncSetAttribute(k_factor_level<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, cap_big * 8));
-  const long long classes[3] = {1024, 5632, cap_big};  // 8 KB, 44 KB, ~225 KB panels
-  plan.clear();
-  if (S.nlevels > 0) {
-    const int b = S.level_ptr[0], e = S.level_ptr[1];
-    std::vector<int> order[4], order1, big;
-    std::vector<int> not_mine;       // sharded: fronts of other ranks are parked at the end of the level's range
-    for (int t = b; t < e; t++) {
-      const int s = S.level_tasks[t];
-      const long long ns = S.sn_first[s + 1] - S.sn_first[s];
-      const long long nr = S.sn_rowptr[s + 1] - S.sn_rowptr[s];
-      if (is_big(s)) { big.push_back(s); continue; }
-      if (!mine(s)) { not_mine.push_back(s); continue; }
-      if (ns == 1) { order1.push_back(s); continue; }
-      const long long p = (ns + nr) * ns;
-      int c = p <= classes[0] ? 0 : p <= classes[1] ? 1 : p <= classes[2] ? 2 : 3;
-      order[c].push_back(s);
-    }
-    int pos = b;
-    if (!order1.empty()) {
-      plan.push_back(LaunchSeg{true, pos, (int)order1.size(), 0, 256});
-      for (int s : order1) S.level_tasks[pos++] = s;
-    }
-    for (int c = 3; c >= 0; c--) {
-      if (order[c].empty()) continue;
-      plan.push_back(LaunchSeg{false, pos, (int)order[c].size(), c == 3 ? 0 : (int)classes[c], c == 0 ? 64 : 256});
-      for (int s : order[c]) S.level_tasks[pos++] = s;
-    }
-    for (int s : big) S.level_tasks[pos++] = s;
-    for (int s : not_mine) S.level_tasks[pos++] = s;
-  }
-  if ((rc = upload(&tmp_i, S.level_tasks))) return rc; dev.level_tasks = tmp_i;
-  cb_tmark("ldl: launch plan");
-  // small children (nr <= CB_SMALL_CHILD) of big fronts: one dst-sorted (src,dst) list per panel and per tile
-  std::vector<signed char> small_child;
-  std::vector<int> h_sc_panel_ptr, h_sc_tile_ptr;
+  CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+  const int level_cap = (max_optin - 2048) / 8;  // doubles of the largest k_factor_level class
+  // the solve slab size that goes with SV_MINB resident CTAs per SM (227 KB of shared memory per SM, 1 KB reserved per CTA)
+  const size_t extra2 = (size_t)2 * (2 * CB_PB_MAXNS + SV_MAXROWS + 4 * CB_PB_MAXNS) * sizeof(double);   // NR = 2 vectors
   {
-    std::vector<signed char>& small = small_child;
-    small.assign(S.nsup, 0);
-    struct Ent { int key; int dst; int src; };
-    std::vector<Ent> pe, te;
-    {
-      // two passes over the children on host threads: count (pe / te entries per child), prefix sums, fill -- the
-      // entry order (child, column b, row a) is the one of a single loop
-      const unsigned hc2 = std::max(1u, std::min(16u, host_threads()));
-      const unsigned nth2 = S.nsup < 20000 ? 1u : hc2;
-      std::vector<int64_t> npe((size_t)S.nsup + 1, 0), nte((size_t)S.nsup + 1, 0);
-      auto eligible = [&](int c) {
-        const int p = S.sn_parent[c];
-        if (p < 0 || big_pos[p] < 0) return false;
-        const int nrc = (int)(S.sn_rowptr[c + 1] - S.sn_rowptr[c]);
-        if (nrc > CB_SMALL_CHILD) return false;
-        if (S.upd_off[c] + (int64_t)nrc * nrc > 0x7fffffffLL) return false;   // int32 source indices
-        return true;
-      };
-      auto run = [&](auto&& fn) {
-        if (nth2 == 1) { fn(0, S.nsup); return; }
-        std::vector<std::thread> th;
-        for (unsigned t = 0; t < nth2; t++)
-          th.emplace_back([&, t]() { fn((int)((int64_t)S.nsup * t / nth2), (int)((int64_t)S.nsup * (t + 1) / nth2)); });
-        for (auto& x : th) x.join();
-      };
-      run([&](int c0, int c1) {
-        for (int c = c0; c < c1; c++) {
-          if (!eligible(c)) continue;
-          small[c] = 1;
-          const int p = S.sn_parent[c];
-          const int64_t b0 = S.sn_rowptr[c];
-          const int nrc = (int)(S.sn_rowptr[c + 1] - b0);
-          const int pns = S.sn_first[p + 1] - S.sn_first[p];
-          int64_t np_ = 0;
-          for (int b = 0; b < nrc; b++) if (S.rel[b0 + b] < pns) np_ += nrc - b;
-          npe[c + 1] = np_;
-          nte[c + 1] = (int64_t)nrc * (nrc + 1) / 2 - np_;
-        }
-      });
-      for (int c = 0; c < S.nsup; c++) { npe[c + 1] += npe[c]; nte[c + 1] += nte[c]; }
-      pe.resize((size_t)npe[S.nsup]);
-      te.resize((size_t)nte[S.nsup]);
-      run([&](int c0, int c1) {
-        for (int c = c0; c < c1; c++) {
-          if (!small[c]) continue;
-          const int p = S.sn_parent[c];
-          const int64_t b0 = S.sn_rowptr[c];
-          const int nrc = (int)(S.sn_rowptr[c + 1] - b0);
-          const int pns = S.sn_first[p + 1] - S.sn_first[p];
-          const int pld = pns + (int)(S.sn_rowptr[p + 1] - S.sn_rowptr[p]);
-          Ent* wp = pe.data() + npe[c];
-          Ent* wt = te.data() + nte[c];
-          for (int b = 0; b < nrc; b++)
-            for (int a = b; a < nrc; a++) {
-              const int ra = S.rel[b0 + a], rb = S.rel[b0 + b];
-              const int64_t src = S.upd_off[c] + (int64_t)b * nrc + a;
-              if (rb < pns) *wp++ = Ent{big_pos[p], rb * pld + ra, (int)src};
-              else {
-                const int ti = (ra - pns) / TS, tj = (rb - pns) / TS;
-                *wt++ = Ent{tile_base[p] + ti * (ti + 1) / 2 + tj,
-                            (ra - pns - ti * TS) * (TS + 1) + (rb - pns - tj * TS), (int)src};
-              }
-            }
-        }
-      });
-    }
-    cb_tmark("ldl:   small-child: entries");
-    // bucket by key (counting sort keeps the child order inside a key), then order every bucket by dst with a
-    // stable sort; buckets are independent, so host threads share them
-    auto build = [&](std::vector<Ent>& v, size_t nkeys, std::vector<int>& ptr, std::vector<int>& src, std::vector<int>& dst) {
-      ptr.assign(nkeys + 1, 0);
-      for (auto& e : v) ptr[e.key + 1]++;
-      for (size_t i = 0; i < nkeys; i++) ptr[i + 1] += ptr[i];
-      std::vector<Ent> w(v.size());
-      {
-        std::vector<int> pos(ptr.begin(), ptr.end() - 1);
-        for (auto& e : v) w[pos[e.key]++] = e;
-      }
-      const unsigned hc = std::max(1u, std::min(16u, host_threads()));
-      std::vector<std::thread> th;
-      for (unsigned t = 0; t < hc; t++)
-        th.emplace_back([&, t]() {
-          for (size_t k = t; k < nkeys; k += hc)
-            std::stable_sort(w.begin() + ptr[k], w.begin() + ptr[k + 1], [](const Ent& x, const Ent& y) { return x.dst < y.dst; });
-        });
-      for (auto& x : th) x.join();
-      src.resize(w.size() ? w.size() : 1); dst.resize(w.size() ? w.size() : 1);
-      for (size_t i = 0; i < w.size(); i++) { src[i] = w[i].src; dst[i] = w[i].dst; }
-    };
-    // the panel lists and the tile lists are independent: the tile lists are built on a second host thread
-    std::vector<int> ptr, src, dst, tptr, tsrc, tdst;
-    int* t1 = nullptr;
-    {
-      std::thread tb([&]() { build(te, ntiles, tptr, tsrc, tdst); });
-      build(pe, nbig, ptr, src, dst);
-      tb.join();
-    }
-    cb_tmark("ldl:   small-child: panel + tile lists");
-    h_sc_panel_ptr = ptr;
-    if ((rc = upload(&t1, src))) return rc; dev.sc_panel_src = t1;
-    if ((rc = upload(&t1, dst))) return rc; dev.sc_panel_dst = t1;
-    h_sc_tile_ptr = tptr;
-    if ((rc = upload(&t1, tsrc))) return rc; dev.sc_tile_src = t1;
-    if ((rc = upload(&t1, tdst))) return rc; dev.sc_tile_dst = t1;
+    const size_t per_cta = ((size_t)227 * 1024) / SV_MINB - 1024 - 64;
+    sv_cap = (int)((per_cta - extra2) / sizeof(double)) - 2;
+    sv_cap &= ~1;
+    sv_cap = std::min(sv_cap, 16384);
   }
-  th_child.join();
-  if (rc_child) return rc_child;
-  cb_tmark("ldl: small-child entry lists");
-  // solve plan (ldl_solve.cuh): level-0 narrow fronts get plain kernels, everything else becomes queue tasks in level
-  // order -- batches of narrow fronts, and for every wide front a head task (pivot block + first rows) followed by row
-  // tasks when the panel exceeds the shared-memory slab.
-  {
-    int nsm = 0;
-    CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
-    // the slab size that goes with SV_MINB resident CTAs per SM (227 KB of shared memory per SM, 1 KB reserved per CTA)
-    const size_t extra2 = (size_t)2 * (2 * CB_PB_MAXNS + SV_MAXROWS + 4 * CB_PB_MAXNS) * sizeof(double);   // NR = 2 vectors
-    {
-      const size_t per_cta = ((size_t)227 * 1024) / SV_MINB - 1024 - 64;
-      sv_cap = (int)((per_cta - extra2) / sizeof(double)) - 2;
-      sv_cap &= ~1;
-      sv_cap = std::min(sv_cap, 16384);
-    }
-    const int cap = sv_cap;
-    auto wide = [&](int s) { return S.sn_first[s + 1] - S.sn_first[s] > CB_SOLVE_SMALL_NS; };
-    auto has_kids = [&](int s) { return S.child_ptr[s + 1] > S.child_ptr[s]; };
-    // head rows / rows per row task of a wide front
-    auto split = [&](int ns, int nr, int& rh, int& nrt, int& chunk) {
-      // a panel that fits goes to shared memory whole (one bulk copy, leading dimension ld); otherwise the head takes
-      // the pivot block + as many rows as fit and row tasks take the rest: a slab of r staged rows needs
-      // sv_lds(r, ld) * ns doubles + one for the alignment offset
-      const int ld = ns + nr;
-      if (nr <= SV_MAXROWS && (long long)ns * ld + 1 <= cap) { rh = nr; nrt = 0; chunk = 0; return; }
-      auto fits = [&](int staged) { return (long long)sv_lds(staged, ld) * ns + 1 <= (long long)cap; };
-      rh = std::min(nr, SV_MAXROWS);
-      while (rh > 0 && !fits(ns + rh)) rh--;
-      int rmax = SV_MAXROWS;
-      while (rmax > 1 && !fits(rmax)) rmax--;
-      const int rest = nr - rh;
-      nrt = rest > 0 ? (rest + rmax - 1) / rmax : 0;
-      chunk = nrt ? (rest + nrt - 1) / nrt : 0;
-    };
-    std::vector<int> leaf1, leafn, leafw, fronts, f2t(S.nsup, -1), nrt_of(S.nsup, 0), rh_of(S.nsup, 0), chunk_of(S.nsup, 0);
-    std::vector<SVTask> tk;
-    const int per = SV_NT / 32;
-    for (int ph = 0; ph < (sharded() ? 2 : 1); ph++) {
-      if (ph == 1) sv_ntask_owned = (int)tk.size();
-      std::vector<std::vector<int>> lev_small(S.nlevels), lev_big(S.nlevels);
-      for (int s = 0; s < S.nsup; s++) {
-        if (sharded() && (ph == 0 ? !owned(s) : shard.owner[s] >= 0)) continue;
-        if (!wide(s) && !has_kids(s)) { (S.sn_first[s + 1] - S.sn_first[s] == 1 ? leaf1 : leafn).push_back(s); continue; }
-        if (wide(s) && !has_kids(s) && S.sn_rowptr[s + 1] - S.sn_rowptr[s] <= 1024) {
-          leafw.push_back(s);
-          sv_leafw_nrmax = std::max(sv_leafw_nrmax, (int)(S.sn_rowptr[s + 1] - S.sn_rowptr[s]));
-          continue;
-        }
-        (wide(s) ? lev_big : lev_small)[S.sn_level[s]].push_back(s);
-      }
-      for (int l = 0; l < S.nlevels; l++) {
-        for (size_t i = 0; i < lev_small[l].size(); i += per) {
-          const int c = (int)std::min<size_t>(per, lev_small[l].size() - i);
-          SVTask t{};
-          t.kind = 0; t.s = (int)fronts.size(); t.cnt = c; t.dep1 = -1; t.dep2 = -1; t.bowner = -1; t.ptask = -1; t.cuoff = -1;
-          for (int k = 0; k < c; k++) { f2t[lev_small[l][i + k]] = (int)tk.size(); fronts.push_back(lev_small[l][i + k]); }
-          tk.push_back(t);
-        }
-        for (int s : lev_big[l]) {
-          const int ns = S.sn_first[s + 1] - S.sn_first[s], nr = (int)(S.sn_rowptr[s + 1] - S.sn_rowptr[s]);
-          int rh, nrt, chunk;
-          split(ns, nr, rh, nrt, chunk);
-          rh_of[s] = rh; nrt_of[s] = nrt; chunk_of[s] = chunk;
-          f2t[s] = (int)tk.size();
-          for (int b = -1; b < nrt; b++) {
-            SVTask t{};
-            t.kind = b < 0 ? 1 : 2; t.s = s; t.f = S.sn_first[s]; t.ns = ns; t.nr = nr;
-            t.r0 = b < 0 ? 0 : rh + b * chunk;
-            t.r1 = b < 0 ? rh : std::min(nr, rh + (b + 1) * chunk);
-            t.poff = S.panel_off[s]; t.rp = S.sn_rowptr[s];
-            t.dep0 = 0; t.dep1 = -1; t.dep2 = -1; t.nrt = nrt; t.bowner = -1; t.bslot = 0; t.pure = 0; t.ptask = -1; t.cuoff = -1;
-            t.notify = 1;
-            tk.push_back(t);
-          }
-        }
-      }
-    }
-    const int nt = (int)tk.size();
-    if (!sharded()) sv_ntask_owned = nt;
-    // chain children of wide fronts: followed slab by slab instead of awaited as a whole
-    std::vector<int> chain_child(S.nsup, -1), col2sn(n, 0);
-    for (int s = 0; s < S.nsup; s++)
-      for (int j = S.sn_first[s]; j < S.sn_first[s + 1]; j++) col2sn[j] = s;
-    for (int c = 0; c < S.nsup; c++) {
-      const int p = S.sn_parent[c];
-      if (p < 0 || !wide(c) || !wide(p) || chain_child[p] >= 0) continue;
-      const int64_t nrc = S.sn_rowptr[c + 1] - S.sn_rowptr[c];
-      const int64_t nsp = S.sn_first[p + 1] - S.sn_first[p], nrp = S.sn_rowptr[p + 1] - S.sn_rowptr[p];
-      if (nrc == nsp + nrp) chain_child[p] = c;       // rows(c) is a subset of cols(p)+rows(p): equal sizes = equal sets
-    }
-    // task of front c covering its row i (of its L21 part)
-    auto task_of_row = [&](int c, int i) {
-      if (i < rh_of[c]) return f2t[c];
-      return f2t[c] + 1 + (i - rh_of[c]) / chunk_of[c];
-    };
-    int nslots = 0;
-    std::vector<int> pend(nt, 0), fleft(S.nsup, 0), bleft(S.nsup, 0);
-    for (int s = 0; s < S.nsup; s++) {
-      if (f2t[s] < 0 || !wide(s)) continue;
-      const int ns = S.sn_first[s + 1] - S.sn_first[s], nr = (int)(S.sn_rowptr[s + 1] - S.sn_rowptr[s]);
-      const int h = f2t[s], nrt = nrt_of[s], p = S.sn_parent[s];
-      fleft[s] = 1 + nrt; bleft[s] = nrt;
-      const int c = chain_child[s];
-      const bool follow = c >= 0 && f2t[c] >= 0;      // a chain child of another rank is complete before this phase starts
-      const bool pure = c >= 0 && S.child_ptr[s + 1] - S.child_ptr[s] == 1;
-      for (int b = -1; b < nrt; b++) {
-        SVTask& t = tk[h + 1 + b];
-        t.ptask = p >= 0 ? f2t[p] : -1;
-        t.notify = (p >= 0 && chain_child[p] == s) ? 0 : 1;
-        t.pure = pure ? 1 : 0;
-        t.cuoff = pure ? (long long)S.sn_rowptr[c] : -1;
-        t.bslot = b < 0 ? nslots : nslots + b;
-        if (t.r1 > t.r0) t.bowner = col2sn[S.sn_rows[S.sn_rowptr[s] + t.r0]];
-        if (follow) {
-          if (b < 0) {
-            t.dep0 = task_of_row(c, 0); t.dep1 = task_of_row(c, ns - 1);
-            t.dep2 = t.r1 > 0 ? task_of_row(c, ns + t.r1 - 1) : t.dep1;
-          } else {
-            t.dep0 = task_of_row(c, ns + t.r0); t.dep1 = task_of_row(c, ns + t.r1 - 1);
-          }
-        }
-      }
-      nslots += nrt;
-      (void)nr;
-    }
-    for (int s = 0; s < S.nsup; s++) {
-      const int p = S.sn_parent[s];
-      if (p >= 0 && f2t[s] >= 0 && chain_child[p] != s) pend[f2t[p]]++;   // leaves and other ranks' fronts are complete before the sweep starts
-    }
-    // wide fronts whose pivot block is inverted after every refactorisation (all that this rank factors)
-    std::vector<int> wlist;
-    for (int s = 0; s < S.nsup; s++) if (wide(s) && mine(s)) wlist.push_back(s);
-    sv_nwide = (int)wlist.size();
-    // sorted by pivot count, cut into at most 8 runs (each run is launched with the shared memory of its widest front)
-    std::stable_sort(wlist.begin(), wlist.end(), [&](int a, int b) { return S.sn_first[a + 1] - S.sn_first[a] < S.sn_first[b + 1] - S.sn_first[b]; });
-    sv_wide_runs.clear();
-    {
-      const int bounds[] = {16, 24, 32, 40, 48, 56, CB_PB_MAXNS};
-      int pos = 0;
-      for (int bd : bounds) {
-        int e = pos;
-        while (e < sv_nwide && S.sn_first[wlist[e] + 1] - S.sn_first[wlist[e]] <= bd) e++;
-        if (e > pos) { sv_wide_runs.push_back(pos); sv_wide_runs.push_back(bd); pos = e; }
-      }
-      sv_wide_runs.push_back(sv_nwide); sv_wide_runs.push_back(0);
-    }
-    sv_nleaf1 = (int)leaf1.size(); sv_nleafn = (int)leafn.size(); sv_nleafw = (int)leafw.size();
-    sv_leafw_grid = sv_nleafw;      // one CTA per front (a loop over fronts inside fewer CTAs was slower: 312 vs 189 us forward on C4)
-    int* t1 = nullptr;
-    if ((rc = upload(&t1, wlist))) return rc; d_sv_wide = t1;
-    if ((rc = upload(&t1, leaf1))) return rc; d_sv_leaf1 = t1;
-    if ((rc = upload(&t1, leafn))) return rc; d_sv_leafn = t1;
-    if ((rc = upload(&t1, leafw))) return rc; d_sv_leafw = t1;
-    if ((rc = upload(&t1, fronts))) return rc; sv.fronts = t1;
-    if ((rc = upload(&t1, f2t))) return rc; sv.front2task = t1;
-    if ((rc = upload(&t1, S.sn_parent))) return rc; sv.parent = t1;
-    {
-      static_assert(sizeof(SVTask) == 96, "SVTask is 6 x int4");
-      int4* t4 = nullptr;
-      CK(cudaMalloc((void**)&t4, (size_t)(nt ? nt : 1) * sizeof(SVTask)));
-      if (nt) CK(cudaMemcpy(t4, tk.data(), (size_t)nt * sizeof(SVTask), cudaMemcpyHostToDevice));
-      sv.tasks = t4;
-    }
-    // counters: [pend(nt) | fleft(nsup) | bleft(nsup)] are copied from their initial values before every solve,
-    // [tdone(nt) | ydone(nsup) | done(nsup) | qhead(2)] are cleared
-    sv_ninit = (size_t)nt + 2 * (size_t)S.nsup;
-    sv_nzero = (size_t)nt + 2 * (size_t)S.nsup + 2;
-    std::vector<int> init(sv_ninit ? sv_ninit : 1, 0);
-    std::copy(pend.begin(), pend.end(), init.begin());
-    std::copy(fleft.begin(), fleft.end(), init.begin() + nt);
-    std::copy(bleft.begin(), bleft.end(), init.begin() + nt + S.nsup);
-    if ((rc = upload(&t1, init))) return rc; d_sv_init = t1;
-    CK(cudaMalloc((void**)&d_sv_cnt, (sv_ninit + sv_nzero) * sizeof(int)));
-    sv.pend = d_sv_cnt; sv.fleft = d_sv_cnt + nt; sv.bleft = sv.fleft + S.nsup;
-    sv.tdone = d_sv_cnt + sv_ninit; sv.ydone = sv.tdone + nt; sv.done = sv.ydone + S.nsup; sv.qhead = sv.done + S.nsup;
-    sv.bpart_stride = (long long)(nslots ? nslots : 1) * CB_PB_MAXNS;
-    CK(cudaMalloc((void**)&sv.bpart, (size_t)2 * sv.bpart_stride * sizeof(double)));
-    sv.ntask = nt;
-    // launch geometry: dynamic shared memory = slab + vectors for one or two right-hand sides
-    for (int nr2 = 1; nr2 <= 2; nr2++)
-      sv_smem[nr2 - 1] = ((size_t)cap + 2 + (size_t)nr2 * (2 * CB_PB_MAXNS + SV_MAXROWS + 4 * CB_PB_MAXNS)) * sizeof(double);
-    if ((rc = sv_configure())) return rc;
-    int occ = sv_occupancy();
-    if (occ < 1) return CLDL_E_CUDA;
-    sv_grid = nsm * occ;
-    use_dataflow = true;
-    if (std::getenv("CB_DF_TRACE_SOLVE") && nt > 0) {
-      CK(cudaMalloc((void**)&sv.trace, (size_t)nt * 8 * sizeof(unsigned long long)));
-      CK(cudaMemset(sv.trace, 0, (size_t)nt * 8 * sizeof(unsigned long long)));
-      h_sv_tasks.assign((const int*)tk.data(), (const int*)tk.data() + (size_t)nt * 24);
-    }
-    if (std::getenv("CB_TIMING") != nullptr) std::fprintf(stderr, "[cb timing]     solve plan: %d tasks (%d leaf columns, %d narrow leaves, %d wide leaves, %d wide fronts, %d row slabs), slab %d doubles, %d CTAs\n",
-                                     nt, sv_nleaf1, sv_nleafn, sv_nleafw, sv_nwide, nslots, cap, sv_grid);
+  SolvePlan sp;
+  std::thread th_solve([&]() { sp = build_solve_plan(S, shard.owner, shard_rank, sv_cap); });
+  struct ThJoin { std::thread& t; ~ThJoin() { if (t.joinable()) t.join(); } } th_solve_guard{th_solve};
+  Level0Plan l0 = build_level0_plan(S, shard.owner, shard_rank, level_cap);
+  FactorPlan fp = build_factor_plan(S, shard.owner, shard_rank);
+  th_solve.join();
+  cb_tmark("ldl: plans");
+
+  // tree level 0: plain launches
+  CK(cudaFuncSetAttribute(k_factor_level<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, level_cap * 8));
+  plan = std::move(l0.segs);
+  if ((rc = upload(&dev.level_tasks, l0.level_tasks))) return rc;
+
+  // dataflow factorisation (k_factor_df)
+  if ((rc = upload(&dev.sc_panel_src, fp.sc_panel_src))) return rc;
+  if ((rc = upload(&dev.sc_panel_dst, fp.sc_panel_dst))) return rc;
+  if ((rc = upload(&dev.sc_tile_src, fp.sc_tile_src))) return rc;
+  if ((rc = upload(&dev.sc_tile_dst, fp.sc_tile_dst))) return rc;
+  if (std::getenv("CB_TIMING")) std::fprintf(stderr, "[cb timing]     factor plan: %zu tasks, %zu child records, %zu big fronts, %zu tiles\n",
+                                              fp.tasks.size(), fp.recs.size(), fp.sc_panel_ptr.size() - 1, fp.sc_tile_ptr.size() - 1);
+  dff.ntask = (int)fp.tasks.size();
+  dff_ntask_owned = fp.ntask_owned;
+  if ((rc = upload(&dff.tasks, fp.tasks))) return rc;
+  if ((rc = upload(&dff.recs, fp.recs))) return rc;
+  if ((rc = upload(&d_dff_init, fp.cnt_init))) return rc;
+  CK(cudaMalloc((void**)&d_dff_cnt, fp.cnt_init.size() * sizeof(int) + 16));
+  dff.pend = d_dff_cnt; dff.diag_done = d_dff_cnt + S.nsup; dff.rows_left = d_dff_cnt + 2 * (size_t)S.nsup;
+  dff.tiles_left = d_dff_cnt + 3 * (size_t)S.nsup;
+  CK(cudaMalloc((void**)&dff.qhead, sizeof(int)));
+  if ((rc = upload(&dff.parent, S.sn_parent))) return rc;
+  if ((rc = upload(&dff.big_pos, fp.big_pos))) return rc;
+  if ((rc = upload(&dff.tile_base, fp.tile_base))) return rc;
+  CK(cudaFuncSetAttribute(k_factor_df, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_SMEM_DOUBLES * 8));
+  int occ = 0;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_factor_df, DF_NT, (size_t)DF_SMEM_DOUBLES * 8));
+  dff_grid = nsm * std::max(1, occ);
+  dff_nsup4 = 4 * (size_t)S.nsup;
+  if (std::getenv("CB_DF_TRACE") && dff.ntask > 0) {
+    h_dff_tasks = fp.tasks;
+    CK(cudaMalloc((void**)&dff.trace, (size_t)dff.ntask * 10 * sizeof(unsigned long long)));
+    CK(cudaMemset(dff.trace, 0, (size_t)dff.ntask * 10 * sizeof(unsigned long long)));
   }
-  cb_tmark("ldl:   solve plan: dataflow solve tasks");
-  // dataflow factorisation plan (k_factor_df): level 0's small fronts keep their level-synchronous launch
-  // (no dependencies, ~10^5 tiny CTAs); everything else becomes queue tasks in level order.  Every task
-  // record carries the front's constants and the range of its child records, so a task starts with two
-  // dependent loads (record, child records) instead of walking the tree arrays.
-  {
-    std::vector<int> tk;       // 16 ints per task
-    std::vector<int> desc;     // 12 ints per child record
-    std::vector<int> cnt_init(4 * (size_t)S.nsup, 0);   // [pend | diag_done | rows_left | tiles_left]
-    int* pend = cnt_init.data();
-    int* rows_left = cnt_init.data() + 2 * (size_t)S.nsup;
-    int* tiles_left = cnt_init.data() + 3 * (size_t)S.nsup;
-    for (int s = 0; s < S.nsup; s++) {
-      const int p = S.sn_parent[s];
-      const bool presolved = (S.sn_level[s] == 0 && !is_big(s));
-      if (p >= 0 && !presolved && mine(s)) pend[p]++;   // sharded: another rank's front is complete before the top phase starts
-    }
-    auto push_task = [&](int kind, int s, int a, int b, int d0, int d1, int e0, int e1) {
-      const size_t o = tk.size();
-      tk.resize(o + 16, 0);
-      int* t = tk.data() + o;
-      t[0] = kind; t[1] = s; t[2] = a; t[3] = b;
-      t[4] = S.sn_first[s + 1] - S.sn_first[s];
-      t[5] = (int)(S.sn_rowptr[s + 1] - S.sn_rowptr[s]);
-      t[6] = S.sn_first[s];
-      t[7] = d0; t[8] = d1; t[9] = e0; t[10] = e1;
-      const long long po = S.panel_off[s], uo = S.upd_off[s];
-      std::memcpy(t + 12, &po, 8);
-      std::memcpy(t + 14, &uo, 8);
-    };
-    auto push_desc = [&](int c, int a0, int a1, int b0, int b1) {
-      const size_t o = desc.size();
-      desc.resize(o + 12, 0);
-      int* t = desc.data() + o;
-      const long long uo = S.upd_off[c], rp = S.sn_rowptr[c];
-      std::memcpy(t, &uo, 8);
-      std::memcpy(t + 2, &rp, 8);
-      t[4] = (int)(S.sn_rowptr[c + 1] - S.sn_rowptr[c]);
-      t[5] = a0; t[6] = a1; t[7] = b0; t[8] = b1;
-      const int* rl = S.rel.data() + rp;
-      const bool rc_ = rl[a1 - 1] - rl[a0] == a1 - 1 - a0, cc_ = rl[b1 - 1] - rl[b0] == b1 - 1 - b0;
-      t[9] = (rc_ ? 1 : 0) | (cc_ ? 2 : 0);
-      t[10] = rl[a0];
-      t[11] = rl[b0];
-    };
-    // sharded: tasks of the owned subtrees first, then the tasks of the top part; nothing for other ranks' fronts
-    std::vector<int> kidsbuf, tp;
-    for (int ph = 0; ph < (sharded() ? 2 : 1); ph++) {
-    if (ph == 1) dff_ntask_owned = (int)(tk.size() / 16);
-    std::vector<std::vector<int>> lev(S.nlevels);
-    for (int s = 0; s < S.nsup; s++) {
-      if (sharded() && (ph == 0 ? !owned(s) : shard.owner[s] >= 0)) continue;
-      lev[S.sn_level[s]].push_back(s);
-    }
-    for (int l = 0; l < S.nlevels; l++) {
-      for (int s : lev[l]) if (!is_big(s) && l > 0) push_task(0, s, 0, 0, 0, 0, 0, 0);
-      // the children of a big front that go through child records (the small ones use the sorted entry lists)
-      auto heavy_kids = [&](int s) {
-        kidsbuf.clear();
-        for (int64_t ci = S.child_ptr[s]; ci < S.child_ptr[s + 1]; ci++) {
-          const int c = S.child_list[ci];
-          if (!small_child[c] && S.sn_rowptr[c + 1] > S.sn_rowptr[c]) kidsbuf.push_back(c);
-        }
-      };
-      for (int s : lev[l]) if (is_big(s)) {
-        heavy_kids(s);
-        const int d0 = (int)(desc.size() / 12);
-        for (int c : kidsbuf) if (h_child_nb[c] > 0) push_desc(c, 0, h_child_nb[c], 0, h_child_nb[c]);
-        push_task(1, s, 0, 0, d0, (int)(desc.size() / 12), h_sc_panel_ptr[big_pos[s]], h_sc_panel_ptr[big_pos[s] + 1]);
-      }
-      for (int s : lev[l]) if (is_big(s)) {
-        heavy_kids(s);
-        const int ns = S.sn_first[s + 1] - S.sn_first[s];
-        const int nr = (int)(S.sn_rowptr[s + 1] - S.sn_rowptr[s]);
-        const int nb = (nr + DF_RB - 1) / DF_RB;
-        rows_left[s] = nb;
-        for (int b = 0; b < nb; b++) {
-          const int g0 = ns + b * DF_RB, g1 = std::min(ns + nr, g0 + DF_RB);
-          const int d0 = (int)(desc.size() / 12);
-          for (int c : kidsbuf) {
-            if (h_child_nb[c] == 0) continue;
-            const int* rb = S.rel.data() + S.sn_rowptr[c];
-            const int* re = S.rel.data() + S.sn_rowptr[c + 1];
-            const int alo = (int)(std::lower_bound(rb, re, g0) - rb), ahi = (int)(std::lower_bound(rb, re, g1) - rb);
-            if (ahi > alo) push_desc(c, alo, ahi, 0, h_child_nb[c]);
-          }
-          push_task(2, s, b, 0, d0, (int)(desc.size() / 12), h_sc_panel_ptr[big_pos[s]], h_sc_panel_ptr[big_pos[s] + 1]);
-        }
-      }
-      for (int s : lev[l]) if (is_big(s)) {
-        heavy_kids(s);
-        const int ns = S.sn_first[s + 1] - S.sn_first[s];
-        const int nr = (int)(S.sn_rowptr[s + 1] - S.sn_rowptr[s]);
-        const int nt = (nr + TS - 1) / TS;
-        tiles_left[s] = nt * (nt + 1) / 2;
-        // per child: first child row of every tile row
-        std::vector<std::vector<int>> ctp(kidsbuf.size());
-        for (size_t k = 0; k < kidsbuf.size(); k++) {
-          const int c = kidsbuf[k];
-          const int* rb = S.rel.data() + S.sn_rowptr[c];
-          const int* re = S.rel.data() + S.sn_rowptr[c + 1];
-          ctp[k].resize(nt + 1);
-          for (int t = 0; t <= nt; t++) ctp[k][t] = (int)(std::lower_bound(rb, re, ns + t * TS) - rb);
-        }
-        // the children that reach tile (ti, tj), in child order: bucketed per tile from each child's own tile rows
-        // (a front under hundreds of children and with hundreds of tile rows -- the linking block of a
-        // block-angular problem -- would otherwise test every child against every tile)
-        const int ntile = nt * (nt + 1) / 2;
-        std::vector<int> tile_ptr(ntile + 1, 0), tile_kid;
-        {
-          std::vector<std::vector<int>> trows(kidsbuf.size());
-          for (size_t k = 0; k < kidsbuf.size(); k++)
-            for (int t = 0; t < nt; t++) if (ctp[k][t + 1] > ctp[k][t]) trows[k].push_back(t);
-          for (size_t k = 0; k < kidsbuf.size(); k++)
-            for (size_t a = 0; a < trows[k].size(); a++)
-              for (size_t b = 0; b <= a; b++) tile_ptr[trows[k][a] * (trows[k][a] + 1) / 2 + trows[k][b] + 1]++;
-          for (int t = 0; t < ntile; t++) tile_ptr[t + 1] += tile_ptr[t];
-          tile_kid.resize(tile_ptr[ntile]);
-          std::vector<int> pos(tile_ptr.begin(), tile_ptr.end() - 1);
-          for (size_t k = 0; k < kidsbuf.size(); k++)
-            for (size_t a = 0; a < trows[k].size(); a++)
-              for (size_t b = 0; b <= a; b++) tile_kid[pos[trows[k][a] * (trows[k][a] + 1) / 2 + trows[k][b]]++] = (int)k;
-        }
-        for (int ti = 0; ti < nt; ti++)
-          for (int tj = 0; tj <= ti; tj++) {
-            const int d0 = (int)(desc.size() / 12);
-            // children whose block is contiguous in the tile go first: the tile task adds them in registers
-            int ndense = 0;
-            const int tix = ti * (ti + 1) / 2 + tj;
-            for (int pass = 0; pass < 2; pass++)
-              for (int q = tile_ptr[tix]; q < tile_ptr[tix + 1]; q++) {
-                const size_t k = (size_t)tile_kid[q];
-                const int a0 = ctp[k][ti], a1 = ctp[k][ti + 1], b0 = ctp[k][tj], b1 = ctp[k][tj + 1];
-                if (!(a1 > a0 && b1 > b0)) continue;
-                const int* rl = S.rel.data() + S.sn_rowptr[kidsbuf[k]];
-                const bool dense = rl[a1 - 1] - rl[a0] == a1 - 1 - a0 && rl[b1 - 1] - rl[b0] == b1 - 1 - b0;
-                if (dense != (pass == 0)) continue;
-                push_desc(kidsbuf[k], a0, a1, b0, b1);
-                if (dense) ndense++;
-              }
-            const int t = tile_base[s] + ti * (ti + 1) / 2 + tj;
-            push_task(3, s, ti, tj, d0, (int)(desc.size() / 12), h_sc_tile_ptr[t], h_sc_tile_ptr[t + 1]);
-            tk[tk.size() - 16 + 11] = ndense;
-          }
-      }
-    }
-    }
-    cb_tmark("ldl:   solve plan: factor tasks built");
-    if (std::getenv("CB_TIMING")) std::fprintf(stderr, "[cb timing]     factor plan: %zu tasks, %zu child records, %d big fronts, %d tiles\n",
-                                                tk.size() / 16, desc.size() / 12, nbig, ntiles);
-    dff.ntask = (int)(tk.size() / 16);
-    if (!sharded()) dff_ntask_owned = dff.ntask;
-    int4* t4 = nullptr;
-    CK(cudaMalloc((void**)&t4, (tk.size() ? tk.size() : 16) * sizeof(int)));
-    if (!tk.empty()) CK(cudaMemcpy(t4, tk.data(), tk.size() * sizeof(int), cudaMemcpyHostToDevice));
-    dff.tasks = t4;
-    int* t1 = nullptr;
-    if ((rc = upload(&t1, desc))) return rc; dff.desc = t1;
-    if ((rc = upload(&t1, cnt_init))) return rc; d_dff_init = t1;
-    CK(cudaMalloc((void**)&d_dff_cnt, cnt_init.size() * sizeof(int) + 16));
-    dff.pend = d_dff_cnt; dff.diag_done = d_dff_cnt + S.nsup; dff.rows_left = d_dff_cnt + 2 * (size_t)S.nsup;
-    dff.tiles_left = d_dff_cnt + 3 * (size_t)S.nsup;
-    CK(cudaMalloc((void**)&dff.qhead, sizeof(int)));
-    if ((rc = upload(&t1, S.sn_parent))) return rc; dff.parent = t1;
-    if ((rc = upload(&t1, big_pos))) return rc; dff.big_pos = t1;
-    if ((rc = upload(&t1, tile_base))) return rc; dff.tile_base = t1;
-    CK(cudaFuncSetAttribute(k_factor_df, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_SMEM_DOUBLES * 8));
-    int nsm = 0, occ = 0;
-    CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_factor_df, DF_NT, (size_t)DF_SMEM_DOUBLES * 8));
-    dff_grid = nsm * std::max(1, occ);
-    dff_nsup4 = 4 * (size_t)S.nsup;
-    if (std::getenv("CB_DF_TRACE") && dff.ntask > 0) {
-      h_dff_tasks = tk;
-      CK(cudaMalloc((void**)&dff.trace, (size_t)dff.ntask * 10 * sizeof(unsigned long long)));
-      CK(cudaMemset(dff.trace, 0, (size_t)dff.ntask * 10 * sizeof(unsigned long long)));
-    }
+
+  // dataflow solves (ldl_solve.cuh)
+  const int nt = (int)sp.tasks.size();
+  sv_nwide = (int)sp.wide.size();
+  sv_wide_runs = std::move(sp.wide_runs);
+  sv_nleaf1 = (int)sp.leaf1.size(); sv_nleafn = (int)sp.leafn.size(); sv_nleafw = (int)sp.leafw.size();
+  sv_leafw_nrmax = sp.leafw_nrmax;
+  sv_leafw_grid = sv_nleafw;      // one CTA per front (a loop over fronts inside fewer CTAs was slower: 312 vs 189 us forward on C4)
+  sv_ntask_owned = sp.ntask_owned;
+  if ((rc = upload(&dev.gat_ptr, sp.gat_ptr))) return rc;
+  if ((rc = upload(&dev.gat_src, sp.gat_src))) return rc;
+  if ((rc = upload(&d_sv_wide, sp.wide))) return rc;
+  if ((rc = upload(&d_sv_leaf1, sp.leaf1))) return rc;
+  if ((rc = upload(&d_sv_leafn, sp.leafn))) return rc;
+  if ((rc = upload(&d_sv_leafw, sp.leafw))) return rc;
+  if ((rc = upload(&sv.fronts, sp.fronts))) return rc;
+  if ((rc = upload(&sv.front2task, sp.front2task))) return rc;
+  if ((rc = upload(&sv.parent, S.sn_parent))) return rc;
+  if ((rc = upload(&sv.tasks, sp.tasks))) return rc;
+  // counters: [pend(nt) | fleft(nsup) | bleft(nsup)] are copied from their initial values before every solve,
+  // [tdone(nt) | ydone(nsup) | done(nsup) | qhead(2)] are cleared
+  sv_ninit = sp.cnt_init.size();
+  sv_nzero = (size_t)nt + 2 * (size_t)S.nsup + 2;
+  if ((rc = upload(&d_sv_init, sp.cnt_init))) return rc;
+  CK(cudaMalloc((void**)&d_sv_cnt, (sv_ninit + sv_nzero) * sizeof(int)));
+  sv.pend = d_sv_cnt; sv.fleft = d_sv_cnt + nt; sv.bleft = sv.fleft + S.nsup;
+  sv.tdone = d_sv_cnt + sv_ninit; sv.ydone = sv.tdone + nt; sv.done = sv.ydone + S.nsup; sv.qhead = sv.done + S.nsup;
+  sv.bpart_stride = (long long)(sp.nslots ? sp.nslots : 1) * CB_PB_MAXNS;
+  CK(cudaMalloc((void**)&sv.bpart, (size_t)2 * sv.bpart_stride * sizeof(double)));
+  sv.ntask = nt;
+  // launch geometry: dynamic shared memory = slab + vectors for one or two right-hand sides
+  for (int nr2 = 1; nr2 <= 2; nr2++)
+    sv_smem[nr2 - 1] = ((size_t)sv_cap + 2 + (size_t)nr2 * (2 * CB_PB_MAXNS + SV_MAXROWS + 4 * CB_PB_MAXNS)) * sizeof(double);
+  if ((rc = sv_configure())) return rc;
+  const int sv_occ = sv_occupancy();
+  if (sv_occ < 1) return CLDL_E_CUDA;
+  sv_grid = nsm * sv_occ;
+  use_dataflow = true;
+  if (std::getenv("CB_DF_TRACE_SOLVE") && nt > 0) {
+    CK(cudaMalloc((void**)&sv.trace, (size_t)nt * 8 * sizeof(unsigned long long)));
+    CK(cudaMemset(sv.trace, 0, (size_t)nt * 8 * sizeof(unsigned long long)));
+    h_sv_tasks = sp.tasks;
   }
-  cb_tmark("ldl: solve plan");
+  if (std::getenv("CB_TIMING") != nullptr) std::fprintf(stderr, "[cb timing]     solve plan: %d tasks (%d leaf columns, %d narrow leaves, %d wide leaves, %d wide fronts, %d row slabs), slab %d doubles, %d CTAs\n",
+                                   nt, sv_nleaf1, sv_nleafn, sv_nleafw, sv_nwide, sp.nslots, sv_cap, sv_grid);
+  cb_tmark("ldl: plan uploads");
   if (sharded()) {
     d_shard_xidx.assign(shard_nranks, nullptr);
     for (int w = 0; w < 2; w++) { d_shard_segs[w].assign(shard_nranks, nullptr); shard_nsegs[w].assign(shard_nranks, 0); }
-    for (int g = 0; g < shard_nranks; g++) { int* t1 = nullptr; if ((rc = upload(&t1, shard_xidx[g]))) return rc; d_shard_xidx[g] = t1; }
+    for (int g = 0; g < shard_nranks; g++) { int* t1 = nullptr; if ((rc = upload(&d_shard_xidx[g], shard_xidx[g]))) return rc; }
   }
   if (big_alloc.joinable()) big_alloc.join();
   if (big_alloc_rc) { std::fprintf(stderr, "[clarabel_b200] device allocation of the factor storage failed\n"); return CLDL_E_CUDA; }
@@ -1719,7 +1243,7 @@ void LDLObject::release() {
   fr(dev.rel); fr(dev.panel_off); fr(dev.upd_off); fr(dev.asm_ptr); fr(dev.asm_src);
   fr(dev.asm_dst); fr(dev.level_tasks); fr(dev.perm); fr(dev.dsigns); fr(dev.vals); fr(dev.L);
   fr(dev.U); fr(dev.D); fr(dev.Dinv); fr(dev.u); fr(dev.status); fr(d_xp); fr(d_bx);
-  fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_wide); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.desc); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
+  fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_wide); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.recs); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
   if (h_status) cudaFreeHost(h_status);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
@@ -1781,7 +1305,7 @@ int LDLObject::sync_status() {
     if (FILE* fp = std::fopen(std::getenv("CB_DF_TRACE"), "wb")) {
       const long long nt = dff.ntask;
       std::fwrite(&nt, sizeof(nt), 1, fp);
-      std::fwrite(h_dff_tasks.data(), sizeof(int), (size_t)nt * 16, fp);
+      std::fwrite(h_dff_tasks.data(), sizeof(DFTask), (size_t)nt, fp);
       std::fwrite(tr.data(), sizeof(unsigned long long), tr.size(), fp);
       std::fclose(fp);
     }
@@ -2234,7 +1758,7 @@ int cldl_solve(cldl_t* h, double* x, const double* b) {
     cudaMemcpy(tr.data(), o.sv.trace, tr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost);
     if (FILE* fp = std::fopen(std::getenv("CB_DF_TRACE_SOLVE"), "wb")) {
       std::fwrite(&nt, sizeof(nt), 1, fp);
-      std::fwrite(o.h_sv_tasks.data(), sizeof(int), (size_t)nt * 24, fp);
+      std::fwrite(o.h_sv_tasks.data(), sizeof(cb::SVTask), (size_t)nt, fp);
       std::fwrite(tr.data(), sizeof(unsigned long long), tr.size(), fp);
       std::fclose(fp);
     }

@@ -8,14 +8,11 @@
 
 #include "../../include/clarabel_b200.h"
 #include "symbolic.h"
+#include "ldl_plan.h"
 #include "ldl_solve_plan.h"
 
 #define CB_MAX_PANEL 128
-#define CB_PB_MAXNS 64     /* widest panel (columns) of a front */
 #define CB_PB_LD 66        /* padded leading dimension of the pivot block in shared memory */
-#define CB_SOLVE_SMALL_NS 8 /* solves: fronts with at most this many pivots get one warp, wider ones one CTA */
-#define CB_SMALL_CHILD 16  /* children of big fronts with at most this many rows go through sorted entry lists */
-#define CB_BIG_NR 96       /* fronts with at least this many rows below the pivot block are factored by D, R and T tasks */
 
 namespace cb {
 
@@ -54,18 +51,11 @@ struct LDLDev {
   int reg_enable = 1;
 };
 
-// one launch of the level-0 factorisation over level_tasks[base, base + count): k_factor_leaf1 (single-column fronts,
-// one thread each) or k_factor_level<threads> with smem_doubles of dynamic shared memory
-struct LaunchSeg {
-  bool leaf1;
-  int base, count, smem_doubles, threads;
-};
-
 // dataflow factorisation plan (see k_factor_df in ldl.cu)
 struct DFFactor {
   int ntask = 0;
-  const int4* tasks = nullptr;      // 4 x int4 per task: see DFTask in ldl.cu
-  const int* desc = nullptr;        // 12 ints per child record
+  const int4* tasks = nullptr;      // 4 x int4 per task: DFTask
+  const DFChildRec* recs = nullptr;
   int* pend = nullptr;              // [nsup] children still running
   int* diag_done = nullptr;         // [nsup]
   int* rows_left = nullptr;         // [nsup]
@@ -85,7 +75,7 @@ class LDLObject {
   int *d_sv_init = nullptr, *d_sv_cnt = nullptr, *d_sv_wide = nullptr, *d_sv_leaf1 = nullptr, *d_sv_leafn = nullptr, *d_sv_leafw = nullptr;
   size_t sv_ninit = 0, sv_nzero = 0, sv_smem[2] = {0, 0};
   int sv_cap = 0, sv_nwide = 0, sv_nleaf1 = 0, sv_nleafn = 0, sv_nleafw = 0, sv_leafw_nrmax = 0, sv_leafw_grid = 1, sv_ntask_owned = 0;
-  std::vector<int> h_sv_tasks;
+  std::vector<SVTask> h_sv_tasks;
   std::vector<int> sv_wide_runs;   // (first, widest ns) pairs of the launches of k_invert_pivots, closed by (count, 0)
   int sv_configure();
   int sv_occupancy();
@@ -95,7 +85,7 @@ class LDLObject {
   void invert_pivots();
   DFFactor dff;
   int *d_dff_init = nullptr, *d_dff_cnt = nullptr;
-  std::vector<int> h_dff_tasks;
+  std::vector<DFTask> h_dff_tasks;
   int dff_grid = 0;
   size_t dff_nsup4 = 0;
   int sv_grid = 0;                  // CTAs of a sweep kernel (as many as can be co-resident)
@@ -136,8 +126,6 @@ class LDLObject {
   int h_phase_start[2] = {0, 0};         // pinned-lifetime host copies of the queue heads the top phases start from
   uint64_t shard_count_owned[2] = {0, 0};    // regularize_count / positive_inertia of the owned phase
   bool sharded() const { return shard_nranks > 1; }
-  bool mine(int s) const { return !sharded() || shard.owner[s] == shard_rank || shard.owner[s] < 0; }
-  bool owned(int s) const { return !sharded() || shard.owner[s] == shard_rank; }
   int refactor_phase_async(int phase);   // 0: owned subtrees, 1: top part (after the cut roots' update matrices arrived)
   int solve_phase_async(double* d_x, const double* d_b, int phase);   // 0: permute + forward owned, 1: forward top + backward
   // what: 0 update matrices of the cut roots (per refactor), 1 their update vectors (per solve), 2 x entries

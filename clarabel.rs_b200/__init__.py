@@ -720,7 +720,9 @@ CONE_CODES = {"zero": 0, "nonneg": 1, "soc": 2, "psd": 3, "exp": 4, "pow": 5, "g
 SCALING_PRIMAL_DUAL, SCALING_DUAL = 0, 1
 STATUS_NAMES = ["Unsolved", "Solved", "PrimalInfeasible", "DualInfeasible", "AlmostSolved",
                 "AlmostPrimalInfeasible", "AlmostDualInfeasible", "MaxIterations", "MaxTime",
-                "NumericalError", "InsufficientProgress"]
+                "NumericalError", "InsufficientProgress", "CallbackTerminated"]
+# cipm_set_print_target kinds (print_to_stdout / _sink / _buffer / _file / _stream)
+PRINT_STDOUT, PRINT_SINK, PRINT_BUFFER, PRINT_FILE, PRINT_STREAM = 0, 1, 2, 3, 4
 
 
 class cipm_settings(C.Structure):
@@ -746,6 +748,7 @@ class cipm_settings(C.Structure):
         ("iterative_refinement_stop_ratio", C.c_double),
         ("linesearch_backtrack_step", C.c_double), ("min_switch_step_length", C.c_double),
         ("presolve_enable", C.c_int32),
+        ("verbose", C.c_int32),
     ]
 
 
@@ -768,6 +771,12 @@ class cipm_info(C.Structure):
         return STATUS_NAMES[self.status]
 
 
+# cipm_callback_fn: int (*)(const cipm_info* info, void* user_data); nonzero = stop
+CALLBACK_FN = C.CFUNCTYPE(C.c_int, C.POINTER(cipm_info), C.c_void_p)
+# cipm_write_fn: int (*)(void* ctx, const char* buf, uint64_t len)
+WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_uint64)
+
+
 EXPORTED_SYMBOLS += [
     "cipm_default_settings", "cipm_create", "cipm_destroy", "cipm_solve", "cipm_get_info",
     "cipm_get_solution", "cipm_trace", "cipm_iter_ms", "cipm_launch_count", "cipm_time_ms", "cipm_kkt_dim", "cipm_kkt_nnz", "cipm_get_kkt",
@@ -779,7 +788,8 @@ EXPORTED_SYMBOLS += [
     "ccone_affine_ds_ex", "ccone_compute_barrier", "cipm_m_reduced", "cipm_get_equilibration", "cipm_get_infinity", "cipm_set_infinity", "cipm_default_infinity", "cipm_test_spmv", "cipm_test_vec", "cipm_create_gp",
     "cldl_shard_refactor_phase_dev", "cldl_shard_solve_phase_dev", "cldl_shard_count", "cldl_shard_pack_dev",
     "cldl_shard_unpack_dev", "cldl_shard_counts", "cipm_abi_sizes", "cldl_set_transport", "cipm_set_transport",
-    "cldl_copy_dev", "cipm_update_settings",
+    "cldl_copy_dev", "cipm_update_settings", "cipm_set_termination_callback", "cipm_unset_termination_callback",
+    "cipm_set_print_target", "cipm_get_print_buffer",
 ]
 
 _l2_ready = False
@@ -853,6 +863,11 @@ def _lib2():
     L.ccone_step_length.argtypes = [vp, f64p, f64p, f64p, f64p, C.c_double, f64p]
     L.ccone_margins.argtypes = [vp, f64p, f64p, f64p]
     L.ccone_scaled_unit_shift.argtypes = [vp, f64p, C.c_double, C.c_int]
+    L.cipm_set_termination_callback.argtypes = [vp, CALLBACK_FN, vp]
+    L.cipm_unset_termination_callback.argtypes = [vp]
+    L.cipm_set_print_target.argtypes = [vp, C.c_int, C.c_char_p, WRITE_FN, vp]
+    L.cipm_get_print_buffer.argtypes = [vp, C.c_char_p, C.c_uint64]
+    L.cipm_get_print_buffer.restype = C.c_int64
     _l2_ready = True
     return L
 
@@ -874,20 +889,27 @@ class CudaSolver:
     {"zero", "nonneg", "soc", "psd"}, ("exp", 3) for an ExponentialConeT(),
     ("pow", alpha) for a PowerConeT(alpha) and ("genpow", (alphas, dim2)) for a
     GenPowerConeT(alphas, dim2).
+
+    With ``shard=(nranks, rank)``, ranks other than 0 run with ``verbose`` off, so that one table is printed per
+    solve; ``print_all_ranks=True`` leaves every rank's setting as given.
     """
 
     def __init__(self, P, q, A, b, cones, settings=None, *, ordering=ORDER_BEST, kkt_perm=None,
-                 device=0, max_panel=0, nd_leaf=0, shard=None, transport=None):
+                 device=0, max_panel=0, nd_leaf=0, shard=None, transport=None, print_all_ranks=False):
         import scipy.sparse as sp
         L = _lib2()
         self._L = L
+        self._callback = None        # ctypes objects the library holds pointers to: alive while installed
+        self._print_fn = None
+        self._pending_exc = None     # an exception raised inside a callback or a stream write, re-raised by solve()
+        self._quiet_rank = shard is not None and int(shard[1]) != 0 and not print_all_ranks
         P, A = sp.csc_matrix(P), sp.csc_matrix(A)
         check_dimensions(P, q, A, b, cones)
         P = sp.triu(P, format="csc")
         P.sort_indices()
         A.sort_indices()
         self.n, self.m = P.shape[0], A.shape[0]
-        self.settings = settings if settings is not None else default_settings()
+        self.settings = self._rank_settings(settings if settings is not None else default_settings())
         o = cldl_opts()
         L.cldl_default_opts(C.byref(o))
         o.ordering, o.device, o.max_panel, o.nd_leaf = ordering, device, max_panel, nd_leaf
@@ -955,8 +977,78 @@ class CudaSolver:
         s = cipm_settings.from_buffer_copy(self.settings)
         for k, v in kw.items():
             setattr(s, k, v)
+        s = self._rank_settings(s)
         _check(self._L.cipm_update_settings(self._h, C.byref(s)), "cipm_update_settings")
         self.settings = s
+
+    def _rank_settings(self, s):
+        if self._quiet_rank and s.verbose:
+            s = cipm_settings.from_buffer_copy(s)
+            s.verbose = 0
+        return s
+
+    # ---- termination callback (core/solver.rs: set_termination_callback / _c, unset_termination_callback) ----
+    def set_termination_callback(self, fn):
+        """`fn(info) -> bool` is called once per pass of the iteration loop with a copy of the current `cipm_info`;
+        True ends the solve with status CallbackTerminated.  An exception raised by `fn` ends the solve too, and
+        solve() raises it.  On a sharded solver every rank installs its own callback."""
+        def call(pinfo, _user_data):
+            try:
+                return 1 if fn(cipm_info.from_buffer_copy(pinfo.contents)) else 0
+            except BaseException as e:         # never let an exception cross the C boundary
+                if self._pending_exc is None:
+                    self._pending_exc = e
+                return 1
+        self.set_termination_callback_c(CALLBACK_FN(call))
+
+    def set_termination_callback_c(self, cfn, user_data=None):
+        """a C callback: a `CALLBACK_FN` (int (*)(const cipm_info*, void*)) and the pointer handed to it"""
+        _check(self._L.cipm_set_termination_callback(self._h, cfn, user_data), "cipm_set_termination_callback")
+        self._callback = (cfn, user_data)
+
+    def unset_termination_callback(self):
+        _check(self._L.cipm_unset_termination_callback(self._h), "cipm_unset_termination_callback")
+        self._callback = None
+
+    # ---- print targets (io/mod.rs: ConfigurablePrintTarget); output only appears with settings.verbose ----
+    def _set_print(self, kind, path=None, fn=None):
+        _check(self._L.cipm_set_print_target(self._h, kind, path, fn if fn is not None else WRITE_FN(), None),
+               "cipm_set_print_target")
+        self._print_fn = fn
+
+    def print_to_stdout(self):
+        self._set_print(PRINT_STDOUT)
+
+    def print_to_file(self, path):
+        """append the output to the file at `path`"""
+        self._set_print(PRINT_FILE, path=os.fsencode(path))
+
+    def print_to_stream(self, stream):
+        """hand the output to `stream.write(str)`"""
+        def write(_ctx, buf, n):
+            try:
+                stream.write(C.string_at(buf, n).decode("utf-8", "replace"))
+                return 0
+            except BaseException as e:
+                if self._pending_exc is None:
+                    self._pending_exc = e
+                return -1
+        self._set_print(PRINT_STREAM, fn=WRITE_FN(write))
+
+    def print_to_sink(self):
+        self._set_print(PRINT_SINK)
+
+    def print_to_buffer(self):
+        """collect the output in the solver (a fresh, empty buffer); read it with get_print_buffer()"""
+        self._set_print(PRINT_BUFFER)
+
+    def get_print_buffer(self):
+        n = int(self._L.cipm_get_print_buffer(self._h, None, 0))
+        if n < 0:
+            raise BackendError("Print buffering is not configured.")
+        buf = C.create_string_buffer(max(n, 1))
+        self._L.cipm_get_print_buffer(self._h, buf, n)
+        return buf.raw[:n].decode("utf-8", "replace")
 
     def is_data_update_allowed(self):
         """DefaultSolver::is_data_update_allowed (data_updating.rs:165-180): not while the presolver has removed rows"""
@@ -1016,7 +1108,12 @@ class CudaSolver:
             pass
 
     def solve(self):
-        _check(self._L.cipm_solve(self._h), "cipm_solve")
+        self._pending_exc = None
+        rc = self._L.cipm_solve(self._h)
+        exc, self._pending_exc = self._pending_exc, None
+        if exc is not None:
+            raise exc
+        _check(rc, "cipm_solve")
         info = cipm_info()
         self._L.cipm_get_info(self._h, C.byref(info))
         x, z, s = np.zeros(max(self.n, 1)), np.zeros(max(self.m, 1)), np.zeros(max(self.m, 1))

@@ -1488,6 +1488,7 @@ int LDLObject::set_nccl(const char* libpath, const unsigned char* id128, int nra
   const int r = a->CommInitRank(&c, nranks, id, rank);
   if (r != 0) { std::fprintf(stderr, "[clarabel_b200] ncclCommInitRank: %s\n", a->GetErrorString ? a->GetErrorString(r) : "error"); return CLDL_E_CUDA; }
   nccl_comm = c;
+  nccl_allgather = a->AllGather; nccl_error = a->GetErrorString;
   return CLDL_OK;
 }
 
@@ -1504,15 +1505,7 @@ int LDLObject::exchange(int what, double* d_x) {
   }
   int rc = shard_pack(what, d_xsend, d_x);
   if (rc) return rc;
-  if (nccl_comm) {      // stream-ordered: the unpack kernels below simply follow the collective on `stream`
-    NcclApi* a = nccl_api(nullptr);
-    const int r = a->AllGather(d_xsend, d_xrecv, (size_t)cnt, /* ncclFloat64 */ 8, (cb_ncclComm_t)nccl_comm, stream);
-    if (r != 0) { std::fprintf(stderr, "[clarabel_b200] ncclAllGather: %s\n", a->GetErrorString ? a->GetErrorString(r) : "error"); return CLDL_E_CUDA; }
-    n_collectives++;
-  } else {
-    CK(cudaStreamSynchronize(stream));
-    if (transport(transport_ctx, d_xsend, d_xrecv, cnt) != 0) return CLDL_E_CUDA;
-  }
+  if ((rc = allgather(d_xsend, d_xrecv, cnt))) return rc;
   for (int r = 0; r < shard_nranks; r++)
     if (r != shard_rank && (rc = shard_unpack(what, r, d_xrecv + (size_t)r * cnt, d_x))) return rc;
   return CLDL_OK;

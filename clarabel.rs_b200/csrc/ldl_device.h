@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <cstdio>
 #include <thread>
 #include <vector>
 
@@ -15,6 +16,8 @@
 #define CB_PB_LD 66        /* padded leading dimension of the pivot block in shared memory */
 
 namespace cb {
+
+struct ncclComm;   // NCCL's communicator, opaque (ldl.cu loads NCCL with dlopen)
 
 enum { ST_REGCOUNT = 0, ST_ZEROPIV = 1, ST_POSINERTIA = 2, ST_NONFINITE = 3, ST_COUNT = 8 };
 
@@ -142,6 +145,21 @@ class LDLObject {
   double *d_xsend = nullptr, *d_xrecv = nullptr;
   size_t xbuf_cap = 0;
   int exchange(int what, double* d_x);
+  // the communicator's ncclAllGather / ncclGetErrorString, taken by set_nccl from the NCCL library it loaded
+  int (*nccl_allgather)(const void*, void*, size_t, int, ncclComm*, cudaStream_t) = nullptr;
+  const char* (*nccl_error)(int) = nullptr;
+  // one all-gather of `cnt` doubles per rank between device buffers through the installed transport; defined here
+  // rather than in ldl.cu because the interior-point driver uses it too (the sharded termination-callback verdicts)
+  int allgather(const double* d_send, double* d_recv, uint64_t cnt) {
+    if (nccl_comm) {      // stream-ordered: whatever follows on `stream` simply follows the collective
+      const int r = nccl_allgather(d_send, d_recv, (size_t)cnt, /* ncclFloat64 */ 8, (ncclComm*)nccl_comm, stream);
+      if (r != 0) { std::fprintf(stderr, "[clarabel_b200] ncclAllGather: %s\n", nccl_error ? nccl_error(r) : "error"); return CLDL_E_CUDA; }
+      n_collectives++;
+      return CLDL_OK;
+    }
+    if (cudaStreamSynchronize(stream) != cudaSuccess) return CLDL_E_CUDA;
+    return transport(transport_ctx, d_send, d_recv, cnt) != 0 ? CLDL_E_CUDA : CLDL_OK;
+  }
   int refactor_sharded();
   int solve_sharded(double* d_x, const double* d_b);
 

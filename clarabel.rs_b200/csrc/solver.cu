@@ -25,6 +25,7 @@
 
 #include "../../include/clarabel_b200.h"
 #include "cones.h"
+#include "ipm_print.h"
 #include "ldl_device.h"
 #include "vec.cuh"
 
@@ -595,7 +596,7 @@ int KKTDevice::solve2(double* ax, double* az, double* bx, double* bz) {
 
 // ------------------------------------------------------------------ the IPM
 enum { IST_UNSOLVED = 0, IST_SOLVED, IST_PINF, IST_DINF, IST_ALMOST_SOLVED, IST_ALMOST_PINF, IST_ALMOST_DINF,
-       IST_MAXIT, IST_MAXTIME, IST_NUMERR, IST_INSUFF };
+       IST_MAXIT, IST_MAXTIME, IST_NUMERR, IST_INSUFF, IST_CALLBACK };
 
 class IPM {
  public:
@@ -633,6 +634,13 @@ class IPM {
   std::vector<cudaEvent_t> iter_ev;   // one event at the start of every iteration
   std::vector<double> iter_ms;        // ms since the start of solve()
   int n_iter_ev = 0;
+  // termination callback and verbose output (core/solver.rs:297-313, default/info_print.rs)
+  cipm_callback_fn cb_fn = nullptr;
+  void* cb_data = nullptr;
+  double* d_verdict = nullptr;   // sharded: [this rank's verdict, every rank's verdict] on the device ...
+  double* h_verdict = nullptr;   // ... and its pinned host mirror
+  PrintTarget out;
+  PrintSetup psetup;
 
   int init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const double* Pxv, const double* q_,
            const uint64_t* Ap, const uint64_t* Ai, const double* Axv, const double* b_, uint64_t ncones,
@@ -661,6 +669,7 @@ class IPM {
   int shift_to_interior(double* v, bool primal);
   int step_length(bool combined, double* alpha, int scaling = SCALING_PRIMAL_DUAL);
   int variables_barrier(double a, double* out);
+  int report_pass(bool verbose, bool* stop);
 };
 
 void IPM::equilibrate() {
@@ -959,6 +968,17 @@ int IPM::init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const doub
   info.nnzK = (uint64_t)kkt.nnzK;
   info.nnzL = (uint64_t)kkt.ldl.S.nnzL_simplicial;
   info.kkt_dim = (uint64_t)kkt.N;
+  // what the verbose configuration block reports (info_print.rs: print_configuration / print_settings)
+  psetup.n = n; psetup.m = m; psetup.nnzP = P.colptr[n]; psetup.nnzA = A.colptr[n];
+  psetup.presolve_removed = mfull - m;
+  psetup.cones.clear();
+  for (const ConeSpec& c : cones.cones) psetup.cones.emplace_back(c.type, (int64_t)c.dim);
+#ifdef CB_EMU   /* host build of the test suite (tests/emu): no device to name */
+  psetup.device = "CUDA-on-CPU emulator";
+#else
+  cudaDeviceProp prop;
+  if (cudaGetDeviceProperties(&prop, lo.device) == cudaSuccess) psetup.device = prop.name;
+#endif
   return 0;
 }
 
@@ -974,6 +994,8 @@ void IPM::release() {
                          (const void*)tmpn})
     dfree(p_);
   for (auto ev : iter_ev) cudaEventDestroy(ev);
+  dfree(d_verdict);
+  if (h_verdict) cudaFreeHost(h_verdict);
   cones.release();
   sc.release();
   kkt.release();
@@ -1228,6 +1250,9 @@ int IPM::solve() {
   kkt.n_refactor = kkt.n_ldl_solve = kkt.n_ir_steps = 0;
   trace.clear();
   cudaEvent_t e0 = kkt.ldl.ev0, e1 = kkt.ldl.ev1;
+  // printing and the termination callback only read host copies of the info: with both off a pass costs one branch
+  const bool verbose = set.verbose != 0, hooks = verbose || cb_fn != nullptr;
+  if (verbose) out.write(print_banner() + print_configuration(psetup, set) + print_header());
   SCK(cudaEventRecord(e0, st));
 
   // default start (core/solver.rs:525-541)
@@ -1258,6 +1283,11 @@ int IPM::solve() {
     info_update(t0);
     trace.resize((size_t)(iter + 1) * 6);     // one row per iteration; a strategy switch re-enters the same row
     { double* tr = trace.data() + (size_t)iter * 6; tr[0] = mu; tr[1] = alpha; tr[2] = sigma; tr[3] = info.res_primal; tr[4] = info.res_dual; tr[5] = info.gap_abs; }
+    if (hooks) {   // the row, then the user's termination check (core/solver.rs:297-313)
+      bool stop = false;
+      if ((rc = report_pass(verbose, &stop))) return rc;
+      if (stop) { info.status = IST_CALLBACK; break; }
+    }
     if (check_termination(iter)) {
       if (info.status == IST_INSUFF) {  // recover the previous iterate (core/solver.rs:586-611)
         info.cost_primal = prev_cost_primal; info.cost_dual = prev_cost_dual;
@@ -1319,7 +1349,10 @@ int IPM::solve() {
     V.axpby(z, alpha, lz, 1.0, m);
     tau += alpha * ltau; kap += alpha * lkap;
   }
-  if (alpha == 0.0) { info.mu = mu; info.step_length = alpha; info.sigma = sigma; info.iterations = (uint32_t)iter; }
+  if (alpha == 0.0) {   // no final step: the scalars are captured again, and printed once more (core/solver.rs:444-448)
+    info.mu = mu; info.step_length = alpha; info.sigma = sigma; info.iterations = (uint32_t)iter;
+    if (verbose) out.write(print_row(info));
+  }
   if (info.status == IST_NUMERR || info.status == IST_INSUFF || info.status == IST_MAXIT || info.status == IST_MAXTIME)
     check_convergence(set.reduced_tol_gap_abs, set.reduced_tol_gap_rel, set.reduced_tol_feas,
                       set.reduced_tol_infeas_abs, set.reduced_tol_infeas_rel, set.reduced_tol_ktratio,
@@ -1337,6 +1370,31 @@ int IPM::solve() {
   info.n_ldl_solve = (uint64_t)kkt.n_ldl_solve;
   info.n_ir_steps = (uint64_t)kkt.n_ir_steps;
   info.regularize_count = kkt.ldl.regularize_count;
+  if (verbose) out.write(print_footer(info));
+  return 0;
+}
+
+// One pass's row and the termination callback.  On a sharded solver every rank runs the same passes: the verdicts of
+// all ranks are all-gathered, and all stop when any asked to, so that no rank is left waiting in a collective.
+int IPM::report_pass(bool verbose, bool* stop) {
+  if (verbose) out.write(print_row(info));
+  *stop = false;
+  if (!cb_fn) return 0;
+  const bool mine = cb_fn(&info, cb_data) != 0;
+  LDLObject& L = kkt.ldl;
+  if (!L.sharded() || !L.has_transport()) { *stop = mine; return 0; }
+  const int R = L.shard_nranks;
+  if (!d_verdict) {
+    SCK(cudaMalloc((void**)&d_verdict, (size_t)(1 + R) * sizeof(double)));
+    SCK(cudaMallocHost((void**)&h_verdict, (size_t)(1 + R) * sizeof(double)));
+  }
+  h_verdict[0] = mine ? 1.0 : 0.0;
+  SCK(cudaMemcpyAsync(d_verdict, h_verdict, sizeof(double), cudaMemcpyHostToDevice, st));
+  int rc = L.allgather(d_verdict, d_verdict + 1, 1);
+  if (rc) return rc;
+  SCK(cudaMemcpyAsync(h_verdict + 1, d_verdict + 1, (size_t)R * sizeof(double), cudaMemcpyDeviceToHost, st));
+  SCK(cudaStreamSynchronize(st));
+  for (int r = 0; r < R; r++) *stop = *stop || h_verdict[1 + r] != 0.0;
   return 0;
 }
 
@@ -1369,6 +1427,7 @@ void cipm_default_settings(cipm_settings* s) {
   s->iterative_refinement_stop_ratio = 5.0;
   s->linesearch_backtrack_step = 0.8; s->min_switch_step_length = 0.1;
   s->presolve_enable = 1;
+  s->verbose = 0;   // the reference prints by default; a library call below other code stays silent unless asked
 }
 
 int cipm_create(cipm_t** out, uint64_t n, uint64_t m, const uint64_t* P_colptr, const uint64_t* P_rowval,
@@ -1467,6 +1526,29 @@ void cipm_destroy(cipm_t* h) {
 }
 
 int cipm_solve(cipm_t* h) { return h ? h->ipm.solve() : CLDL_E_ARG; }
+
+// set_termination_callback_c / unset_termination_callback (core/solver.rs); on a sharded handle every rank makes the
+// call, since a solve with a callback all-gathers every rank's verdict once per pass
+int cipm_set_termination_callback(cipm_t* h, cipm_callback_fn fn, void* user_data) {
+  if (!h || !fn) return CLDL_E_ARG;
+  h->ipm.cb_fn = fn; h->ipm.cb_data = user_data;
+  return CLDL_OK;
+}
+int cipm_unset_termination_callback(cipm_t* h) {
+  if (!h) return CLDL_E_ARG;
+  h->ipm.cb_fn = nullptr; h->ipm.cb_data = nullptr;
+  return CLDL_OK;
+}
+
+int cipm_set_print_target(cipm_t* h, int kind, const char* path, cipm_write_fn fn, void* ctx) {
+  return h ? h->ipm.out.set(kind, path, fn, ctx) : CLDL_E_ARG;
+}
+int64_t cipm_get_print_buffer(cipm_t* h, char* out, uint64_t cap) {
+  if (!h || h->ipm.out.kind != CIPM_PRINT_BUFFER) return CLDL_E_ARG;
+  const std::string& b = h->ipm.out.buffer;
+  if (out) std::memcpy(out, b.data(), std::min<uint64_t>(cap, b.size()));
+  return (int64_t)b.size();
+}
 
 void cipm_get_info(const cipm_t* h, cipm_info* out) { if (h && out) *out = h->ipm.info; }
 

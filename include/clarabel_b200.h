@@ -194,7 +194,8 @@ enum { CIPM_SCALING_PRIMAL_DUAL = 0, CIPM_SCALING_DUAL = 1 };
 /* SolverStatus (src/solver/core/traits.rs / default/info.rs) */
 enum { CIPM_UNSOLVED = 0, CIPM_SOLVED, CIPM_PRIMAL_INFEASIBLE, CIPM_DUAL_INFEASIBLE, CIPM_ALMOST_SOLVED,
        CIPM_ALMOST_PRIMAL_INFEASIBLE, CIPM_ALMOST_DUAL_INFEASIBLE, CIPM_MAX_ITERATIONS, CIPM_MAX_TIME,
-       CIPM_NUMERICAL_ERROR, CIPM_INSUFFICIENT_PROGRESS };
+       CIPM_NUMERICAL_ERROR, CIPM_INSUFFICIENT_PROGRESS,
+       CIPM_CALLBACK_TERMINATED   /* the termination callback asked to stop (SolverStatus::CallbackTerminated) */ };
 
 /* The fields of DefaultSettings the path reads (default/settings.rs:30-193),
  * same names, same defaults (cipm_default_settings). */
@@ -219,6 +220,10 @@ typedef struct {
   /* nonsymmetric cones only (settings.rs:114-124) */
   double linesearch_backtrack_step, min_switch_step_length;
   int32_t presolve_enable;   /* drop nonnegative rows with an infinite bound (presolver.rs); default 1 */
+  /* print a banner, the problem and settings, one row per iteration and a footer to the handle's print target
+   * (cipm_set_print_target).  Default 0, where the reference defaults to true: this library sits below other code,
+   * and a caller that did not ask for output gets none.  May change in cipm_update_settings. */
+  int32_t verbose;
 } cipm_settings;
 
 /* DefaultInfo (default/info.rs:13-64) + timers of core/solver.rs:330-396 + counters */
@@ -271,6 +276,30 @@ uint64_t cipm_collective_count(const cipm_t *h);      /* NCCL all-gathers the ha
 int cipm_update_settings(cipm_t *h, const cipm_settings *settings);
 void cipm_destroy(cipm_t *h);
 int cipm_solve(cipm_t *h);                                   /* IPSolver::solve */
+
+/* Termination callback (set_termination_callback_c / unset_termination_callback, core/solver.rs; callbacks.rs).
+ * cipm_solve calls `fn` once per pass of its iteration loop, iteration 0 included, after the iteration's info is
+ * complete and its row printed and before the built-in termination checks; a pass that a strategy switch repeats calls
+ * it again.  `info` is what cipm_get_info would return at that moment, valid for the duration of the call.  A nonzero
+ * return ends the solve with CIPM_CALLBACK_TERMINATED on the current iterate (cipm_get_solution unscales it as usual).
+ * On a sharded handle (a transport or NCCL installed) both calls are collective: every rank makes them, each with
+ * its own function, before its next cipm_solve.  While a callback is set every pass all-gathers one value per rank
+ * through the handle's transport, and the solve stops on every rank when the callback of any rank asked to.  With no
+ * callback set no collective is added. */
+typedef int (*cipm_callback_fn)(const cipm_info *info, void *user_data);
+int cipm_set_termination_callback(cipm_t *h, cipm_callback_fn fn, void *user_data);
+int cipm_unset_termination_callback(cipm_t *h);
+
+/* Where verbose output goes (print_to_stdout / _file / _stream / _sink / _buffer, src/io/mod.rs).  STDOUT is the
+ * default; FILE appends to `path`; STREAM hands every chunk of text to `fn(ctx, buf, len)`; BUFFER collects the text
+ * in the handle (a new BUFFER target starts empty).  Arguments a kind does not use are ignored.  Every rank of a
+ * sharded solver prints to its own target. */
+enum { CIPM_PRINT_STDOUT = 0, CIPM_PRINT_SINK = 1, CIPM_PRINT_BUFFER = 2, CIPM_PRINT_FILE = 3, CIPM_PRINT_STREAM = 4 };
+typedef int (*cipm_write_fn)(void *ctx, const char *buf, uint64_t len);
+int cipm_set_print_target(cipm_t *h, int kind, const char *path, cipm_write_fn fn, void *ctx);
+/* get_print_buffer: copies min(cap, length) bytes of the BUFFER target's text to `out` (no terminating zero) and returns
+ * the full length; the buffer is not cleared.  CLDL_E_ARG when the target is not a buffer. */
+int64_t cipm_get_print_buffer(cipm_t *h, char *out, uint64_t cap);
 void cipm_get_info(const cipm_t *h, cipm_info *out);
 int cipm_get_solution(cipm_t *h, double *x, double *z, double *s);   /* unscaled, host buffers */
 uint64_t cipm_trace(const cipm_t *h, double *out, uint64_t cap_rows); /* rows of [mu,alpha,sigma,pres,dres,gap] */

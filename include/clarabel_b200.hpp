@@ -101,7 +101,7 @@ enum class SolverStatus : int32_t {
   DualInfeasible = CIPM_DUAL_INFEASIBLE, AlmostSolved = CIPM_ALMOST_SOLVED,
   AlmostPrimalInfeasible = CIPM_ALMOST_PRIMAL_INFEASIBLE, AlmostDualInfeasible = CIPM_ALMOST_DUAL_INFEASIBLE,
   MaxIterations = CIPM_MAX_ITERATIONS, MaxTime = CIPM_MAX_TIME, NumericalError = CIPM_NUMERICAL_ERROR,
-  InsufficientProgress = CIPM_INSUFFICIENT_PROGRESS
+  InsufficientProgress = CIPM_INSUFFICIENT_PROGRESS, CallbackTerminated = CIPM_CALLBACK_TERMINATED
 };
 
 // DefaultSolution (default/solution.rs:12-40)

@@ -789,7 +789,7 @@ EXPORTED_SYMBOLS += [
     "cldl_shard_refactor_phase_dev", "cldl_shard_solve_phase_dev", "cldl_shard_count", "cldl_shard_pack_dev",
     "cldl_shard_unpack_dev", "cldl_shard_counts", "cipm_abi_sizes", "cldl_set_transport", "cipm_set_transport",
     "cldl_copy_dev", "cipm_update_settings", "cipm_set_termination_callback", "cipm_unset_termination_callback",
-    "cipm_set_print_target", "cipm_get_print_buffer",
+    "cipm_set_print_target", "cipm_get_print_buffer", "cipm_derivative", "cipm_adjoint_derivative",
 ]
 
 _l2_ready = False
@@ -868,6 +868,8 @@ def _lib2():
     L.cipm_set_print_target.argtypes = [vp, C.c_int, C.c_char_p, WRITE_FN, vp]
     L.cipm_get_print_buffer.argtypes = [vp, C.c_char_p, C.c_uint64]
     L.cipm_get_print_buffer.restype = C.c_int64
+    L.cipm_derivative.argtypes = [vp, f64p, f64p, f64p, f64p, f64p, f64p, f64p]
+    L.cipm_adjoint_derivative.argtypes = [vp, f64p, f64p, f64p, f64p, f64p, f64p, f64p]
     _l2_ready = True
     return L
 
@@ -902,6 +904,7 @@ class CudaSolver:
         self._callback = None        # ctypes objects the library holds pointers to: alive while installed
         self._print_fn = None
         self._pending_exc = None     # an exception raised inside a callback or a stream write, re-raised by solve()
+        self._stamp = 0              # counts solves and data updates (autograd.py: the backward pass checks it)
         self._quiet_rank = shard is not None and int(shard[1]) != 0 and not print_all_ranks
         P, A = sp.csc_matrix(P), sp.csc_matrix(A)
         check_dimensions(P, q, A, b, cones)
@@ -1060,41 +1063,91 @@ class CudaSolver:
         takes the reference's three forms: a matrix / full vector, the vector of nonzero values, or a pair
         `(index, values)` that overwrites single entries (`zip(&index, &values)` there); `None` or an empty
         sequence leaves that part alone."""
-        import scipy.sparse as sp
         if not self.is_data_update_allowed():
             raise DataUpdateError("PresolveIsActive")
-
-        def new_values(arg, current, triu):
-            if arg is None:
-                return None
-            if sp.issparse(arg):
-                M = sp.csc_matrix(sp.triu(arg, format="csc") if triu else arg)
-                M.sort_indices()
-                # CscMatrix::is_equal_sparsity (algebra/csc/core.rs:436-445): same pattern, not just the same count
-                ip, ix = self._pattern["P" if triu else "A"]
-                if M.shape != self._shape["P" if triu else "A"] or not (np.array_equal(M.indptr, ip) and np.array_equal(M.indices, ix)):
-                    raise DataUpdateError("SparsityPattern")
-                v = _f64(M.data)
-            elif isinstance(arg, tuple) and len(arg) == 2 and not np.isscalar(arg[0]):
-                idx, val = np.asarray(arg[0], dtype=np.int64), _f64(arg[1])
-                if idx.size == 0:
-                    return None
-                v = current.copy()
-                v[idx] = val
-            else:
-                v = _f64(arg)
-                if v.size == 0:
-                    return None
-            if v.size != current.size:
-                raise DataUpdateError("BadVectorDimension" if current.ndim == 1 else "BadFormat")
-            return v
+        new_values = self._new_values
         Pv, qv = new_values(P, self._cur["P"], True), new_values(q, self._cur["q"], False)
         Av, bv = new_values(A, self._cur["A"], False), new_values(b, self._cur["b"], False)
         f = lambda a: _p(a, C.c_double) if a is not None else None
         _check(self._L.cipm_update_data(self._h, f(Pv), f(qv), f(Av), f(bv)), "cipm_update_data")
+        self._stamp += 1
         for k, v in (("P", Pv), ("q", qv), ("A", Av), ("b", bv)):
             if v is not None:
                 self._cur[k] = v.copy()
+
+    def _new_values(self, arg, current, triu):
+        """the values update_data and the derivatives take: a matrix on the stored pattern (P: its upper triangle), a
+        full vector, or a pair (index, values) that overwrites single entries of `current`; None or an empty sequence is
+        None"""
+        import scipy.sparse as sp
+        if arg is None:
+            return None
+        if sp.issparse(arg):
+            M = sp.csc_matrix(sp.triu(arg, format="csc") if triu else arg)
+            M.sort_indices()
+            # CscMatrix::is_equal_sparsity (algebra/csc/core.rs:436-445): same pattern, not just the same count
+            ip, ix = self._pattern["P" if triu else "A"]
+            if M.shape != self._shape["P" if triu else "A"] or not (np.array_equal(M.indptr, ip) and np.array_equal(M.indices, ix)):
+                raise DataUpdateError("SparsityPattern")
+            v = _f64(M.data)
+        elif isinstance(arg, tuple) and len(arg) == 2 and not np.isscalar(arg[0]):
+            idx, val = np.asarray(arg[0], dtype=np.int64), _f64(arg[1])
+            if idx.size == 0:
+                return None
+            v = current.copy()
+            v[idx] = val
+        else:
+            v = _f64(arg)
+            if v.size == 0:
+                return None
+        if v.size != current.size:
+            raise DataUpdateError("BadVectorDimension" if current.ndim == 1 else "BadFormat")
+        return v
+
+    # ---- derivatives of the solution at the last solve (cipm_derivative / cipm_adjoint_derivative) ----
+    def _derivative_rc(self, rc, what):
+        if rc == CLDL_E_ARG:
+            if not self.is_data_update_allowed():
+                raise BackendError(f"{what}: the presolve removed rows of this problem; derivatives are not available")
+            raise BackendError(f"{what}: needs a solve that ended Solved or AlmostSolved, with no data update since")
+        if rc == CLDL_E_NOT_FACTORED:
+            raise BackendError(f"{what}: the cone scaling or the factorisation of the KKT matrix failed at the solution")
+        _check(rc, what)
+
+    def derivative(self, dP=None, dq=None, dA=None, db=None):
+        """Forward derivative at the last solve: (dx, dz, ds) for the data perturbation (dP, dq, dA, db).  dP and dA
+        take the forms of update_data (matrix on the stored pattern, value vector, or (index, values) pairs of a
+        perturbation that is zero elsewhere); None = zero.  See include/clarabel_b200.h for the linear system solved."""
+        zero = {k: np.zeros_like(v) for k, v in self._cur.items()}
+        Pv, qv = self._new_values(dP, zero["P"], True), self._new_values(dq, zero["q"], False)
+        Av, bv = self._new_values(dA, zero["A"], False), self._new_values(db, zero["b"], False)
+        dx, dz, ds = np.zeros(max(self.n, 1)), np.zeros(max(self.m, 1)), np.zeros(max(self.m, 1))
+        f = lambda a: _p(a, C.c_double) if a is not None else None
+        self._derivative_rc(self._L.cipm_derivative(self._h, f(Pv), f(qv), f(Av), f(bv), f(dx), f(dz), f(ds)),
+                            "derivative")
+        return dx[:self.n], dz[:self.m], ds[:self.m]
+
+    def adjoint_derivative(self, dx=None, dz=None, ds=None):
+        """Adjoint derivative at the last solve: the gradients of <dx, x> + <dz, z> + <ds, s> w.r.t. the data, as
+        dict(P=csc on P's stored upper triangle, q=..., A=csc on A's stored pattern, b=...).  None = zero."""
+        import scipy.sparse as sp
+
+        def vec(a, n):
+            if a is None:
+                return None
+            v = _f64(a)
+            if v.size != n:
+                raise DataUpdateError("BadVectorDimension")
+            return v
+        gx, gz, gs = vec(dx, self.n), vec(dz, self.m), vec(ds, self.m)
+        nP, nA = self._cur["P"].size, self._cur["A"].size
+        gP, gq, gA, gb = np.zeros(max(nP, 1)), np.zeros(max(self.n, 1)), np.zeros(max(nA, 1)), np.zeros(max(self.m, 1))
+        f = lambda a: _p(a, C.c_double) if a is not None else None
+        self._derivative_rc(self._L.cipm_adjoint_derivative(self._h, f(gx), f(gz), f(gs), f(gP), f(gq), f(gA), f(gb)),
+                            "adjoint_derivative")
+        (Pp, Pi), (Ap, Ai) = self._pattern["P"], self._pattern["A"]
+        return dict(P=sp.csc_matrix((gP[:nP], Pi.copy(), Pp.copy()), shape=self._shape["P"]), q=gq[:self.n],
+                    A=sp.csc_matrix((gA[:nA], Ai.copy(), Ap.copy()), shape=self._shape["A"]), b=gb[:self.m])
 
     def close(self):
         if getattr(self, "_h", None):
@@ -1109,6 +1162,7 @@ class CudaSolver:
 
     def solve(self):
         self._pending_exc = None
+        self._stamp += 1
         rc = self._L.cipm_solve(self._h)
         exc, self._pending_exc = self._pending_exc, None
         if exc is not None:

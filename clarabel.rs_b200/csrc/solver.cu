@@ -117,7 +117,7 @@ static void dfree(const void* p) { if (p) cudaFree((void*)p); }
 // scalar slots shared between device reductions and the host
 enum Slot { S_NORMB = 0, S_NORME, S_MAXDIAG, S_QX, S_BZ, S_SZ, S_XPX, S_ALPHA, S_MARG0, S_MARG1,
             S_D0, S_D1, S_D2, S_D3, S_D4, S_D5, S_D6, S_D7, S_N0, S_N1, S_N2, S_N3, S_N4, S_N5, S_N6, S_N7,
-            S_NORMB2, S_NORME2, S_BARR, S_BP0, S_BP1, S_BP2, S_BP3, S_BP4, S_SZSH, S_COUNT = 40 };
+            S_NORMB2, S_NORME2, S_BARR, S_BP0, S_BP1, S_BP2, S_BP3, S_BP4, S_SZSH, S_DMU, S_COUNT = 40 };
 
 struct Scalars {
   double* d = nullptr;  // device [S_COUNT]
@@ -594,6 +594,82 @@ int KKTDevice::solve2(double* ax, double* az, double* bx, double* bz) {
   return 1;
 }
 
+// ------------------------------------------------------- solution derivatives
+// Elementwise kernels of IPM::derivative / IPM::adjoint_derivative.  The solver holds P̂ = cDPD, Â = EAD and the iterate
+// (x̂, ŝ, ẑ, τ); the derivative system K = [P A'; A -H] of the caller's coordinates is solved as K̂ [a; b] = [c D r1; E r2]
+// with [dx; dz] = [D a; E b / c] (DESIGN.md, "Solution derivatives").  Every output element is written by one thread.
+
+// the final iterate in the caller's coordinates, xo = D x̂ / τ and zo = E ẑ / (c τ) (the arithmetic of
+// cipm_get_solution), and normalised for the cone scaling, sn = ŝ / τ and zn = ẑ / τ
+__global__ void k_deriv_point(int n, int m, const double* __restrict__ x, const double* __restrict__ s,
+                              const double* __restrict__ z, const double* __restrict__ d, const double* __restrict__ e,
+                              double tauinv, double cinv, double* __restrict__ xo, double* __restrict__ zo,
+                              double* __restrict__ sn, double* __restrict__ zn) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) xo[i] = x[i] * d[i] * tauinv;
+  if (i < m) { zo[i] = z[i] * e[i] * (tauinv * cinv); sn[i] = s[i] * tauinv; zn[i] = z[i] * tauinv; }
+}
+// forward right-hand side [c D r1; E r2], r1 = -(dq + dP x + dA' z), r2 = db - dA x
+__global__ void k_deriv_rhs(int n, int m, double c, const double* __restrict__ d, const double* __restrict__ e,
+                            const double* __restrict__ dq, const double* __restrict__ dPx, const double* __restrict__ dAtz,
+                            const double* __restrict__ db, const double* __restrict__ dAx, double* __restrict__ r1,
+                            double* __restrict__ r2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) r1[i] = -c * d[i] * (dq[i] + dPx[i] + dAtz[i]);
+  if (i < m) r2[i] = e[i] * (db[i] - dAx[i]);
+}
+// forward solution in the caller's coordinates: dx = D a, dz = E b / c, ds = E⁻¹ (E r2 - Â a) = r2 - A dx
+__global__ void k_deriv_unscale(int n, int m, double cinv, const double* __restrict__ d, const double* __restrict__ e,
+                                const double* __restrict__ einv, const double* __restrict__ a,
+                                const double* __restrict__ b, const double* __restrict__ r2a, double* __restrict__ dx,
+                                double* __restrict__ dz, double* __restrict__ ds) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) dx[i] = d[i] * a[i];
+  if (i < m) { dz[i] = e[i] * b[i] * cinv; ds[i] = einv[i] * r2a[i]; }
+}
+// adjoint right-hand side [c D (gx - A' gs); E gz] before its Â' product: r1 = c D gx, r2 = E gz, t = E⁻¹ gs, after
+// which r1 -= c Â' t  (A' gs = D⁻¹ Â' E⁻¹ gs)
+__global__ void k_adj_rhs(int n, int m, double c, const double* __restrict__ d, const double* __restrict__ e,
+                          const double* __restrict__ einv, const double* __restrict__ gx, const double* __restrict__ gz,
+                          const double* __restrict__ gs, double* __restrict__ r1, double* __restrict__ r2,
+                          double* __restrict__ t) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) r1[i] = c * d[i] * gx[i];
+  if (i < m) { r2[i] = e[i] * gz[i]; t[i] = einv[i] * gs[i]; }
+}
+// adjoint solution in the caller's coordinates: u = D a, w = E b / c + gs; the gradients w.r.t. q and b are -u and w
+__global__ void k_adj_unscale(int n, int m, double cinv, const double* __restrict__ d, const double* __restrict__ e,
+                              const double* __restrict__ a, const double* __restrict__ b, const double* __restrict__ gs,
+                              double* __restrict__ u, double* __restrict__ gq, double* __restrict__ w) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) { const double ui = d[i] * a[i]; u[i] = ui; gq[i] = -ui; }
+  if (i < m) w[i] = e[i] * b[i] * cinv + gs[i];
+}
+// gradient on the stored pattern of A (CSC, the caller's order): -(z_i u_j + w_i x_j); one warp per column
+__global__ void k_grad_A(int n, const int* __restrict__ colptr, const int* __restrict__ rowval,
+                         const double* __restrict__ x, const double* __restrict__ u, const double* __restrict__ z,
+                         const double* __restrict__ w, double* __restrict__ g) {
+  const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (j >= n) return;
+  const double xj = x[j], uj = u[j];
+  for (int p = colptr[j] + lane; p < colptr[j + 1]; p += 32) {
+    const int i = rowval[p];
+    g[p] = -(z[i] * uj + w[i] * xj);
+  }
+}
+// gradient on the stored upper triangle of P (CSC, the caller's order): -(u_i x_j + x_i u_j) off the diagonal, -u_i x_i
+// on it; one warp per column
+__global__ void k_grad_P(int n, const int* __restrict__ colptr, const int* __restrict__ rowval,
+                         const double* __restrict__ x, const double* __restrict__ u, double* __restrict__ g) {
+  const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (j >= n) return;
+  const double xj = x[j], uj = u[j];
+  for (int p = colptr[j] + lane; p < colptr[j + 1]; p += 32) {
+    const int i = rowval[p];
+    g[p] = i == j ? -(u[i] * xj) : -(u[i] * xj + x[i] * uj);
+  }
+}
+
 // ------------------------------------------------------------------ the IPM
 enum { IST_UNSOLVED = 0, IST_SOLVED, IST_PINF, IST_DINF, IST_ALMOST_SOLVED, IST_ALMOST_PINF, IST_ALMOST_DINF,
        IST_MAXIT, IST_MAXTIME, IST_NUMERR, IST_INSUFF, IST_CALLBACK };
@@ -670,6 +746,25 @@ class IPM {
   int step_length(bool combined, double* alpha, int scaling = SCALING_PRIMAL_DUAL);
   int variables_barrier(double a, double* out);
   int report_pass(bool verbose, bool* stop);
+  // derivatives of the solution at the last solve (DESIGN.md, "Solution derivatives").  Valid after a solve that ended
+  // Solved / AlmostSolved until the data changes.  The scratch below is allocated by the first call.
+  bool deriv_valid = false;
+  struct DerivWS {
+    int *map_Psym = nullptr, *map_Acsr = nullptr;   // CSC position of every entry of Psym / Acsr
+    int *Pcp = nullptr, *Pri = nullptr;             // P's upper triangle as CSC (the caller's order)
+    double* arena = nullptr;
+    double *xo, *vn0, *vn1, *vn2, *rn, *an, *on0, *on1;                  // length n
+    double *zo, *sn, *zn, *vm0, *vm1, *vm2, *rm, *bm, *om0, *om1;        // length m
+    double *vP, *vPs, *vA, *vAc;                    // values on P's triu pattern, Psym, A's CSC and Acsr patterns
+    int nnzPs = 0;                                  // entries of Psym
+  } dw;
+  int derivative(const double* dPnz, const double* dqv, const double* dAnz, const double* dbv, double* dx, double* dz,
+                 double* ds);
+  int adjoint_derivative(const double* gx, const double* gz, const double* gs, double* gP, double* gq, double* gA,
+                         double* gb);
+  int deriv_prepare();
+  int deriv_factor();
+  int deriv_solve();
 };
 
 void IPM::equilibrate() {
@@ -742,15 +837,39 @@ void IPM::equilibrate() {
   for (int i = 0; i < m; i++) einv[i] = 1.0 / e[i];
 }
 
-static void csc_to_csr(const HostCsc& M, std::vector<int>& rp, std::vector<int>& ci, std::vector<double>& v) {
+// CSR of a CSC matrix; src (if given) receives, for every CSR entry, the position of its value in the CSC arrays
+static void csc_to_csr(const HostCsc& M, std::vector<int>& rp, std::vector<int>& ci, std::vector<double>& v,
+                       std::vector<int>* src = nullptr) {
   rp.assign(M.m + 1, 0);
   const int64_t nnz = M.colptr[M.n];
   for (int64_t t = 0; t < nnz; t++) rp[M.rowval[t] + 1]++;
   for (int i = 0; i < M.m; i++) rp[i + 1] += rp[i];
   ci.resize(nnz); v.resize(nnz);
+  if (src) src->resize(nnz);
   std::vector<int> pos(rp.begin(), rp.end() - 1);
   for (int j = 0; j < M.n; j++)
-    for (int64_t t = M.colptr[j]; t < M.colptr[j + 1]; t++) { int d = pos[M.rowval[t]]++; ci[d] = j; v[d] = M.nzval[t]; }
+    for (int64_t t = M.colptr[j]; t < M.colptr[j + 1]; t++) {
+      int d = pos[M.rowval[t]]++; ci[d] = j; v[d] = M.nzval[t];
+      if (src) (*src)[d] = (int)t;
+    }
+}
+
+// full symmetric CSR of an upper-triangular CSC matrix (P): row pointers, columns, and for every entry the position of
+// its value in the CSC arrays (an off-diagonal entry appears twice, at (i, j) and at (j, i))
+static void triu_to_sym_csr(const HostCsc& M, std::vector<int>& rp, std::vector<int>& ci, std::vector<int>& src) {
+  const int n = M.n;
+  rp.assign(n + 1, 0);
+  for (int j = 0; j < n; j++)
+    for (int64_t t = M.colptr[j]; t < M.colptr[j + 1]; t++) { rp[M.rowval[t] + 1]++; if (M.rowval[t] != j) rp[j + 1]++; }
+  for (int i = 0; i < n; i++) rp[i + 1] += rp[i];
+  ci.resize(rp[n]); src.resize(rp[n]);
+  std::vector<int> pos(rp.begin(), rp.end() - 1);
+  for (int j = 0; j < n; j++)
+    for (int64_t t = M.colptr[j]; t < M.colptr[j + 1]; t++) {
+      const int i = M.rowval[t];
+      ci[pos[i]] = j; src[pos[i]++] = (int)t;
+      if (i != j) { ci[pos[j]] = i; src[pos[j]++] = (int)t; }
+    }
 }
 
 int IPM::upload_problem() {
@@ -763,18 +882,10 @@ int IPM::upload_problem() {
   if (upv(&dAtr, cp32) || upv(&dAtc, A.rowval) || upv(&dAtv, A.nzval)) return CLDL_E_CUDA;
   Atcsr.nrows = n; Atcsr.rowptr = dAtr; Atcsr.col = dAtc; Atcsr.val = dAtv;
   {
-    std::vector<int> cnt(n + 1, 0);
-    for (int j = 0; j < n; j++)
-      for (int64_t t = P.colptr[j]; t < P.colptr[j + 1]; t++) { cnt[P.rowval[t] + 1]++; if (P.rowval[t] != j) cnt[j + 1]++; }
-    for (int i = 0; i < n; i++) cnt[i + 1] += cnt[i];
-    std::vector<int> col(cnt[n]), pos(cnt.begin(), cnt.end() - 1);
-    std::vector<double> val(cnt[n]);
-    for (int j = 0; j < n; j++)
-      for (int64_t t = P.colptr[j]; t < P.colptr[j + 1]; t++) {
-        const int i = P.rowval[t];
-        col[pos[i]] = j; val[pos[i]++] = P.nzval[t];
-        if (i != j) { col[pos[j]] = i; val[pos[j]++] = P.nzval[t]; }
-      }
+    std::vector<int> cnt, col, src;
+    triu_to_sym_csr(P, cnt, col, src);
+    std::vector<double> val(src.size());
+    for (size_t k = 0; k < src.size(); k++) val[k] = P.nzval[src[k]];
     if (upv(&dPr, cnt) || upv(&dPc, col) || upv(&dPv, val)) return CLDL_E_CUDA;
     Psym.nrows = n; Psym.rowptr = dPr; Psym.col = dPc; Psym.val = dPv;
   }
@@ -788,22 +899,15 @@ int IPM::upload_problem() {
 int IPM::update_data(const double* Pnz, const double* qv, const double* Anz, const double* bv) {
   if (!keep.empty()) return CLDL_E_ARG;   // data updates are refused on a presolved problem (data_updating.rs:165-180)
   SCK(cudaSetDevice(kkt.ldl.device));
+  deriv_valid = false;                    // the last solve no longer belongs to this data
   if (Pnz) {
     for (int j = 0; j < n; j++)
       for (int64_t t = P.colptr[j]; t < P.colptr[j + 1]; t++) P.nzval[t] = Pnz[t] * d[P.rowval[t]] * d[j] * c;
     // same traversal as upload_problem: values of the full symmetric CSR
-    std::vector<int> cnt(n + 1, 0);
-    for (int j = 0; j < n; j++)
-      for (int64_t t = P.colptr[j]; t < P.colptr[j + 1]; t++) { cnt[P.rowval[t] + 1]++; if (P.rowval[t] != j) cnt[j + 1]++; }
-    for (int i = 0; i < n; i++) cnt[i + 1] += cnt[i];
-    std::vector<int> pos(cnt.begin(), cnt.end() - 1);
-    std::vector<double> val(cnt[n]);
-    for (int j = 0; j < n; j++)
-      for (int64_t t = P.colptr[j]; t < P.colptr[j + 1]; t++) {
-        const int i = P.rowval[t];
-        val[pos[i]++] = P.nzval[t];
-        if (i != j) val[pos[j]++] = P.nzval[t];
-      }
+    std::vector<int> cnt, col, src;
+    triu_to_sym_csr(P, cnt, col, src);
+    std::vector<double> val(src.size());
+    for (size_t k = 0; k < src.size(); k++) val[k] = P.nzval[src[k]];
     if (!val.empty()) SCK(cudaMemcpy((void*)dPv, val.data(), val.size() * 8, cudaMemcpyHostToDevice));
   }
   if (Anz) {
@@ -994,6 +1098,7 @@ void IPM::release() {
                          (const void*)tmpn})
     dfree(p_);
   for (auto ev : iter_ev) cudaEventDestroy(ev);
+  dfree(dw.map_Psym); dfree(dw.map_Acsr); dfree(dw.Pcp); dfree(dw.Pri); dfree(dw.arena);
   dfree(d_verdict);
   if (h_verdict) cudaFreeHost(h_verdict);
   cones.release();
@@ -1246,6 +1351,7 @@ int IPM::solve() {
   double sigma = 1.0, alpha = 0.0, mu = 0.0;
   const double t0 = wall();
   info.status = IST_UNSOLVED; info.iterations = 0;
+  deriv_valid = false;
   info.t_kkt_update = info.t_kkt_solve = info.t_scale_cones = 0;
   kkt.n_refactor = kkt.n_ldl_solve = kkt.n_ir_steps = 0;
   trace.clear();
@@ -1370,7 +1476,164 @@ int IPM::solve() {
   info.n_ldl_solve = (uint64_t)kkt.n_ldl_solve;
   info.n_ir_steps = (uint64_t)kkt.n_ir_steps;
   info.regularize_count = kkt.ldl.regularize_count;
+  deriv_valid = info.status == IST_SOLVED || info.status == IST_ALMOST_SOLVED;
   if (verbose) out.write(print_footer(info));
+  return 0;
+}
+
+// ------------------------------------------------------- solution derivatives
+// First derivative call: position maps from the caller's CSC orders to Psym / Acsr, P's triu pattern on the device and
+// one scratch arena.  A handle that never differentiates allocates none of it.
+int IPM::deriv_prepare() {
+  if (dw.arena) return 0;
+  // what an earlier call that failed half way uploaded is freed, not overwritten
+  for (int** p : {&dw.map_Psym, &dw.map_Acsr, &dw.Pcp, &dw.Pri}) { dfree(*p); *p = nullptr; }
+  std::vector<int> rp, ci, psrc, asrc;
+  std::vector<double> vv;
+  triu_to_sym_csr(P, rp, ci, psrc);
+  csc_to_csr(A, rp, ci, vv, &asrc);
+  std::vector<int> pcp(P.colptr.begin(), P.colptr.end());
+  if (upv(&dw.map_Psym, psrc) || upv(&dw.map_Acsr, asrc) || upv(&dw.Pcp, pcp) || upv(&dw.Pri, P.rowval))
+    return CLDL_E_CUDA;
+  const size_t nnzP = (size_t)P.colptr[n], nnzA = (size_t)A.colptr[n], nnzPs = psrc.size();
+  const size_t total = 8 * (size_t)n + 10 * (size_t)m + nnzP + nnzPs + 2 * nnzA;
+  double* a = nullptr;
+  SCK(cudaMalloc((void**)&a, total * 8));
+  dw.arena = a;
+  for (double** p : {&dw.xo, &dw.vn0, &dw.vn1, &dw.vn2, &dw.rn, &dw.an, &dw.on0, &dw.on1}) { *p = a; a += n; }
+  for (double** p : {&dw.zo, &dw.sn, &dw.zn, &dw.vm0, &dw.vm1, &dw.vm2, &dw.rm, &dw.bm, &dw.om0, &dw.om1}) { *p = a; a += m; }
+  dw.vP = a; a += nnzP;
+  dw.vPs = a; a += nnzPs;
+  dw.vA = a; a += nnzA;
+  dw.vAc = a;
+  dw.nnzPs = (int)nnzPs;
+  return 0;
+}
+
+// Steps 1-3 of both derivative calls: the final iterate normalised by τ, the cone scaling H at it (NT scaling on the
+// symmetric cones, μ∇²f*(z) with μ = <s, z> / ν on the others), the KKT values, static regularisation and refactor.
+int IPM::deriv_factor() {
+  if (!deriv_valid || !keep.empty()) return CLDL_E_ARG;
+  SCK(cudaSetDevice(kkt.ldl.device));
+  int rc = deriv_prepare();
+  if (rc) return rc;
+  g_launches++;
+  k_deriv_point<<<(std::max(n, m) + 255) / 256, 256, 0, st>>>(n, m, x, s, z, dd, de, 1.0 / tau, 1.0 / c, dw.xo, dw.zo,
+                                                              dw.sn, dw.zn);
+  double mu = 0.0;
+  if (!cones.all_symmetric) {
+    V.dot(dw.sn, dw.zn, m, sc.d + S_DMU);
+    if ((rc = sc.fetch())) return rc;
+    mu = sc.h[S_DMU] / (double)cones.degree;
+  }
+  SCK(cudaMemsetAsync(cones.dev.fail, 0, sizeof(int), st));
+  cones.update_scaling(dw.sn, dw.zn, mu, SCALING_DUAL);
+  if (cones.dev.nsoc || cones.dev.npsd || cones.dev.ngp) {
+    int failflag = 0;
+    SCK(cudaMemcpyAsync(&failflag, cones.dev.fail, sizeof(int), cudaMemcpyDeviceToHost, st));
+    SCK(cudaStreamSynchronize(st));
+    if (failflag) return CLDL_E_NOT_FACTORED;
+  }
+  rc = kkt.update();
+  if (rc < 0) return rc;
+  return rc == 1 ? 0 : CLDL_E_NOT_FACTORED;
+}
+
+// K̂ [an; bm] = [rn; rm], refined against the unregularised K̂
+int IPM::deriv_solve() {
+  kkt.setrhs(dw.rn, dw.rm);
+  const int ok = kkt.solve(dw.an, dw.bm);
+  if (ok < 0) return ok;
+  return ok == 1 ? 0 : CLDL_E_NOT_FACTORED;
+}
+
+// host -> device on the solver's stream; NULL = zero
+static int deriv_upload(double* dst, const double* src, size_t len, cudaStream_t st) {
+  if (len == 0) return 0;
+  if (src) SCK(cudaMemcpyAsync(dst, src, len * 8, cudaMemcpyHostToDevice, st));
+  else SCK(cudaMemsetAsync(dst, 0, len * 8, st));
+  return 0;
+}
+// device -> host on the solver's stream; NULL = not wanted
+static int deriv_download(double* dst, const double* src, size_t len, cudaStream_t st) {
+  if (dst && len) SCK(cudaMemcpyAsync(dst, src, len * 8, cudaMemcpyDeviceToHost, st));
+  return 0;
+}
+
+int IPM::derivative(const double* dPnz, const double* dqv, const double* dAnz, const double* dbv, double* dxo,
+                    double* dzo, double* dso) {
+  int rc = deriv_factor();
+  if (rc) return rc;
+  const size_t nnzP = (size_t)P.colptr[n], nnzA = (size_t)A.colptr[n];
+  const unsigned grid = (std::max(n, m) + 255) / 256;
+  if ((rc = deriv_upload(dw.vn0, dqv, n, st)) || (rc = deriv_upload(dw.vm0, dbv, m, st))) return rc;
+  // dP x: the caller's values gathered into Psym order, then Psym's product
+  if (dPnz && dw.nnzPs) {
+    if ((rc = deriv_upload(dw.vP, dPnz, nnzP, st))) return rc;
+    g_launches++;
+    k_gather<<<(dw.nnzPs + 255) / 256, 256, 0, st>>>(dw.vPs, dw.vP, dw.map_Psym, dw.nnzPs);
+    CsrDev M = Psym;
+    M.val = dw.vPs;
+    spmv(M, dw.vn1, dw.xo, 1.0, 0.0);
+  } else {
+    V.zero(dw.vn1, n);
+  }
+  // dA' z on A's own CSC (Atcsr's pattern) and dA x through the values gathered into Acsr order
+  if (dAnz && nnzA) {
+    if ((rc = deriv_upload(dw.vA, dAnz, nnzA, st))) return rc;
+    CsrDev Mt = Atcsr;
+    Mt.val = dw.vA;
+    spmv(Mt, dw.vn2, dw.zo, 1.0, 0.0);
+    g_launches++;
+    k_gather<<<(unsigned)((nnzA + 255) / 256), 256, 0, st>>>(dw.vAc, dw.vA, dw.map_Acsr, (int)nnzA);
+    CsrDev M = Acsr;
+    M.val = dw.vAc;
+    spmv(M, dw.vm1, dw.xo, 1.0, 0.0);
+  } else {
+    V.zero(dw.vn2, n);
+    V.zero(dw.vm1, m);
+  }
+  g_launches++;
+  k_deriv_rhs<<<grid, 256, 0, st>>>(n, m, c, dd, de, dw.vn0, dw.vn1, dw.vn2, dw.vm0, dw.vm1, dw.rn, dw.rm);
+  if ((rc = deriv_solve())) return rc;
+  spmv(Acsr, dw.rm, dw.an, -1.0, 1.0);     // E r2 - Â a
+  g_launches++;
+  k_deriv_unscale<<<grid, 256, 0, st>>>(n, m, 1.0 / c, dd, de, deinv, dw.an, dw.bm, dw.rm, dw.on0, dw.om0, dw.om1);
+  if ((rc = deriv_download(dxo, dw.on0, n, st)) || (rc = deriv_download(dzo, dw.om0, m, st)) ||
+      (rc = deriv_download(dso, dw.om1, m, st)))
+    return rc;
+  SCK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int IPM::adjoint_derivative(const double* gx, const double* gz, const double* gs, double* gPo, double* gqo,
+                            double* gAo, double* gbo) {
+  int rc = deriv_factor();
+  if (rc) return rc;
+  const size_t nnzP = (size_t)P.colptr[n], nnzA = (size_t)A.colptr[n];
+  const unsigned grid = (std::max(n, m) + 255) / 256;
+  if ((rc = deriv_upload(dw.vn0, gx, n, st)) || (rc = deriv_upload(dw.vm0, gz, m, st)) ||
+      (rc = deriv_upload(dw.vm1, gs, m, st)))
+    return rc;
+  g_launches++;
+  k_adj_rhs<<<grid, 256, 0, st>>>(n, m, c, dd, de, deinv, dw.vn0, dw.vm0, dw.vm1, dw.rn, dw.rm, dw.vm2);
+  if (m) spmv(Atcsr, dw.rn, dw.vm2, -c, 1.0);
+  if ((rc = deriv_solve())) return rc;
+  g_launches++;
+  k_adj_unscale<<<grid, 256, 0, st>>>(n, m, 1.0 / c, dd, de, dw.an, dw.bm, dw.vm1, dw.on0, dw.on1, dw.om0);
+  const unsigned wgrid = (unsigned)((n + 7) / 8);   // 8 warps of 256 threads: one column each
+  if (nnzP) {
+    g_launches++;
+    k_grad_P<<<wgrid, 256, 0, st>>>(n, dw.Pcp, dw.Pri, dw.xo, dw.on0, dw.vP);
+  }
+  if (nnzA) {
+    g_launches++;
+    k_grad_A<<<wgrid, 256, 0, st>>>(n, dAtr, dAtc, dw.xo, dw.on0, dw.zo, dw.om0, dw.vA);
+  }
+  if ((rc = deriv_download(gPo, dw.vP, nnzP, st)) || (rc = deriv_download(gqo, dw.on1, n, st)) ||
+      (rc = deriv_download(gAo, dw.vA, nnzA, st)) || (rc = deriv_download(gbo, dw.om0, m, st)))
+    return rc;
+  SCK(cudaStreamSynchronize(st));
   return 0;
 }
 
@@ -1738,10 +2001,23 @@ int cipm_update_data(cipm_t* h, const double* P_nzval, const double* q, const do
   if (!h) return CLDL_E_ARG;
   return h->ipm.update_data(P_nzval, q, A_nzval, b);
 }
+// derivatives at the last solve (DESIGN.md, "Solution derivatives"); host buffers, NULL input = zero, NULL output = not
+// wanted.  Collective on a sharded handle: the refactor and the solve run the LDL's exchanges.
+int cipm_derivative(cipm_t* h, const double* dP_nzval, const double* dq, const double* dA_nzval, const double* db,
+                    double* dx, double* dz, double* ds) {
+  if (!h) return CLDL_E_ARG;
+  return h->ipm.derivative(dP_nzval, dq, dA_nzval, db, dx, dz, ds);
+}
+int cipm_adjoint_derivative(cipm_t* h, const double* gx, const double* gz, const double* gs, double* gP_nzval,
+                            double* gq, double* gA_nzval, double* gb) {
+  if (!h) return CLDL_E_ARG;
+  return h->ipm.adjoint_derivative(gx, gz, gs, gP_nzval, gq, gA_nzval, gb);
+}
 int ckkt_update_P(cipm_t* h, const double* P_nzval_scaled) {
   if (!h) return CLDL_E_ARG;
   IPM& I = h->ipm;
   if (cudaSetDevice(I.kkt.ldl.device) != cudaSuccess) return CLDL_E_CUDA;
+  I.deriv_valid = false;     // K no longer holds the data of the last solve
   const size_t len = I.kkt.map_P.size();
   double* tmp = nullptr;
   if (cudaMalloc((void**)&tmp, (len ? len : 1) * 8) != cudaSuccess) return CLDL_E_CUDA;
@@ -1754,6 +2030,7 @@ int ckkt_update_A(cipm_t* h, const double* A_nzval_scaled) {
   if (!h) return CLDL_E_ARG;
   IPM& I = h->ipm;
   if (cudaSetDevice(I.kkt.ldl.device) != cudaSuccess) return CLDL_E_CUDA;
+  I.deriv_valid = false;     // K no longer holds the data of the last solve
   const size_t len = I.kkt.map_A.size();
   double* tmp = nullptr;
   if (cudaMalloc((void**)&tmp, (len ? len : 1) * 8) != cudaSuccess) return CLDL_E_CUDA;

@@ -340,6 +340,36 @@ void cipm_ldl_info(const cipm_t *h, cldl_info_t *info);
  * analysis and device plans are reused, the next cipm_solve starts from the default initial point.  NULL = unchanged. */
 int cipm_update_data(cipm_t *h, const double *P_nzval, const double *q, const double *A_nzval, const double *b);
 
+/* Derivatives of the solution map at the last solve.  With (x, z, s) the solution cipm_get_solution returns, the
+ * optimality conditions linearised about it, with the complementarity of the final iterate held fixed, are
+ *     K [dx; dz] = [-dq - dP x - dA' z;  db - dA x],   K = [P A'; A -H],   ds = db - dA x - A dx.
+ * H is the cone scaling at the final iterate: on zero cones 0; on nonnegative, second-order and PSD cones the NT
+ * scaling the interior-point method uses (s/z on a nonnegative row, the exact linearisation of s_i z_i = const); on
+ * exponential, power and generalised power cones always the dual scaling mu * Hess f*(z) with mu = <s, z> / nu (the
+ * linearisation of the central-path equation s = -mu grad f*(z)), whichever scaling strategy the solve ended in.
+ * As mu -> 0 this tends to the derivative of the solution map wherever that map is differentiable, i.e. under strict
+ * complementarity; at a finite mu it is the derivative of the point the solver returned.  On polyhedral cones the
+ * limit is reached whatever the path; on second-order and PSD cones with s and z both on the boundary the NT scaling's
+ * limit depends on how centred the final iterate is, so there the result approaches the solution map's derivative
+ * only as the iterate approaches the central path.
+ * Each call builds H, refactors K (static regularisation as in a solve) and solves once with iterative refinement
+ * against the unregularised K; nothing is cached between calls.  It changes neither cipm_get_info, the trace, the
+ * solution nor what the next cipm_solve computes.
+ * Valid only after a cipm_solve that ended CIPM_SOLVED or CIPM_ALMOST_SOLVED, with no cipm_update_data, ckkt_update_P
+ * or ckkt_update_A since, and only when the inf-bound presolve removed no rows (cipm_m_reduced == m); otherwise
+ * CLDL_E_ARG.  CLDL_E_NOT_FACTORED when the cone scaling, the factorisation or the solve fails numerically.
+ * On a sharded handle both calls are collective: every rank makes them, with the same inputs.
+ *
+ * Forward derivative: (dx, dz, ds) for a data perturbation (dP on P's triu pattern, dq, dA on A's pattern, db).
+ * NULL input = zero; NULL output = not wanted. */
+int cipm_derivative(cipm_t *h, const double *dP_nzval, const double *dq, const double *dA_nzval, const double *db,
+                    double *dx, double *dz, double *ds);
+/* Adjoint: gradients w.r.t. (P triu values, q, A values, b) of <gx,x> + <gz,z> + <gs,s>.  NULL input = zero; NULL
+ * output = not wanted.  With K [u; v] = [gx - A' gs; gz] and w = v + gs: dq = -u, db = w, dA_ij = -(z_i u_j + w_i x_j)
+ * on A's pattern, dP_ij = -(u_i x_j + x_i u_j) on P's stored upper triangle (i != j) and -u_i x_i on its diagonal. */
+int cipm_adjoint_derivative(cipm_t *h, const double *gx, const double *gz, const double *gs,
+                            double *gP_nzval, double *gq, double *gA_nzval, double *gb);
+
 /* KKTSolver trait on the handle's KKT object (host buffers; x has length n, z length m).
  * ckkt_update / ckkt_solve return 1 (true) / 0 (false) like the trait's bools. */
 int ckkt_update(cipm_t *h);                                  /* KKTSolver::update(cones, settings) */

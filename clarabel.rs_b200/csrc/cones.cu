@@ -367,98 +367,13 @@ k_soc_step_length(ConeDev c, const double* __restrict__ dz_, const double* __res
 // --------------------------------------------------------------------- host
 #define CCK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { std::fprintf(stderr, "[clarabel_b200] CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); return -20; } } while (0)
 
-int ConeSet::collapse(const int32_t* types, const uint64_t* dims, uint64_t n, std::vector<ConeSpec>& out,
-                      const double* params, const uint64_t* gp_dim2, const double* gp_alpha) {
-  out.clear();
-  uint64_t k = 0, gp_cursor = 0;
-  // rows a cone occupies; exponential / power cones are three rows whatever dims[] says (supportedcone.rs:54-71)
-  auto numel = [](int t, uint64_t d) -> uint64_t { return t == CT_PSD ? d * (d + 1) / 2 : (t == CT_EXP || t == CT_POW) ? 3 : (t == CT_GENPOW ? (d ? d : 1) : d); };
-  while (k < n) {
-    const int t = types[k];
-    if (t < 0 || t > CT_GENPOW) return -21;
-    if (t == CT_GENPOW) {   // GenPowerConeT(alpha, dim2): dims[k] = len(alpha) (supportedcone.rs:44, genpowcone.rs:41-49)
-      if (!gp_dim2 || !gp_alpha || dims[k] < 1) return -21;
-      const uint64_t d1 = dims[k], d2 = gp_dim2[k];
-      ConeSpec cs{t, (int)(d1 + d2), 0, 0.0, std::vector<double>(gp_alpha + gp_cursor, gp_alpha + gp_cursor + d1)};
-      gp_cursor += d1;
-      double sum = 0.0;
-      for (double a : cs.alphas) { if (!(a > 0.0)) return -21; sum += a; }
-      if (!(std::fabs(1.0 - sum) < 2.220446049250313e-16 * (double)d1 * 0.5 + 1e-300)) return -21;
-      out.push_back(cs);
-      k++;
-      continue;
-    }
-    if (t == CT_EXP || t == CT_POW) {   // 3 rows each, never merged (supportedcone.rs:105-161)
-      const double a = (t == CT_POW && params) ? params[k] : 0.0;
-      if (t == CT_POW && !(a > 0.0 && a < 1.0)) return -21;
-      out.push_back({t, 3, 0, a, {}});
-      k++;
-      continue;
-    }
-    const uint64_t d = dims[k];
-    if (numel(t, d) == 0) { k++; continue; }
-    const bool coll = (t == CT_NONNEG) || ((t == CT_SOC || t == CT_PSD) && d == 1);
-    if (coll) {
-      uint64_t tot = (t == CT_NONNEG) ? d : 1;
-      k++;
-      while (k < n) {
-        const int t2 = types[k];
-        const uint64_t d2 = dims[k];
-        if (numel(t2, d2) != 0) {
-          if (t2 == CT_NONNEG) tot += d2;
-          else if ((t2 == CT_SOC || t2 == CT_PSD) && d2 == 1) tot += 1;
-          else break;
-        }
-        k++;
-      }
-      out.push_back({CT_NONNEG, (int)tot, 0, 0.0, {}});
-    } else {
-      if (t == CT_SOC && d < 2) return -21;
-      if (t == CT_PSD) { if (d > (uint64_t)CB_PSD_MAX_N) return -21; out.push_back({t, (int)(d * (d + 1) / 2), (int)d, 0.0, {}}); }
-      else out.push_back({t, (int)d, 0, 0.0, {}});
-      k++;
-    }
-  }
-  return 0;
-}
-
-template <class T>
-static int up(const T** dst, const std::vector<T>& v) {
-  T* p = nullptr;
-  if (cudaMalloc((void**)&p, (v.size() ? v.size() : 1) * sizeof(T)) != cudaSuccess) return -20;
-  if (!v.empty() && cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return -20;
-  *dst = p;
-  return 0;
-}
-
-static const int* g_row2blk_dummy = nullptr;
-
-int ConeSet::init(const std::vector<ConeSpec>& cs, cudaStream_t st) {
-  cones = cs;
+int ConeSet::init(const ConeLayout& layout, cudaStream_t st) {
+  static_cast<ConeLayout&>(*this) = layout;
   stream = st;
+  const std::vector<ConeSpec>& cs = cones;
   const int nc = (int)cs.size();
-  off.assign(nc, 0); boff.assign(nc, 0); sparse_flag.assign(nc, 0); soc_list.clear(); ns_list.clear(); all_symmetric = true;
-  gp_list.clear(); pdim.assign(nc, 0); allows_primal_dual = true;
-  m = 0; nHs = 0; degree = 0; p = 0;
   std::vector<int> type(nc), dim(nc);
-  for (int k = 0; k < nc; k++) {
-    type[k] = cs[k].type; dim[k] = cs[k].dim;
-    off[k] = m; boff[k] = nHs;
-    const bool sp = cs[k].type == CT_SOC && cs[k].dim > SOC_NO_EXPANSION_MAX_SIZE;
-    sparse_flag[k] = sp ? 1 : 0;
-    const bool diag = cs[k].type == CT_ZERO || cs[k].type == CT_NONNEG || sp || cs[k].type == CT_GENPOW;
-    if ((long long)nHs + (diag ? (long long)cs[k].dim : (long long)cs[k].dim * (cs[k].dim + 1) / 2) > 2000000000LL) return -21;
-    nHs += diag ? cs[k].dim : cs[k].dim * (cs[k].dim + 1) / 2;
-    m += cs[k].dim;
-    const bool ns3c = cs[k].type == CT_EXP || cs[k].type == CT_POW;
-    const bool gpc = cs[k].type == CT_GENPOW;
-    degree += cs[k].type == CT_ZERO ? 0 : (cs[k].type == CT_NONNEG ? cs[k].dim : (cs[k].type == CT_PSD ? cs[k].psd_n : (ns3c ? 3 : (gpc ? (int)cs[k].alphas.size() + 1 : 1))));
-    if (ns3c) { ns_list.push_back(k); all_symmetric = false; }
-    if (gpc) { gp_list.push_back(k); all_symmetric = false; allows_primal_dual = false; pdim[k] = 3; p += 3; }
-    if (cs[k].type == CT_SOC) soc_list.push_back(k);
-    if (cs[k].type == CT_PSD) psd_list.push_back(k);
-    if (sp) { p += 2; pdim[k] = 2; }
-  }
+  for (int k = 0; k < nc; k++) { type[k] = cs[k].type; dim[k] = cs[k].dim; }
   std::vector<signed char> tag(m);
   std::vector<int> row2blk(m, 0);
   for (int k = 0; k < nc; k++)
@@ -467,9 +382,9 @@ int ConeSet::init(const std::vector<ConeSpec>& cs, cudaStream_t st) {
       row2blk[off[k] + i] = boff[k] + i;  // valid for diagonal-block cones
     }
   dev.ncones = nc; dev.m = m; dev.nsoc = (int)soc_list.size();
-  if (up(&dev.type, type) || up(&dev.off, off) || up(&dev.dim, dim) || up(&dev.boff, boff) ||
-      up(&dev.sparse, sparse_flag) || up(&dev.soc_list, soc_list) || up(&dev.rowtag, tag)) return -20;
-  if (up(&row2blk_dev, row2blk)) return -20;
+  CCK(upload(&dev.type, type)); CCK(upload(&dev.off, off)); CCK(upload(&dev.dim, dim)); CCK(upload(&dev.boff, boff));
+  CCK(upload(&dev.sparse, sparse_flag)); CCK(upload(&dev.soc_list, soc_list)); CCK(upload(&dev.rowtag, tag));
+  CCK(upload(&row2blk_dev, row2blk));
   const size_t mm = (size_t)(m ? m : 1), cc = (size_t)(nc ? nc : 1);
   CCK(cudaMalloc((void**)&dev.w, mm * 8)); CCK(cudaMalloc((void**)&dev.lam, mm * 8));
   CCK(cudaMalloc((void**)&dev.u, mm * 8)); CCK(cudaMalloc((void**)&dev.v, mm * 8));
@@ -494,7 +409,7 @@ int ConeSet::init(const std::vector<ConeSpec>& cs, cudaStream_t st) {
         if (cs[k].dim > psd_numel_max) psd_numel_max = cs[k].dim;
       }
     dev.npsd = (int)psd_list.size();
-    if (up(&dev.psd_list, psd_list) || up(&dev.psd_n, pn) || up(&dev.psd_moff, mo)) return -20;
+    CCK(upload(&dev.psd_list, psd_list)); CCK(upload(&dev.psd_n, pn)); CCK(upload(&dev.psd_moff, mo));
     const size_t tb = (size_t)(tot ? tot : 1) * 8;
     psd_mat_total = tot;
     CCK(cudaMalloc((void**)&dev.psd_R, tb)); CCK(cudaMalloc((void**)&dev.psd_Rinv, tb)); CCK(cudaMalloc((void**)&dev.psd_RRt, tb));
@@ -510,7 +425,6 @@ int ConeSet::init(const std::vector<ConeSpec>& cs, cudaStream_t st) {
   }
   const size_t np = (size_t)RED_BLOCKS + soc_list.size() + psd_list.size() + 8;
   CCK(cudaMalloc((void**)&d_pmin, np * 8)); CCK(cudaMalloc((void**)&d_psum, np * 8));
-  (void)g_row2blk_dummy;
   return 0;
 }
 

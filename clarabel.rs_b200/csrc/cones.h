@@ -13,13 +13,12 @@
 #include <cstdint>
 #include <vector>
 
+#include "problem_setup.h"
 #include "vec.cuh"
 
 namespace cb {
 
-enum { CT_ZERO = 0, CT_NONNEG = 1, CT_SOC = 2, CT_PSD = 3, CT_EXP = 4, CT_POW = 5, CT_GENPOW = 6 };
 enum { SCALING_PRIMAL_DUAL = 0, SCALING_DUAL = 1 };   // ScalingStrategy (cones/mod.rs)
-constexpr int SOC_NO_EXPANSION_MAX_SIZE = 4;  // socone.rs:46
 
 struct ConeDev {
   int ncones = 0, m = 0, nsoc = 0;
@@ -64,17 +63,9 @@ struct ConeDev {
   double *gp_d2 = nullptr, *gp_mu = nullptr;                                                            // [ngp]
 };
 
-constexpr int CB_PSD_MAX_N = 128;   // Hs block of one cone: tri(tri(128)) = 3.4e7 entries
-
-// dim = number of rows the cone occupies (numel); psd_n = matrix dimension of a PSD cone
-// param: exponent of a power cone; alphas: exponents of a generalised power cone (dim = alphas.size() + dim2)
-struct ConeSpec { int type; int dim; int psd_n = 0; double param = 0.0; std::vector<double> alphas; };
-
-class ConeSet {
+// the device half of a cone layout
+class ConeSet : public ConeLayout {
  public:
-  std::vector<ConeSpec> cones;       // after collapsing
-  std::vector<int> off, boff, sparse_flag, soc_list;
-  int m = 0, nHs = 0, degree = 0, p = 0;  // p = number of sparse expansion rows
   ConeDev dev;
   cudaStream_t stream = nullptr;
   ReduceWS ws;
@@ -82,11 +73,7 @@ class ConeSet {
   double* d_pmin = nullptr;
   double* d_psum = nullptr;
 
-  // collapse like SupportedConeT::new_collapsed (supportedcone.rs:105-161)
-  static int collapse(const int32_t* types, const uint64_t* dims, uint64_t n, std::vector<ConeSpec>& out,
-                      const double* params = nullptr, const uint64_t* gp_dim2 = nullptr,
-                      const double* gp_alpha = nullptr);
-  int init(const std::vector<ConeSpec>& cs, cudaStream_t st);
+  int init(const ConeLayout& layout, cudaStream_t st);   // uploads the layout
   void release();
 
   void set_identity_scaling();
@@ -104,10 +91,6 @@ class ConeSet {
   void scaled_unit_shift(double* z, double alpha, bool primal);
 
   // nonsymmetric pieces (cones_nonsym.cu)
-  std::vector<int> ns_list;
-  bool all_symmetric = true;
-  bool allows_primal_dual = true;        // false as soon as a generalised power cone is present (genpowcone.rs:108-110)
-  std::vector<int> gp_list, pdim;        // pdim[k]: extra KKT columns of cone k (2 sparse SOC, 3 GenPow, else 0)
   int gp_prepare();
   void gp_release();
   // the three KKT columns + diagonal entries of every generalised power cone (datamaps.rs:314-337)
@@ -127,7 +110,6 @@ class ConeSet {
                        double* partial, double* out);
 
   // PSD pieces (cones_psd.cu)
-  std::vector<int> psd_list;
   int psd_nmax = 0, psd_numel_max = 0, psd_warps = 4;
   long long psd_mat_total = 0;     // sum of n^2 over the PSD cones
   int psd_prepare();

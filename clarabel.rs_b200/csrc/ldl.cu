@@ -1011,16 +1011,6 @@ __global__ void k_offset_values(double* __restrict__ vals, const int* __restrict
     }                                                                                \
   } while (0)
 
-// a device copy of v (at least one element) in *dptr
-template <class D, class T>
-static int upload(D** dptr, const std::vector<T>& v) {
-  T* p = nullptr;
-  CK(cudaMalloc((void**)&p, (v.size() ? v.size() : 1) * sizeof(T)));
-  if (!v.empty()) CK(cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  *dptr = reinterpret_cast<D*>(p);
-  return 0;
-}
-
 int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* Ax,
                     const int8_t* dsigns, const cldl_opts& o, const int* perm_in) {
   n = n_;
@@ -1069,22 +1059,22 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   CK(cudaMallocHost((void**)&h_status, ST_COUNT * sizeof(int)));
 
   auto to_ll = [](const std::vector<int64_t>& v) { return std::vector<long long>(v.begin(), v.end()); };
-  if ((rc = upload(&dev.sn_first, S.sn_first))) return rc;
-  if ((rc = upload(&dev.sn_rowptr, to_ll(S.sn_rowptr)))) return rc;
-  if ((rc = upload(&dev.sn_rows, S.sn_rows))) return rc;
-  if ((rc = upload(&dev.child_ptr, to_ll(S.child_ptr)))) return rc;
-  if ((rc = upload(&dev.child_list, S.child_list))) return rc;
-  if ((rc = upload(&dev.rel, S.rel))) return rc;
-  if ((rc = upload(&dev.panel_off, to_ll(S.panel_off)))) return rc;
-  if ((rc = upload(&dev.upd_off, to_ll(S.upd_off)))) return rc;
-  if ((rc = upload(&dev.asm_ptr, to_ll(S.asm_ptr)))) return rc;
-  if ((rc = upload(&dev.asm_src, S.asm_src))) return rc;
-  if ((rc = upload(&dev.asm_dst, to_ll(S.asm_dst)))) return rc;
-  if ((rc = upload(&dev.perm, S.perm))) return rc;
+  CK(upload(&dev.sn_first, S.sn_first));
+  CK(upload(&dev.sn_rowptr, to_ll(S.sn_rowptr)));
+  CK(upload(&dev.sn_rows, S.sn_rows));
+  CK(upload(&dev.child_ptr, to_ll(S.child_ptr)));
+  CK(upload(&dev.child_list, S.child_list));
+  CK(upload(&dev.rel, S.rel));
+  CK(upload(&dev.panel_off, to_ll(S.panel_off)));
+  CK(upload(&dev.upd_off, to_ll(S.upd_off)));
+  CK(upload(&dev.asm_ptr, to_ll(S.asm_ptr)));
+  CK(upload(&dev.asm_src, S.asm_src));
+  CK(upload(&dev.asm_dst, to_ll(S.asm_dst)));
+  CK(upload(&dev.perm, S.perm));
   {
     std::vector<signed char> ds(n);
     for (int k = 0; k < n; k++) ds[k] = dsigns ? (signed char)dsigns[S.perm[k]] : (signed char)1;
-    if ((rc = upload(&dev.dsigns, ds))) return rc;
+    CK(upload(&dev.dsigns, ds));
   }
   nnzA = Ap[n];
   CK(cudaMalloc((void**)&dev.vals, (size_t)(nnzA ? nnzA : 1) * sizeof(double)));
@@ -1139,27 +1129,27 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   // tree level 0: plain launches
   CK(cudaFuncSetAttribute(k_factor_level<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, level_cap * 8));
   plan = std::move(l0.segs);
-  if ((rc = upload(&dev.level_tasks, l0.level_tasks))) return rc;
+  CK(upload(&dev.level_tasks, l0.level_tasks));
 
   // dataflow factorisation (k_factor_df)
-  if ((rc = upload(&dev.sc_panel_src, fp.sc_panel_src))) return rc;
-  if ((rc = upload(&dev.sc_panel_dst, fp.sc_panel_dst))) return rc;
-  if ((rc = upload(&dev.sc_tile_src, fp.sc_tile_src))) return rc;
-  if ((rc = upload(&dev.sc_tile_dst, fp.sc_tile_dst))) return rc;
+  CK(upload(&dev.sc_panel_src, fp.sc_panel_src));
+  CK(upload(&dev.sc_panel_dst, fp.sc_panel_dst));
+  CK(upload(&dev.sc_tile_src, fp.sc_tile_src));
+  CK(upload(&dev.sc_tile_dst, fp.sc_tile_dst));
   if (std::getenv("CB_TIMING")) std::fprintf(stderr, "[cb timing]     factor plan: %zu tasks, %zu child records, %zu big fronts, %zu tiles\n",
                                               fp.tasks.size(), fp.recs.size(), fp.sc_panel_ptr.size() - 1, fp.sc_tile_ptr.size() - 1);
   dff.ntask = (int)fp.tasks.size();
   dff_ntask_owned = fp.ntask_owned;
-  if ((rc = upload(&dff.tasks, fp.tasks))) return rc;
-  if ((rc = upload(&dff.recs, fp.recs))) return rc;
-  if ((rc = upload(&d_dff_init, fp.cnt_init))) return rc;
+  CK(upload(&dff.tasks, fp.tasks));
+  CK(upload(&dff.recs, fp.recs));
+  CK(upload(&d_dff_init, fp.cnt_init));
   CK(cudaMalloc((void**)&d_dff_cnt, fp.cnt_init.size() * sizeof(int) + 16));
   dff.pend = d_dff_cnt; dff.diag_done = d_dff_cnt + S.nsup; dff.rows_left = d_dff_cnt + 2 * (size_t)S.nsup;
   dff.tiles_left = d_dff_cnt + 3 * (size_t)S.nsup;
   CK(cudaMalloc((void**)&dff.qhead, sizeof(int)));
-  if ((rc = upload(&dff.parent, S.sn_parent))) return rc;
-  if ((rc = upload(&dff.big_pos, fp.big_pos))) return rc;
-  if ((rc = upload(&dff.tile_base, fp.tile_base))) return rc;
+  CK(upload(&dff.parent, S.sn_parent));
+  CK(upload(&dff.big_pos, fp.big_pos));
+  CK(upload(&dff.tile_base, fp.tile_base));
   CK(cudaFuncSetAttribute(k_factor_df, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_SMEM_DOUBLES * 8));
   int occ = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_factor_df, DF_NT, (size_t)DF_SMEM_DOUBLES * 8));
@@ -1179,21 +1169,21 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   sv_leafw_nrmax = sp.leafw_nrmax;
   sv_leafw_grid = sv_nleafw;      // one CTA per front (a loop over fronts inside fewer CTAs was slower: 312 vs 189 us forward on C4)
   sv_ntask_owned = sp.ntask_owned;
-  if ((rc = upload(&dev.gat_ptr, sp.gat_ptr))) return rc;
-  if ((rc = upload(&dev.gat_src, sp.gat_src))) return rc;
-  if ((rc = upload(&d_sv_wide, sp.wide))) return rc;
-  if ((rc = upload(&d_sv_leaf1, sp.leaf1))) return rc;
-  if ((rc = upload(&d_sv_leafn, sp.leafn))) return rc;
-  if ((rc = upload(&d_sv_leafw, sp.leafw))) return rc;
-  if ((rc = upload(&sv.fronts, sp.fronts))) return rc;
-  if ((rc = upload(&sv.front2task, sp.front2task))) return rc;
-  if ((rc = upload(&sv.parent, S.sn_parent))) return rc;
-  if ((rc = upload(&sv.tasks, sp.tasks))) return rc;
+  CK(upload(&dev.gat_ptr, sp.gat_ptr));
+  CK(upload(&dev.gat_src, sp.gat_src));
+  CK(upload(&d_sv_wide, sp.wide));
+  CK(upload(&d_sv_leaf1, sp.leaf1));
+  CK(upload(&d_sv_leafn, sp.leafn));
+  CK(upload(&d_sv_leafw, sp.leafw));
+  CK(upload(&sv.fronts, sp.fronts));
+  CK(upload(&sv.front2task, sp.front2task));
+  CK(upload(&sv.parent, S.sn_parent));
+  CK(upload(&sv.tasks, sp.tasks));
   // counters: [pend(nt) | fleft(nsup) | bleft(nsup)] are copied from their initial values before every solve,
   // [tdone(nt) | ydone(nsup) | done(nsup) | qhead(2)] are cleared
   sv_ninit = sp.cnt_init.size();
   sv_nzero = (size_t)nt + 2 * (size_t)S.nsup + 2;
-  if ((rc = upload(&d_sv_init, sp.cnt_init))) return rc;
+  CK(upload(&d_sv_init, sp.cnt_init));
   CK(cudaMalloc((void**)&d_sv_cnt, (sv_ninit + sv_nzero) * sizeof(int)));
   sv.pend = d_sv_cnt; sv.fleft = d_sv_cnt + nt; sv.bleft = sv.fleft + S.nsup;
   sv.tdone = d_sv_cnt + sv_ninit; sv.ydone = sv.tdone + nt; sv.done = sv.ydone + S.nsup; sv.qhead = sv.done + S.nsup;
@@ -1219,7 +1209,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   if (sharded()) {
     d_shard_xidx.assign(shard_nranks, nullptr);
     for (int w = 0; w < 2; w++) { d_shard_segs[w].assign(shard_nranks, nullptr); shard_nsegs[w].assign(shard_nranks, 0); }
-    for (int g = 0; g < shard_nranks; g++) { int* t1 = nullptr; if ((rc = upload(&d_shard_xidx[g], shard_xidx[g]))) return rc; }
+    for (int g = 0; g < shard_nranks; g++) CK(upload(&d_shard_xidx[g], shard_xidx[g]));
   }
   if (big_alloc.joinable()) big_alloc.join();
   if (big_alloc_rc) { std::fprintf(stderr, "[clarabel_b200] device allocation of the factor storage failed\n"); return CLDL_E_CUDA; }

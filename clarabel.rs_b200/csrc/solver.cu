@@ -1,9 +1,10 @@
 // Device-resident KKT solver and interior-point driver (sm_90a) + ckkt_* /
 // ccone_* / cipm_* C-ABI (include/clarabel_b200.h).
 //
+// The set-up on the host (input checks, presolve, equilibration, KKT assembly) is in problem_setup.{h,cpp}.
+//
 // What it replaces in the reference (all file:line under /root/reference/src):
-//   KKTDevice::assemble    solver/core/kktsolvers/direct/quasidef/kkt_assembly.rs:20-183,
-//                          datamaps.rs:112-221, 350-405, directldlkktsolver.rs:392-405
+//   KKTDevice::init        directldlkktsolver.rs:392-405
 //   KKTDevice::update      directldlkktsolver.rs:134-158, 217-264, 324-329
 //   KKTDevice::solve       directldlkktsolver.rs:168-189, 266-347 (iterative refinement)
 //   k_csr_spmv             algebra/csc/matrix_math.rs:178-208, 261-343 (symv / gemv, as gathers)
@@ -27,6 +28,7 @@
 #include "cones.h"
 #include "ipm_print.h"
 #include "ldl_device.h"
+#include "problem_setup.h"
 #include "vec.cuh"
 
 // the bound beyond which a constraint counts as absent (src/utils/infbounds.rs: INFINITY_DEFAULT = 1e20, process-wide,
@@ -97,21 +99,6 @@ __global__ void k_sparse_soc_fill(ConeDev c, double* __restrict__ vals, const in
 }
 
 // ------------------------------------------------------------- host helpers
-struct HostCsc {
-  int m = 0, n = 0;
-  std::vector<int64_t> colptr;
-  std::vector<int> rowval;
-  std::vector<double> nzval;
-};
-
-template <class T>
-static int upv(T** dst, const std::vector<T>& v) {
-  T* p = nullptr;
-  if (cudaMalloc((void**)&p, (v.size() ? v.size() : 1) * sizeof(T)) != cudaSuccess) return CLDL_E_CUDA;
-  if (!v.empty() && cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) return CLDL_E_CUDA;
-  *dst = p;
-  return 0;
-}
 static void dfree(const void* p) { if (p) cudaFree((void*)p); }
 
 // scalar slots shared between device reductions and the host
@@ -186,23 +173,17 @@ struct Vec {
 };
 
 // --------------------------------------------------------------- KKT solver
-class KKTDevice {
+// the device half of a KKT assembly (the host copies stay for tests / get_kkt)
+class KKTDevice : public KKTAssembly {
  public:
-  int n = 0, m = 0, p = 0, N = 0;
-  int64_t nnzK = 0;
+  int n = 0, m = 0, p = 0;
   cipm_settings set{};
   ConeSet* cones = nullptr;
   LDLObject ldl;
   cudaStream_t st = nullptr;
   Scalars* sc = nullptr;
   Vec V{};
-  // host copies of the structure (for tests / get_kkt)
-  std::vector<int64_t> Kp;
-  std::vector<int> Ki;
-  std::vector<double> Kx;
-  std::vector<int8_t> dsigns;
-  std::vector<int> map_P, map_A, map_Hs, map_u, map_v, map_D, map_diag;
-  std::vector<int> map_gqr, map_gp, map_gD;   // generalised power cones: q|r rows, p rows (by row), 3 diagonals per cone
+  std::vector<double> Kx;   // host copy of the values: P and A, zeros elsewhere
   int *d_map_gqr = nullptr, *d_map_gp = nullptr, *d_map_gD = nullptr;
   // device
   int *d_map_P = nullptr, *d_map_A = nullptr, *d_map_Hs = nullptr, *d_map_u = nullptr, *d_map_v = nullptr,
@@ -215,8 +196,6 @@ class KKTDevice {
   double *d_x2 = nullptr, *d_b2 = nullptr, *d_w1b = nullptr, *d_w2b = nullptr;   // second right-hand side in flight
   int64_t n_refactor = 0, n_ldl_solve = 0, n_ir_steps = 0;
 
-  int assemble(const HostCsc& P, const HostCsc& A);
-  bool defer_values = false;   // assemble the pattern only; set_PA_values() fills P and A later
   int set_PA_values(const HostCsc& P, const HostCsc& A);
   int init(const HostCsc& P, const HostCsc& A, ConeSet* cs, const cipm_settings& s, const cldl_opts& lo,
            const int* perm, cudaStream_t stream_unused, Scalars* scal);
@@ -232,135 +211,29 @@ class KKTDevice {
   CsrDev symK() const { CsrDev M; M.nrows = N; M.rowptr = d_srow; M.col = d_scol; M.val = d_sval; return M; }
 };
 
-int KKTDevice::assemble(const HostCsc& P, const HostCsc& A) {
-  // Layout contract (SURVEY 8a): triu; cols 0..n = triu(P) + structural diagonal;
-  // cols n..n+m = A' block then the cone's Hs entries; cols n+m.. = SOC expansion
-  // columns (v first, u second) then their two diagonal entries.  Diagonal is the
-  // last entry of every column.
-  const int nc = (int)cones->cones.size();
-  p = cones->p;
-  N = n + m + p;
-  std::vector<int64_t> cnt(N + 1, 0);
-  auto has_diag = [&](int i) {
-    return P.colptr[i] != P.colptr[i + 1] && P.rowval[P.colptr[i + 1] - 1] == i;
-  };
-  for (int i = 0; i < n; i++) cnt[i] += P.colptr[i + 1] - P.colptr[i] + (has_diag(i) ? 0 : 1);
-  for (int64_t q = 0; q < A.colptr[n]; q++) cnt[n + A.rowval[q]] += 1;
-  int pcol = n + m;
-  for (int k = 0; k < nc; k++) {
-    const ConeSpec& c = cones->cones[k];
-    const int row = n + cones->off[k];
-    const bool diag = c.type == CT_ZERO || c.type == CT_NONNEG || cones->sparse_flag[k] || c.type == CT_GENPOW;
-    for (int i = 0; i < c.dim; i++) cnt[row + i] += diag ? 1 : i + 1;
-    if (cones->sparse_flag[k]) { cnt[pcol] += c.dim + 1; cnt[pcol + 1] += c.dim + 1; pcol += 2; }
-    if (c.type == CT_GENPOW) {   // q, r, p columns + their diagonal entries (datamaps.rs:264-287)
-      const int d1 = (int)c.alphas.size();
-      cnt[pcol] += d1 + 1; cnt[pcol + 1] += c.dim - d1 + 1; cnt[pcol + 2] += c.dim + 1; pcol += 3;
-    }
-  }
-  Kp.assign(N + 1, 0);
-  for (int j = 0; j < N; j++) Kp[j + 1] = Kp[j] + cnt[j];
-  nnzK = Kp[N];
-  if (nnzK > 0x7fffffff) return CLDL_E_DIM;
-  Ki.assign(nnzK, 0);
-  Kx.assign(nnzK, 0.0);
-  std::vector<int64_t> nxt(Kp.begin(), Kp.end() - 1);
-  map_P.assign(P.colptr[n], 0);
-  map_A.assign(A.colptr[n], 0);
-  map_Hs.assign(cones->nHs, 0);
-  map_u.assign(m ? m : 1, 0);
-  map_v.assign(m ? m : 1, 0);
-  map_D.assign(2 * (nc ? nc : 1), 0);
-  map_gqr.assign(m ? m : 1, 0); map_gp.assign(m ? m : 1, 0); map_gD.assign(3 * (cones->gp_list.size() ? cones->gp_list.size() : 1), 0);
-  int gpk = 0;
-  for (int i = 0; i < n; i++) {
-    for (int64_t q = P.colptr[i]; q < P.colptr[i + 1]; q++) {
-      int64_t d = nxt[i]++;
-      Ki[d] = P.rowval[q]; Kx[d] = defer_values ? 0.0 : P.nzval[q]; map_P[q] = (int)d;
-    }
-    if (!has_diag(i)) { int64_t d = nxt[i]++; Ki[d] = i; Kx[d] = 0.0; }
-  }
-  for (int i = 0; i < A.n; i++)
-    for (int64_t q = A.colptr[i]; q < A.colptr[i + 1]; q++) {
-      const int col = n + A.rowval[q];
-      int64_t d = nxt[col]++;
-      Ki[d] = i; Kx[d] = defer_values ? 0.0 : A.nzval[q]; map_A[q] = (int)d;
-    }
-  pcol = n + m;
-  for (int k = 0; k < nc; k++) {
-    const ConeSpec& c = cones->cones[k];
-    const int row = n + cones->off[k];
-    int* blk = map_Hs.data() + cones->boff[k];
-    const bool diag = c.type == CT_ZERO || c.type == CT_NONNEG || cones->sparse_flag[k] || c.type == CT_GENPOW;
-    if (diag) {
-      for (int i = 0; i < c.dim; i++) { int64_t d = nxt[row + i]++; Ki[d] = row + i; blk[i] = (int)d; }
-    } else {
-      int kk = 0;
-      for (int col = row; col < row + c.dim; col++)
-        for (int r = row; r <= col; r++) { int64_t d = nxt[col]++; Ki[d] = r; blk[kk++] = (int)d; }
-    }
-    if (cones->sparse_flag[k]) {
-      const int o = cones->off[k];
-      for (int i = 0; i < c.dim; i++) { int64_t d = nxt[pcol]++; Ki[d] = row + i; map_v[o + i] = (int)d; }
-      for (int i = 0; i < c.dim; i++) { int64_t d = nxt[pcol + 1]++; Ki[d] = row + i; map_u[o + i] = (int)d; }
-      for (int i = 0; i < 2; i++) { int64_t d = nxt[pcol + i]++; Ki[d] = pcol + i; map_D[2 * k + i] = (int)d; }
-      pcol += 2;
-    }
-    if (c.type == CT_GENPOW) {   // datamaps.rs:289-312: q rows [0, dim1), r rows [dim1, dim), p all rows
-      const int o = cones->off[k], d1 = (int)c.alphas.size();
-      for (int i = 0; i < d1; i++) { int64_t d = nxt[pcol]++; Ki[d] = row + i; map_gqr[o + i] = (int)d; }
-      for (int i = d1; i < c.dim; i++) { int64_t d = nxt[pcol + 1]++; Ki[d] = row + i; map_gqr[o + i] = (int)d; }
-      for (int i = 0; i < c.dim; i++) { int64_t d = nxt[pcol + 2]++; Ki[d] = row + i; map_gp[o + i] = (int)d; }
-      for (int i = 0; i < 3; i++) { int64_t d = nxt[pcol + i]++; Ki[d] = pcol + i; map_gD[3 * gpk + i] = (int)d; }
-      gpk++;
-      pcol += 3;
-    }
-  }
-  map_diag.resize(N);
-  for (int j = 0; j < N; j++) map_diag[j] = (int)(Kp[j + 1] - 1);
-  dsigns.assign(N, 1);
-  for (int i = n; i < n + m; i++) dsigns[i] = -1;
-  int pp = n + m;
-  for (int k = 0; k < nc; k++) {
-    if (cones->sparse_flag[k]) { dsigns[pp] = -1; dsigns[pp + 1] = 1; pp += 2; }
-    else if (cones->cones[k].type == CT_GENPOW) { dsigns[pp] = -1; dsigns[pp + 1] = -1; dsigns[pp + 2] = 1; pp += 3; }   // datamaps.rs:252-254
-  }
-  return 0;
-}
-
 int KKTDevice::init(const HostCsc& P, const HostCsc& A, ConeSet* cs, const cipm_settings& s, const cldl_opts& lo,
                     const int* perm, cudaStream_t, Scalars* scal) {
-  n = P.n; m = A.m; cones = cs; set = s; sc = scal;
-  int rc = assemble(P, A);
+  n = P.n; m = A.m; p = cs->p; cones = cs; set = s; sc = scal;
+  int rc = assemble_kkt(P, A, *cones, *this);
   if (rc) return rc;
+  Kx.assign(nnzK, 0.0);
   cb_tmark("kkt: assemble");
-  std::vector<int32_t> Ki32(Ki.begin(), Ki.end());
   cldl_opts o = lo;
   o.regularize_eps = s.dynamic_regularization_eps;
   o.regularize_delta = s.dynamic_regularization_delta;
   o.regularize_enable = 1;  // the reference adapter ignores dynamic_regularization_enable (ldlsolvers/qdldl.rs:38)
-  // Dense cone blocks (PSD, dense SOC): contract every block to one vertex for the ordering
-  // (order_with_groups in symbolic.cpp), unless the caller fixed the permutation.
+  // Dense cone blocks (PSD, dense SOC): contract every block to one vertex for the ordering, unless the caller fixed
+  // the permutation.
   std::vector<int> perm_grp;
-  if (!perm) {
-    std::vector<int> group(N, -1);
-    int ngroups = 0;
-    for (size_t k = 0; k < cones->cones.size(); k++) {
-      const ConeSpec& c = cones->cones[k];
-      if (c.type == CT_ZERO || c.type == CT_NONNEG || cones->sparse_flag[k] || c.type == CT_GENPOW || c.dim <= 8) continue;
-      for (int i = 0; i < c.dim; i++) group[n + cones->off[k] + i] = ngroups;
-      ngroups++;
-    }
-    if (ngroups > 0) {
-      SymbolicOptions so;
-      so.ordering = o.ordering ? o.ordering : ORDER_BEST;
-      if (o.nd_leaf > 0) so.nd_leaf = o.nd_leaf;
-      if (o.max_panel > 0) so.max_panel = o.max_panel > CB_PB_MAXNS ? CB_PB_MAXNS : o.max_panel;
-      int kind = 0;
-      rc = order_with_groups(N, Kp.data(), Ki32.data(), group.data(), ngroups, so, perm_grp, &kind);
-      if (rc) return CLDL_E_ARG;
-      perm = perm_grp.data();
-    }
+  if (!perm && ngroups > 0) {
+    SymbolicOptions so;
+    so.ordering = o.ordering ? o.ordering : ORDER_BEST;
+    if (o.nd_leaf > 0) so.nd_leaf = o.nd_leaf;
+    if (o.max_panel > 0) so.max_panel = o.max_panel > CB_PB_MAXNS ? CB_PB_MAXNS : o.max_panel;
+    int kind = 0;
+    rc = order_with_groups(N, Kp.data(), Ki.data(), group.data(), ngroups, so, perm_grp, &kind);
+    if (rc) return CLDL_E_ARG;
+    perm = perm_grp.data();
   }
   // full symmetric CSR of K with an index into the value array (used by iterative refinement): only needs the
   // assembled pattern, so it is built and uploaded on a host thread next to the ordering / symbolic analysis
@@ -368,28 +241,15 @@ int KKTDevice::init(const HostCsc& P, const HostCsc& A, ConeSet* cs, const cipm_
   const int devid = lo.device;
   auto build_sym_csr = [&]() -> int {
     if (cudaSetDevice(devid) != cudaSuccess) return CLDL_E_CUDA;
-    std::vector<int> rowcnt(N + 1, 0);
-    for (int j = 0; j < N; j++)
-      for (int64_t q = Kp[j]; q < Kp[j + 1]; q++) {
-        rowcnt[Ki[q] + 1]++;
-        if (Ki[q] != j) rowcnt[j + 1]++;
-      }
-    for (int i = 0; i < N; i++) rowcnt[i + 1] += rowcnt[i];
-    nnzS = rowcnt[N];
-    std::vector<int> scol(nnzS), sidx(nnzS), pos(rowcnt.begin(), rowcnt.end() - 1);
-    for (int j = 0; j < N; j++)
-      for (int64_t q = Kp[j]; q < Kp[j + 1]; q++) {
-        const int i = Ki[q];
-        scol[pos[i]] = j; sidx[pos[i]++] = (int)q;
-        if (i != j) { scol[pos[j]] = i; sidx[pos[j]++] = (int)q; }
-      }
-    if (upv(&d_srow, rowcnt) || upv(&d_scol, scol) || upv(&d_sidx, sidx)) return CLDL_E_CUDA;
+    const CsrMap S = triu_to_sym_csr(N, Kp.data(), Ki.data());
+    nnzS = S.rowptr[N];
+    SCK(upload(&d_srow, S.rowptr)); SCK(upload(&d_scol, S.col)); SCK(upload(&d_sidx, S.src));
     SCK(cudaMalloc((void**)&d_sval, (size_t)(nnzS ? nnzS : 1) * 8));
     return 0;
   };
   std::thread th_csr([&]() { rc_csr = build_sym_csr(); });
   struct ThJoin { std::thread* t; ~ThJoin() { if (t->joinable()) t->join(); } } th_csr_guard{&th_csr};
-  rc = ldl.init(N, Kp.data(), Ki32.data(), Kx.data(), dsigns.data(), o, perm);
+  rc = ldl.init(N, Kp.data(), Ki.data(), Kx.data(), dsigns.data(), o, perm);
   if (rc) return rc;
   st = ldl.stream;
   V.st = st;
@@ -397,10 +257,10 @@ int KKTDevice::init(const HostCsc& P, const HostCsc& A, ConeSet* cs, const cipm_
   th_csr.join();
   if (rc_csr) return rc_csr;
   std::vector<signed char> ds8(dsigns.begin(), dsigns.end());
-  if (upv(&d_map_P, map_P) || upv(&d_map_A, map_A) || upv(&d_map_Hs, map_Hs) || upv(&d_map_u, map_u) ||
-      upv(&d_map_v, map_v) || upv(&d_map_D, map_D) || upv(&d_map_diag, map_diag) || upv(&d_dsigns, ds8) ||
-      upv(&d_map_gqr, map_gqr) || upv(&d_map_gp, map_gp) || upv(&d_map_gD, map_gD))
-    return CLDL_E_CUDA;
+  SCK(upload(&d_map_P, map_P)); SCK(upload(&d_map_A, map_A)); SCK(upload(&d_map_Hs, map_Hs));
+  SCK(upload(&d_map_u, map_u)); SCK(upload(&d_map_v, map_v)); SCK(upload(&d_map_D, map_D));
+  SCK(upload(&d_map_diag, map_diag)); SCK(upload(&d_dsigns, ds8));
+  SCK(upload(&d_map_gqr, map_gqr)); SCK(upload(&d_map_gp, map_gp)); SCK(upload(&d_map_gD, map_gD));
   SCK(cudaMalloc((void**)&d_Hs, (size_t)(cones->nHs ? cones->nHs : 1) * 8));
   SCK(cudaMalloc((void**)&d_x, (size_t)N * 8)); SCK(cudaMalloc((void**)&d_b, (size_t)N * 8));
   SCK(cudaMalloc((void**)&d_w1, (size_t)N * 8)); SCK(cudaMalloc((void**)&d_w2, (size_t)N * 8));
@@ -683,8 +543,10 @@ class IPM {
   std::vector<char> keep;        // presolve row mask over the caller's rows, empty = nothing dropped
   cipm_settings set{};
   HostCsc P, A;  // equilibrated copies (host)
-  std::vector<double> q, b, d, dinv, e, einv;
-  double c = 1.0, normq = 0, normb = 0;
+  std::vector<double> q, b;
+  Equilibration eq;
+  double normq = 0, normb = 0;
+  CsrMap hPsym, hAcsr;   // patterns of Psym and Acsr, and where their values sit in P's and A's CSC arrays
   ConeSet cones;
   KKTDevice kkt;
   Scalars sc;
@@ -721,10 +583,9 @@ class IPM {
   int init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const double* Pxv, const double* q_,
            const uint64_t* Ap, const uint64_t* Ai, const double* Axv, const double* b_, uint64_t ncones,
            const int32_t* ctype, const uint64_t* cdim, const cipm_settings& s, const cldl_opts& lo,
-           const int* perm, const double* cparam = nullptr, const uint64_t* gp_dim2 = nullptr,
+           const uint64_t* perm, const double* cparam = nullptr, const uint64_t* gp_dim2 = nullptr,
            const double* gp_alpha = nullptr);
   void release();
-  void equilibrate();
   int upload_problem();
   int solve();
   // pieces
@@ -750,7 +611,7 @@ class IPM {
   // Solved / AlmostSolved until the data changes.  The scratch below is allocated by the first call.
   bool deriv_valid = false;
   struct DerivWS {
-    int *map_Psym = nullptr, *map_Acsr = nullptr;   // CSC position of every entry of Psym / Acsr
+    int *map_Psym = nullptr, *map_Acsr = nullptr;   // hPsym.src, hAcsr.src
     int *Pcp = nullptr, *Pri = nullptr;             // P's upper triangle as CSC (the caller's order)
     double* arena = nullptr;
     double *xo, *vn0, *vn1, *vn2, *rn, *an, *on0, *on1;                  // length n
@@ -767,129 +628,19 @@ class IPM {
   int deriv_solve();
 };
 
-void IPM::equilibrate() {
-  // Ruiz equilibration on the host, one-time (problemdata.rs:229-312)
-  d.assign(n, 1.0); dinv.assign(n, 1.0); e.assign(m, 1.0); einv.assign(m, 1.0); c = 1.0;
-  if (!set.equilibrate_enable) return;
-  std::vector<double>&dw = dinv, &ew = einv;
-  const double smin = set.equilibrate_min_scaling, smax = set.equilibrate_max_scaling;
-  auto clip = [](double v, double lo, double hi) { return v < lo ? lo : (v > hi ? hi : v); };
-  auto scale_data = [&](const double* dd_, const double* ee_) {
-    if (dd_) {
-      for (int col = 0; col < n; col++)
-        for (int64_t t = P.colptr[col]; t < P.colptr[col + 1]; t++) P.nzval[t] *= dd_[P.rowval[t]] * dd_[col];
-      for (int col = 0; col < n; col++)
-        for (int64_t t = A.colptr[col]; t < A.colptr[col + 1]; t++) A.nzval[t] *= ee_[A.rowval[t]] * dd_[col];
-      for (int i = 0; i < n; i++) q[i] *= dd_[i];
-    } else {
-      for (int64_t t = 0; t < A.colptr[n]; t++) A.nzval[t] *= ee_[A.rowval[t]];
-    }
-    for (int i = 0; i < m; i++) b[i] *= ee_[i];
-  };
-  for (int it = 0; it < set.equilibrate_max_iter; it++) {
-    std::fill(dw.begin(), dw.end(), 0.0);
-    for (int i = 0; i < n; i++)
-      for (int64_t t = P.colptr[i]; t < P.colptr[i + 1]; t++) {
-        const double v = std::fabs(P.nzval[t]);
-        const int r = P.rowval[t];
-        dw[i] = std::max(dw[i], v); dw[r] = std::max(dw[r], v);
-      }
-    for (int i = 0; i < n; i++)
-      for (int64_t t = A.colptr[i]; t < A.colptr[i + 1]; t++) dw[i] = std::max(dw[i], std::fabs(A.nzval[t]));
-    std::fill(ew.begin(), ew.end(), 0.0);
-    for (int64_t t = 0; t < A.colptr[n]; t++) ew[A.rowval[t]] = std::max(ew[A.rowval[t]], std::fabs(A.nzval[t]));
-    for (auto& v : dw) { if (v == 0.0) v = 1.0; v = 1.0 / std::sqrt(v); }
-    for (auto& v : ew) { if (v == 0.0) v = 1.0; v = 1.0 / std::sqrt(v); }
-    for (int i = 0; i < n; i++) dw[i] = clip(dw[i], smin / d[i], smax / d[i]);
-    for (int i = 0; i < m; i++) ew[i] = clip(ew[i], smin / e[i], smax / e[i]);
-    scale_data(dw.data(), ew.data());
-    for (int i = 0; i < n; i++) d[i] *= dw[i];
-    for (int i = 0; i < m; i++) e[i] *= ew[i];
-    double meanP = 0.0, infq = 0.0;
-    for (int i = 0; i < n; i++) {
-      double v = 0.0;
-      for (int64_t t = P.colptr[i]; t < P.colptr[i + 1]; t++) v = std::max(v, std::fabs(P.nzval[t]));
-      meanP += v;
-    }
-    meanP = n ? meanP / n : 0.0;
-    for (int i = 0; i < n; i++) infq = std::max(infq, std::fabs(q[i]));
-    if (meanP != 0.0 && infq != 0.0) {
-      const double ct = clip(1.0 / std::max(infq, meanP), smin / c, smax / c);
-      for (auto& v : P.nzval) v *= ct;
-      for (auto& v : q) v *= ct;
-      c *= ct;
-    }
-  }
-  bool changed = false;
-  std::fill(ew.begin(), ew.end(), 1.0);
-  for (size_t k = 0; k < cones.cones.size(); k++)
-    if (cones.cones[k].type == CT_SOC || cones.cones[k].type == CT_PSD || cones.cones[k].type == CT_EXP ||
-        cones.cones[k].type == CT_POW || cones.cones[k].type == CT_GENPOW) {  // scalar scaling inside these cones (socone.rs:97-101, psdtrianglecone.rs:98-101, expcone.rs:71-74, powcone.rs:63-66)
-      const int o = cones.off[k], dm = cones.cones[k].dim;
-      double mean = 0.0;
-      for (int i = 0; i < dm; i++) mean += e[o + i];
-      mean /= dm;
-      for (int i = 0; i < dm; i++) ew[o + i] = (1.0 / e[o + i]) * mean;
-      changed = true;
-    }
-  if (changed) { scale_data(nullptr, ew.data()); for (int i = 0; i < m; i++) e[i] *= ew[i]; }
-  for (int i = 0; i < n; i++) dinv[i] = 1.0 / d[i];
-  for (int i = 0; i < m; i++) einv[i] = 1.0 / e[i];
-}
-
-// CSR of a CSC matrix; src (if given) receives, for every CSR entry, the position of its value in the CSC arrays
-static void csc_to_csr(const HostCsc& M, std::vector<int>& rp, std::vector<int>& ci, std::vector<double>& v,
-                       std::vector<int>* src = nullptr) {
-  rp.assign(M.m + 1, 0);
-  const int64_t nnz = M.colptr[M.n];
-  for (int64_t t = 0; t < nnz; t++) rp[M.rowval[t] + 1]++;
-  for (int i = 0; i < M.m; i++) rp[i + 1] += rp[i];
-  ci.resize(nnz); v.resize(nnz);
-  if (src) src->resize(nnz);
-  std::vector<int> pos(rp.begin(), rp.end() - 1);
-  for (int j = 0; j < M.n; j++)
-    for (int64_t t = M.colptr[j]; t < M.colptr[j + 1]; t++) {
-      int d = pos[M.rowval[t]]++; ci[d] = j; v[d] = M.nzval[t];
-      if (src) (*src)[d] = (int)t;
-    }
-}
-
-// full symmetric CSR of an upper-triangular CSC matrix (P): row pointers, columns, and for every entry the position of
-// its value in the CSC arrays (an off-diagonal entry appears twice, at (i, j) and at (j, i))
-static void triu_to_sym_csr(const HostCsc& M, std::vector<int>& rp, std::vector<int>& ci, std::vector<int>& src) {
-  const int n = M.n;
-  rp.assign(n + 1, 0);
-  for (int j = 0; j < n; j++)
-    for (int64_t t = M.colptr[j]; t < M.colptr[j + 1]; t++) { rp[M.rowval[t] + 1]++; if (M.rowval[t] != j) rp[j + 1]++; }
-  for (int i = 0; i < n; i++) rp[i + 1] += rp[i];
-  ci.resize(rp[n]); src.resize(rp[n]);
-  std::vector<int> pos(rp.begin(), rp.end() - 1);
-  for (int j = 0; j < n; j++)
-    for (int64_t t = M.colptr[j]; t < M.colptr[j + 1]; t++) {
-      const int i = M.rowval[t];
-      ci[pos[i]] = j; src[pos[i]++] = (int)t;
-      if (i != j) { ci[pos[j]] = i; src[pos[j]++] = (int)t; }
-    }
-}
-
 int IPM::upload_problem() {
   // A as CSR (A x) and A' as CSR (== A in CSC) ; P as full symmetric CSR
-  std::vector<int> rp, ci; std::vector<double> vv;
-  csc_to_csr(A, rp, ci, vv);
-  if (upv(&dAr, rp) || upv(&dAc, ci) || upv(&dAv, vv)) return CLDL_E_CUDA;
+  hAcsr = csc_to_csr(A);
+  SCK(upload(&dAr, hAcsr.rowptr)); SCK(upload(&dAc, hAcsr.col)); SCK(upload(&dAv, gather(A.nzval, hAcsr.src)));
   Acsr.nrows = m; Acsr.rowptr = dAr; Acsr.col = dAc; Acsr.val = dAv;
   std::vector<int> cp32(A.colptr.begin(), A.colptr.end());
-  if (upv(&dAtr, cp32) || upv(&dAtc, A.rowval) || upv(&dAtv, A.nzval)) return CLDL_E_CUDA;
+  SCK(upload(&dAtr, cp32)); SCK(upload(&dAtc, A.rowval)); SCK(upload(&dAtv, A.nzval));
   Atcsr.nrows = n; Atcsr.rowptr = dAtr; Atcsr.col = dAtc; Atcsr.val = dAtv;
-  {
-    std::vector<int> cnt, col, src;
-    triu_to_sym_csr(P, cnt, col, src);
-    std::vector<double> val(src.size());
-    for (size_t k = 0; k < src.size(); k++) val[k] = P.nzval[src[k]];
-    if (upv(&dPr, cnt) || upv(&dPc, col) || upv(&dPv, val)) return CLDL_E_CUDA;
-    Psym.nrows = n; Psym.rowptr = dPr; Psym.col = dPc; Psym.val = dPv;
-  }
-  if (upv(&dq, q) || upv(&db, b) || upv(&dd, d) || upv(&ddinv, dinv) || upv(&de, e) || upv(&deinv, einv)) return CLDL_E_CUDA;
+  hPsym = triu_to_sym_csr(n, P.colptr.data(), P.rowval.data());
+  SCK(upload(&dPr, hPsym.rowptr)); SCK(upload(&dPc, hPsym.col)); SCK(upload(&dPv, gather(P.nzval, hPsym.src)));
+  Psym.nrows = n; Psym.rowptr = dPr; Psym.col = dPc; Psym.val = dPv;
+  SCK(upload(&dq, q)); SCK(upload(&db, b)); SCK(upload(&dd, eq.d)); SCK(upload(&ddinv, eq.dinv));
+  SCK(upload(&de, eq.e)); SCK(upload(&deinv, eq.einv));
   return 0;
 }
 
@@ -901,20 +652,13 @@ int IPM::update_data(const double* Pnz, const double* qv, const double* Anz, con
   SCK(cudaSetDevice(kkt.ldl.device));
   deriv_valid = false;                    // the last solve no longer belongs to this data
   if (Pnz) {
-    for (int j = 0; j < n; j++)
-      for (int64_t t = P.colptr[j]; t < P.colptr[j + 1]; t++) P.nzval[t] = Pnz[t] * d[P.rowval[t]] * d[j] * c;
-    // same traversal as upload_problem: values of the full symmetric CSR
-    std::vector<int> cnt, col, src;
-    triu_to_sym_csr(P, cnt, col, src);
-    std::vector<double> val(src.size());
-    for (size_t k = 0; k < src.size(); k++) val[k] = P.nzval[src[k]];
+    eq.scale_P(P, Pnz);
+    const std::vector<double> val = gather(P.nzval, hPsym.src);
     if (!val.empty()) SCK(cudaMemcpy((void*)dPv, val.data(), val.size() * 8, cudaMemcpyHostToDevice));
   }
   if (Anz) {
-    for (int j = 0; j < n; j++)
-      for (int64_t t = A.colptr[j]; t < A.colptr[j + 1]; t++) A.nzval[t] = Anz[t] * e[A.rowval[t]] * d[j];
-    std::vector<int> rp, ci; std::vector<double> vv;
-    csc_to_csr(A, rp, ci, vv);
+    eq.scale_A(A, Anz);
+    const std::vector<double> vv = gather(A.nzval, hAcsr.src);
     if (!vv.empty()) {
       SCK(cudaMemcpy((void*)dAv, vv.data(), vv.size() * 8, cudaMemcpyHostToDevice));
       SCK(cudaMemcpy((void*)dAtv, A.nzval.data(), A.nzval.size() * 8, cudaMemcpyHostToDevice));
@@ -925,14 +669,11 @@ int IPM::update_data(const double* Pnz, const double* qv, const double* Anz, con
     if (rc) return rc;
   }
   if (qv) {
-    normq = 0;
-    for (int i = 0; i < n; i++) { q[i] = qv[i] * d[i] * c; normq = std::max(normq, std::fabs(q[i] * dinv[i])); }
-    normq /= c;                           // problemdata.rs:147-189: unscaled norm recomputed from the scaled data
+    normq = eq.scale_q(q, qv);
     if (n) SCK(cudaMemcpy((void*)dq, q.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
   }
   if (bv) {
-    normb = 0;
-    for (int i = 0; i < m; i++) { b[i] = bv[i] * e[i]; normb = std::max(normb, std::fabs(b[i] * einv[i])); }
+    normb = eq.scale_b(b, bv);
     if (m) SCK(cudaMemcpy((void*)db, b.data(), (size_t)m * 8, cudaMemcpyHostToDevice));
   }
   SCK(cudaDeviceSynchronize());      // pageable-memory copies above: landed before anything on the solver's streams reads them
@@ -942,98 +683,38 @@ int IPM::update_data(const double* Pnz, const double* qv, const double* Anz, con
 int IPM::init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const double* Pxv, const double* q_,
               const uint64_t* Ap, const uint64_t* Ai, const double* Axv, const double* b_, uint64_t ncones,
               const int32_t* ctype, const uint64_t* cdim, const cipm_settings& s_, const cldl_opts& lo,
-              const int* perm, const double* cparam, const uint64_t* gp_dim2, const double* gp_alpha) {
+              const uint64_t* perm, const double* cparam, const uint64_t* gp_dim2, const double* gp_alpha) {
   n = n_; m = m_; set = s_;
-  // the sparse inputs as CscMatrix::check_format would see them (algebra/csc/core.rs): column pointers start at 0 and
-  // never decrease, row indices are in range and strictly increasing inside a column (sorted, no duplicates); P upper
-  // triangular.  The assembly below relies on it (the diagonal of a P column is its LAST entry, kkt_assembly.rs:20-60)
-  // and the equilibration indexes vectors by row: an unchecked caller would get a silently wrong KKT matrix or a
-  // write out of bounds.  Checked before a device is touched.
-  {
-    auto check = [](const uint64_t* cp, const uint64_t* ri, uint64_t rows, int cols, bool triu) {
-      if (!cp || cp[0] != 0) return (int)CLDL_E_ARG;
-      for (int j = 0; j < cols; j++) if (cp[j + 1] < cp[j]) return (int)CLDL_E_ARG;
-      if (cp[cols] > 0 && !ri) return (int)CLDL_E_ARG;
-      for (int j = 0; j < cols; j++)
-        for (uint64_t t = cp[j]; t < cp[j + 1]; t++) {
-          if (ri[t] >= rows) return (int)CLDL_E_DIM;
-          if (t > cp[j] && ri[t] <= ri[t - 1]) return (int)CLDL_E_ARG;
-          if (triu && ri[t] > (uint64_t)j) return (int)CLDL_E_NOT_TRIU;
-        }
-      return 0;
-    };
-    int vrc = check(Pp, Pi, (uint64_t)n, n, true);
-    if (vrc) return vrc;
-    if ((vrc = check(Ap, Ai, (uint64_t)m, n, false))) return vrc;
-  }
+  // checked before a device is touched
+  int rc = check_csc(Pp, Pi, (uint64_t)n, n, true);
+  if (rc || (rc = check_csc(Ap, Ai, (uint64_t)m, n, false))) return rc;
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
     std::fprintf(stderr, "[clarabel_b200] no CUDA device: this backend has no CPU fallback\n");
     return CLDL_E_CUDA;
   }
   SCK(cudaSetDevice(lo.device));
-  P.m = P.n = n; P.colptr.assign(Pp, Pp + n + 1); P.rowval.assign(Pi, Pi + Pp[n]); P.nzval.assign(Pxv, Pxv + Pp[n]);
-  A.m = m; A.n = n; A.colptr.assign(Ap, Ap + n + 1); A.rowval.assign(Ai, Ai + Ap[n]); A.nzval.assign(Axv, Axv + Ap[n]);
-  for (int j = 0; j < n; j++)
-    for (int64_t t = P.colptr[j]; t < P.colptr[j + 1]; t++) if (P.rowval[t] > j) return CLDL_E_NOT_TRIU;
+  P = host_csc(n, n, Pp, Pi, Pxv);
+  A = host_csc(m, n, Ap, Ai, Axv);
   q.assign(q_, q_ + n); b.assign(b_, b_ + m);
-  infbound = g_infinity.load();
-  for (auto& v : b) v = std::min(v, infbound);  // problemdata.rs:130-131
   std::vector<ConeSpec> cs;
-  int rc = ConeSet::collapse(ctype, cdim, ncones, cs, cparam, gp_dim2, gp_alpha);
-  if (rc) return rc;
+  if ((rc = collapse_cones(ctype, cdim, ncones, cs, cparam, gp_dim2, gp_alpha))) return rc;
   cones.ns_amin = set.min_terminate_step_length; cones.ns_step = set.linesearch_backtrack_step;
   if (lo.shard_nranks > 1) pair_solves = false;   // a sharded factorisation runs its exchanges on one solve context
-  int tot = 0;
-  for (auto& cc : cs) tot += cc.dim;
-  if (tot != m) return CLDL_E_DIM;
-  // inf-bound presolve (presolver.rs:75-125, 157-204; problemdata.rs:86-93): rows of nonnegative cones whose bound
-  // is beyond the infinity bound (b was capped at it just above, which still compares as beyond) leave A, b and
-  // their cone; cipm_get_solution puts them back with s = bound, z = 0
-  mfull = m; keep.clear();
-  if (set.presolve_enable) {
-    const double thr = (1.0 - 2.220446049250313e-16 * 10.0) * infbound;
-    std::vector<char> kp(m, 1);
-    int mred = m, r = 0;
-    for (auto& cc : cs) {
-      if (cc.type == CT_NONNEG) { for (int i = 0; i < cc.dim; i++, r++) if (b[r] > thr) { kp[r] = 0; mred--; } }
-      else r += cc.dim;
-    }
-    if (mred < m) {
-      std::vector<ConeSpec> cs2;
-      r = 0;
-      for (auto& cc : cs) {
-        if (cc.type == CT_NONNEG) {
-          int nk = 0;
-          for (int i = 0; i < cc.dim; i++) nk += kp[r + i];
-          r += cc.dim;
-          if (nk > 0) { ConeSpec c2 = cc; c2.dim = nk; cs2.push_back(c2); }
-        } else { r += cc.dim; cs2.push_back(cc); }
-      }
-      cs.swap(cs2);
-      std::vector<int> rowmap(m, -1);
-      int nr = 0;
-      for (int i = 0; i < m; i++) if (kp[i]) rowmap[i] = nr++;
-      int64_t w = 0;
-      for (int j = 0; j < n; j++) {
-        const int64_t b0 = A.colptr[j];
-        A.colptr[j] = w;
-        for (int64_t t = b0; t < A.colptr[j + 1]; t++)
-          if (rowmap[A.rowval[t]] >= 0) { A.rowval[w] = rowmap[A.rowval[t]]; A.nzval[w] = A.nzval[t]; w++; }
-      }
-      A.colptr[n] = w; A.rowval.resize(w); A.nzval.resize(w); A.m = mred;
-      for (int i = 0; i < m; i++) if (kp[i]) b[rowmap[i]] = b[i];
-      b.resize(mred);
-      keep.swap(kp);
-      m = mred;
-    }
-  }
+  infbound = g_infinity.load();
+  mfull = m;
+  if ((rc = presolve(cs, A, b, infbound, set.presolve_enable != 0, keep))) return rc;
+  m = A.m;
+  ConeLayout layout;
+  if ((rc = cone_layout(cs, layout))) return rc;
+  std::vector<int> kperm;
+  if (perm) kperm = kkt_perm(perm, n, m, layout);
   normq = 0; for (double v : q) normq = std::max(normq, std::fabs(v));
   normb = 0; for (double v : b) normb = std::max(normb, std::fabs(v));
   // cone set needs a stream: borrow the LDL's once it exists -> create ours first
   SCK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   cb_tmark(nullptr);
-  if ((rc = cones.init(cs, st))) return rc;
+  if ((rc = cones.init(layout, st))) return rc;
   cb_tmark("ipm: cone set init");
   // Ruiz equilibration only rescales values: it runs on a host thread next to the pattern work of the KKT
   // layer (assembly maps, ordering, symbolic analysis, plans); the values go in afterwards
@@ -1043,16 +724,15 @@ int IPM::init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const doub
     // needs the equilibrated values
     int rc_up = 0;
     const int devid = lo.device;
-    std::thread eq([this, &rc_up, devid]() {
-      equilibrate();
+    std::thread th([this, &rc_up, devid]() {
+      eq = equilibrate(P, A, q, b, cones, set);
       rc_up = cudaSetDevice(devid) == cudaSuccess ? upload_problem() : CLDL_E_CUDA;
     });
     // joined on every way out of this scope: an exception from kkt.init (std::bad_alloc of a host vector) with the
     // thread still joinable would end the process in std::terminate
-    struct EqJoin { std::thread& t; ~EqJoin() { if (t.joinable()) t.join(); } } eq_guard{eq};
-    kkt.defer_values = true;
-    rc = kkt.init(P, A, &cones, set, lo, perm, st, &sc);
-    eq.join();
+    struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } th_guard{th};
+    rc = kkt.init(P, A, &cones, set, lo, perm ? kperm.data() : nullptr, st, &sc);
+    th.join();
     if (rc || rc_up) { cudaStreamDestroy(st); st = nullptr; return rc ? rc : rc_up; }      // the temporary stream does not leak on the error paths
     if ((rc = kkt.set_PA_values(P, A))) { cudaStreamDestroy(st); st = nullptr; return rc; }
   }
@@ -1137,7 +817,7 @@ int IPM::residuals_update() {
 }
 
 void IPM::info_update(double t0) {
-  const double tinv = 1.0 / tau, cinv = 1.0 / c;
+  const double tinv = 1.0 / tau, cinv = 1.0 / eq.c;
   const double xPx2 = dot_xPx * tinv * tinv / 2.0;
   info.cost_primal = (dot_qx * tinv + xPx2) * cinv;
   info.cost_dual = (-dot_bz * tinv - xPx2) * cinv;
@@ -1488,14 +1168,10 @@ int IPM::deriv_prepare() {
   if (dw.arena) return 0;
   // what an earlier call that failed half way uploaded is freed, not overwritten
   for (int** p : {&dw.map_Psym, &dw.map_Acsr, &dw.Pcp, &dw.Pri}) { dfree(*p); *p = nullptr; }
-  std::vector<int> rp, ci, psrc, asrc;
-  std::vector<double> vv;
-  triu_to_sym_csr(P, rp, ci, psrc);
-  csc_to_csr(A, rp, ci, vv, &asrc);
   std::vector<int> pcp(P.colptr.begin(), P.colptr.end());
-  if (upv(&dw.map_Psym, psrc) || upv(&dw.map_Acsr, asrc) || upv(&dw.Pcp, pcp) || upv(&dw.Pri, P.rowval))
-    return CLDL_E_CUDA;
-  const size_t nnzP = (size_t)P.colptr[n], nnzA = (size_t)A.colptr[n], nnzPs = psrc.size();
+  SCK(upload(&dw.map_Psym, hPsym.src)); SCK(upload(&dw.map_Acsr, hAcsr.src));
+  SCK(upload(&dw.Pcp, pcp)); SCK(upload(&dw.Pri, P.rowval));
+  const size_t nnzP = (size_t)P.colptr[n], nnzA = (size_t)A.colptr[n], nnzPs = hPsym.src.size();
   const size_t total = 8 * (size_t)n + 10 * (size_t)m + nnzP + nnzPs + 2 * nnzA;
   double* a = nullptr;
   SCK(cudaMalloc((void**)&a, total * 8));
@@ -1518,7 +1194,7 @@ int IPM::deriv_factor() {
   int rc = deriv_prepare();
   if (rc) return rc;
   g_launches++;
-  k_deriv_point<<<(std::max(n, m) + 255) / 256, 256, 0, st>>>(n, m, x, s, z, dd, de, 1.0 / tau, 1.0 / c, dw.xo, dw.zo,
+  k_deriv_point<<<(std::max(n, m) + 255) / 256, 256, 0, st>>>(n, m, x, s, z, dd, de, 1.0 / tau, 1.0 / eq.c, dw.xo, dw.zo,
                                                               dw.sn, dw.zn);
   double mu = 0.0;
   if (!cones.all_symmetric) {
@@ -1594,11 +1270,11 @@ int IPM::derivative(const double* dPnz, const double* dqv, const double* dAnz, c
     V.zero(dw.vm1, m);
   }
   g_launches++;
-  k_deriv_rhs<<<grid, 256, 0, st>>>(n, m, c, dd, de, dw.vn0, dw.vn1, dw.vn2, dw.vm0, dw.vm1, dw.rn, dw.rm);
+  k_deriv_rhs<<<grid, 256, 0, st>>>(n, m, eq.c, dd, de, dw.vn0, dw.vn1, dw.vn2, dw.vm0, dw.vm1, dw.rn, dw.rm);
   if ((rc = deriv_solve())) return rc;
   spmv(Acsr, dw.rm, dw.an, -1.0, 1.0);     // E r2 - Â a
   g_launches++;
-  k_deriv_unscale<<<grid, 256, 0, st>>>(n, m, 1.0 / c, dd, de, deinv, dw.an, dw.bm, dw.rm, dw.on0, dw.om0, dw.om1);
+  k_deriv_unscale<<<grid, 256, 0, st>>>(n, m, 1.0 / eq.c, dd, de, deinv, dw.an, dw.bm, dw.rm, dw.on0, dw.om0, dw.om1);
   if ((rc = deriv_download(dxo, dw.on0, n, st)) || (rc = deriv_download(dzo, dw.om0, m, st)) ||
       (rc = deriv_download(dso, dw.om1, m, st)))
     return rc;
@@ -1616,11 +1292,11 @@ int IPM::adjoint_derivative(const double* gx, const double* gz, const double* gs
       (rc = deriv_upload(dw.vm1, gs, m, st)))
     return rc;
   g_launches++;
-  k_adj_rhs<<<grid, 256, 0, st>>>(n, m, c, dd, de, deinv, dw.vn0, dw.vm0, dw.vm1, dw.rn, dw.rm, dw.vm2);
-  if (m) spmv(Atcsr, dw.rn, dw.vm2, -c, 1.0);
+  k_adj_rhs<<<grid, 256, 0, st>>>(n, m, eq.c, dd, de, deinv, dw.vn0, dw.vm0, dw.vm1, dw.rn, dw.rm, dw.vm2);
+  if (m) spmv(Atcsr, dw.rn, dw.vm2, -eq.c, 1.0);
   if ((rc = deriv_solve())) return rc;
   g_launches++;
-  k_adj_unscale<<<grid, 256, 0, st>>>(n, m, 1.0 / c, dd, de, dw.an, dw.bm, dw.vm1, dw.on0, dw.on1, dw.om0);
+  k_adj_unscale<<<grid, 256, 0, st>>>(n, m, 1.0 / eq.c, dd, de, dw.an, dw.bm, dw.vm1, dw.on0, dw.on1, dw.om0);
   const unsigned wgrid = (unsigned)((n + 7) / 8);   // 8 warps of 256 threads: one column each
   if (nnzP) {
     g_launches++;
@@ -1726,30 +1402,9 @@ int cipm_create_gp(cipm_t** out, uint64_t n, uint64_t m, const uint64_t* P_colpt
   if (ldl_opts) lo = *ldl_opts; else cldl_default_opts(&lo);
   cipm_handle* h = new (std::nothrow) cipm_handle();
   if (!h) return CLDL_E_ARG;
-  std::vector<int> perm;
-  // the permutation has the length of the KKT system the constructor will assemble: n + rows left after the inf-bound
-  // presolve + sparse expansion columns.  A dry collapse / presolve count gives it before anything is read.
-  if (kkt_perm_or_null) {
-    std::vector<cb::ConeSpec> cs;
-    if (cb::ConeSet::collapse(cone_types, cone_dims, ncones, cs, cone_params, genpow_dim2, genpow_alpha)) { delete h; return CLDL_E_ARG; }
-    uint64_t p = 0, rows = 0, dropped = 0;
-    const double thr = (1.0 - 2.220446049250313e-16 * 10.0) * g_infinity.load();
-    for (auto& c : cs) {
-      if (c.type == cb::CT_SOC && c.dim > cb::SOC_NO_EXPANSION_MAX_SIZE) p += 2;
-      if (c.type == cb::CT_GENPOW) p += 3;
-      if (c.type == cb::CT_NONNEG && s.presolve_enable && rows + (uint64_t)c.dim <= m)
-        for (int i = 0; i < c.dim; i++) if (b[rows + i] > thr) dropped++;
-      rows += (uint64_t)c.dim;
-    }
-    if (rows != m) { delete h; return CLDL_E_DIM; }
-    const uint64_t N = n + (m - dropped) + p;
-    perm.resize(N);
-    for (uint64_t k = 0; k < N; k++) perm[k] = (int)kkt_perm_or_null[k];
-  }
   const double t_create0 = cb::wall();
   int rc = h->ipm.init((int)n, (int)m, P_colptr, P_rowval, P_nzval, q, A_colptr, A_rowval, A_nzval, b, ncones,
-                       cone_types, cone_dims, s, lo, kkt_perm_or_null ? perm.data() : nullptr, cone_params, genpow_dim2,
-                       genpow_alpha);
+                       cone_types, cone_dims, s, lo, kkt_perm_or_null, cone_params, genpow_dim2, genpow_alpha);
   if (rc) { h->ipm.release(); delete h; return rc; }
   h->ipm.setup_time = cb::wall() - t_create0;
   *out = h;
@@ -1822,22 +1477,12 @@ int cipm_get_solution(cipm_t* h, double* x, double* z, double* s) {
   if (cudaSetDevice(I.kkt.ldl.device) != cudaSuccess) return CLDL_E_CUDA;
   const int st = I.info.status;
   const bool infeas = st == cb::IST_PINF || st == cb::IST_DINF || st == cb::IST_ALMOST_PINF || st == cb::IST_ALMOST_DINF;
-  const double scaleinv = infeas ? 1.0 / I.kap : 1.0 / I.tau, cinv = 1.0 / I.c;
+  const double scaleinv = infeas ? 1.0 / I.kap : 1.0 / I.tau;
   std::vector<double> hx(I.n), hz(I.m), hs(I.m);
   if (I.n && cudaMemcpy(hx.data(), I.x, (size_t)I.n * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return CLDL_E_CUDA;
   if (I.m && cudaMemcpy(hz.data(), I.z, (size_t)I.m * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return CLDL_E_CUDA;
   if (I.m && cudaMemcpy(hs.data(), I.s, (size_t)I.m * 8, cudaMemcpyDeviceToHost) != cudaSuccess) return CLDL_E_CUDA;
-  for (int i = 0; i < I.n; i++) x[i] = hx[i] * I.d[i] * scaleinv;
-  if (I.keep.empty()) {
-    for (int i = 0; i < I.m; i++) z[i] = hz[i] * I.e[i] * (scaleinv * cinv);
-    for (int i = 0; i < I.m; i++) s[i] = hs[i] * I.einv[i] * scaleinv;
-  } else {   // reverse_presolve (presolver.rs:127-150)
-    int c = 0;
-    for (int i = 0; i < I.mfull; i++) {
-      if (I.keep[i]) { z[i] = hz[c] * I.e[c] * (scaleinv * cinv); s[i] = hs[c] * I.einv[c] * scaleinv; c++; }
-      else { z[i] = 0.0; s[i] = I.infbound; }
-    }
-  }
+  cb::unscale_solution(I.eq, I.keep, I.infbound, scaleinv, I.n, I.mfull, hx.data(), hz.data(), hs.data(), x, z, s);
   return CLDL_OK;
 }
 
@@ -1888,9 +1533,9 @@ uint64_t cipm_m_reduced(const cipm_t* h) { return h ? (uint64_t)h->ipm.m : 0; }
 int cipm_get_equilibration(const cipm_t* h, double* d, double* e, double* c) {
   if (!h) return CLDL_E_ARG;
   const cb::IPM& I = h->ipm;
-  if (d) for (int i = 0; i < I.n; i++) d[i] = I.d[i];
-  if (e) for (int i = 0; i < I.m; i++) e[i] = I.e[i];
-  if (c) *c = I.c;
+  if (d) for (int i = 0; i < I.n; i++) d[i] = I.eq.d[i];
+  if (e) for (int i = 0; i < I.m; i++) e[i] = I.eq.e[i];
+  if (c) *c = I.eq.c;
   return CLDL_OK;
 }
 uint64_t cipm_kkt_dim(const cipm_t* h) { return h ? (uint64_t)h->ipm.kkt.N : 0; }

@@ -16,6 +16,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <vector>
 
 namespace cb {
 
@@ -200,6 +201,17 @@ __global__ void k_map(int n, F f) {
 inline int red_grid(int n) {
   int g = (n + RED_THREADS - 1) / RED_THREADS;
   return g < 1 ? 1 : (g > RED_BLOCKS ? RED_BLOCKS : g);
+}
+
+// a device copy of v in *dst, at least one element long so that an empty vector still gets a pointer the kernels may
+// be passed; *dst is set as soon as the allocation succeeds, so that a failed copy leaves nothing unowned
+template <class D, class T>
+inline cudaError_t upload(D** dst, const std::vector<T>& v) {
+  T* p = nullptr;
+  cudaError_t e = cudaMalloc((void**)&p, (v.size() ? v.size() : 1) * sizeof(T));
+  if (e != cudaSuccess) return e;
+  *dst = reinterpret_cast<D*>(p);
+  return v.empty() ? cudaSuccess : cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
 }
 
 }  // namespace cb

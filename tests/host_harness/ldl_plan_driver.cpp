@@ -1,5 +1,6 @@
 // TEST INFRASTRUCTURE ONLY -- builds the LDL factorisation and solve plans of one KKT matrix on the host
-// (csrc/ldl_plan.cpp, no CUDA runtime) and writes them out for tests/test_ldl_plan_cpu.py to check.
+// (csrc/ldl_plan.cpp, no CUDA runtime) and writes them out for tests/test_ldl_plan_cpu.py and
+// tests/test_ldl_shapes_cpu.py to check.
 //
 // usage: ldl_plan_driver <in> <out>
 //   in : int64 n, nnz, nranks, has_perm; int64 Ap[n+1]; int32 Ai[nnz]; int32 perm[n] when has_perm
@@ -44,6 +45,8 @@ static void put_plans(const std::string& p, const Symbolic& S, const std::vector
   PUT_FIELD(f, fp.tasks, DFTask, kind); PUT_FIELD(f, fp.tasks, DFTask, s); PUT_FIELD(f, fp.tasks, DFTask, a);
   PUT_FIELD(f, fp.tasks, DFTask, b); PUT_FIELD(f, fp.tasks, DFTask, d0); PUT_FIELD(f, fp.tasks, DFTask, d1);
   PUT_FIELD(f, fp.tasks, DFTask, e0); PUT_FIELD(f, fp.tasks, DFTask, e1);
+  PUT_FIELD(f, fp.tasks, DFTask, ns); PUT_FIELD(f, fp.tasks, DFTask, nr); PUT_FIELD(f, fp.tasks, DFTask, ndense);
+  put(f + "rec.contig", col(fp.recs, &DFChildRec::contig));
   put(f + "cnt_init", fp.cnt_init);
   put(f + "ntask_owned", std::vector<int>{fp.ntask_owned});
   put(f + "big_pos", fp.big_pos);
@@ -56,10 +59,13 @@ static void put_plans(const std::string& p, const Symbolic& S, const std::vector
   PUT_FIELD(s, sp.tasks, SVTask, kind); PUT_FIELD(s, sp.tasks, SVTask, s); PUT_FIELD(s, sp.tasks, SVTask, cnt);
   PUT_FIELD(s, sp.tasks, SVTask, dep0); PUT_FIELD(s, sp.tasks, SVTask, dep1); PUT_FIELD(s, sp.tasks, SVTask, dep2);
   PUT_FIELD(s, sp.tasks, SVTask, bslot); PUT_FIELD(s, sp.tasks, SVTask, ptask); PUT_FIELD(s, sp.tasks, SVTask, nrt);
+  PUT_FIELD(s, sp.tasks, SVTask, ns); PUT_FIELD(s, sp.tasks, SVTask, nr); PUT_FIELD(s, sp.tasks, SVTask, r0);
+  PUT_FIELD(s, sp.tasks, SVTask, r1);
   put(s + "cnt_init", sp.cnt_init);
   put(s + "ntask_owned", std::vector<int>{sp.ntask_owned});
   put(s + "fronts", sp.fronts); put(s + "front2task", sp.front2task);
   put(s + "leaf1", sp.leaf1); put(s + "leafn", sp.leafn); put(s + "leafw", sp.leafw);
+  put(s + "wide", sp.wide);
   put(s + "gat_ptr", sp.gat_ptr); put(s + "gat_src", sp.gat_src);
 }
 

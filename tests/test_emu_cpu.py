@@ -25,7 +25,7 @@ TOO_BIG = ["tests/test_ipm_gpu.py::test_random_sparse_qp_same_iterations[2000-40
 
 
 # ---- the whole product, multifrontal kernels included (tests/emu/libclarabel_emu_full.so) ----
-FULL_MODULES = ["tests/test_ldl_gpu.py", "tests/test_zz_shard_gpu.py"] + MODULES
+FULL_MODULES = ["tests/test_ldl_gpu.py", "tests/test_ldl_shapes_gpu.py", "tests/test_zz_shard_gpu.py"] + MODULES
 FULL_SKIP = [
     # minutes each under emulation (they pass: 68 of 68 in the complete run recorded in DESIGN.md)
     "tests/test_ipm_gpu.py::test_paired_solves_are_bitwise_the_unpaired_ones",
@@ -61,7 +61,8 @@ atexit.register(_reap)
 def _spec(kind, order):
     full = kind == "full" or kind == "full-ldl"
     lib = os.path.join(ROOT, "tests", "emu", "libclarabel_emu_full.so" if full else "libclarabel_emu.so")
-    modules = {"dense": MODULES, "full": FULL_MODULES, "full-ldl": ["tests/test_ldl_gpu.py", "tests/test_zz_shard_gpu.py"]}[kind]
+    modules = {"dense": MODULES, "full": FULL_MODULES, "full-ldl": ["tests/test_ldl_gpu.py", "tests/test_ldl_shapes_gpu.py",
+                                                                   "tests/test_zz_shard_gpu.py"]}[kind]
     cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider"] + modules
     for t in (FULL_SKIP if full else TOO_BIG):
         cmd += ["--deselect", t]

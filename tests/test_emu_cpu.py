@@ -16,12 +16,21 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 MODULES = ["tests/test_cones_gpu.py", "tests/test_psd_gpu.py", "tests/test_ipm_gpu.py", "tests/test_zz_nonsym_gpu.py",
            "tests/test_zz_golden.py", "tests/test_zz_psd_large_gpu.py", "tests/test_zz_equilibration_gpu.py",
-           "tests/test_zz_data_updating_gpu.py", "tests/test_zz_algebra_gpu.py"]
+           "tests/test_zz_data_updating_gpu.py", "tests/test_zz_algebra_gpu.py", "tests/test_cone_shapes_gpu.py"]
+# lists of tests/cone_shapes.py whose KKT matrix exceeds the dense stand-in's cap (PSD 64 and up, the 1e5 SOC, the
+# nonnegative pass boundaries); the full build runs PSD(64, 65)
+CONE_SHAPES_BIG = ["psd-n96-97", "psd-n128", "soc-long", "nonneg-75775", "nonneg-75776", "nonneg-75777", "nonneg-300000"]
 # the dense stand-in for the LDL caps the KKT dimension at 3000
 TOO_BIG = ["tests/test_ipm_gpu.py::test_random_sparse_qp_same_iterations[2000-4000-60-2]",
            "tests/test_ipm_gpu.py::test_random_sparse_qp_same_iterations[1500-2000-None-3]",
            "tests/test_ipm_gpu.py::test_paired_solves_are_bitwise_the_unpaired_ones",
            "tests/test_zz_psd_large_gpu.py::test_large_psd_cone_ops_match_oracle[global-scratch]"]     # runs in the full build below
+_SHAPE_TESTS = ["test_scaling_lambda_and_H", "test_combined_shift_and_ds_offset", "test_step_length"]
+_SHAPE_BIG = [f"tests/test_cone_shapes_gpu.py::{t}[{n}-{r}]" for n in CONE_SHAPES_BIG for t in _SHAPE_TESTS
+              for r in ("opening", "late")] + \
+             [f"tests/test_cone_shapes_gpu.py::test_margins[{n}-{r}]" for n in CONE_SHAPES_BIG for r in ("opening", "late", "indefinite")] + \
+             [f"tests/test_cone_shapes_gpu.py::test_nonnegative_pass_boundaries[{n}]" for n in CONE_SHAPES_BIG]
+TOO_BIG += _SHAPE_BIG + [t.replace("[psd-n96-97", "[psd-n64-65") for t in _SHAPE_BIG if "psd-n96-97" in t]
 
 
 # ---- the whole product, multifrontal kernels included (tests/emu/libclarabel_emu_full.so) ----
@@ -37,7 +46,7 @@ FULL_SKIP = [
     # amplified past the test's 1e-7; both thread orders agree bitwise with each other and the regularisation counts
     # equal the oracle's
     "tests/test_ldl_gpu.py::test_dynamic_regularisation_counts",
-]
+] + _SHAPE_BIG
 
 
 

@@ -76,12 +76,53 @@ static NcclApi* nccl_api(const char* libpath) {
 // kernels
 // ------------------------------------------------------------------------
 
-// Fused front kernel: one CTA per front.
+// Inverse of the unit lower triangular pivot block L11 of a front with more than CB_SOLVE_SMALL_NS pivots, for the
+// solves (ldl_solve.cuh), computed where the factorisation has the block.  A: the pivot block, column major with
+// leading dimension lda, L11 in its strictly lower triangle.  Thread j builds column j of X = L11^-1 by forward
+// substitution on e_j (X[j][j] = 1, X[i][j] = -sum_{k=j..i-1} L[i][k] X[k][j], two interleaved partial sums) and
+// keeps it in the upper triangle, X[i][j] at A[i * lda + j], while the other threads still read L11.
+template <int NT>
+__device__ __forceinline__ void pivot_inverse(double* A, int lda, int ns) {
+  for (int j = threadIdx.x; j < ns; j += NT) {
+    for (int i = j + 1; i < ns; i++) {
+      double a0 = A[(long long)j * lda + i], a1 = 0.0;     // k = j term: L[i][j] * X[j][j]
+      int k = j + 1;
+      for (; k + 1 < i; k += 2) {
+        a0 += A[(long long)k * lda + i] * A[(long long)k * lda + j];
+        a1 += A[(long long)(k + 1) * lda + i] * A[(long long)(k + 1) * lda + j];
+      }
+      if (k < i) a0 += A[(long long)k * lda + i] * A[(long long)k * lda + j];
+      A[(long long)i * lda + j] = -(a0 + a1);
+    }
+  }
+}
+// after pivot_inverse and a barrier: X moves to the strictly lower triangle, the upper triangle is zero again
+template <int NT>
+__device__ __forceinline__ void pivot_inverse_place(double* A, int lda, int ns) {
+  for (int idx = threadIdx.x; idx < ns * ns; idx += NT) {
+    const int j = idx / ns, i = idx - j * ns;
+    if (i > j) {
+      A[(long long)j * lda + i] = A[(long long)i * lda + j];
+      A[(long long)i * lda + j] = 0.0;
+    }
+  }
+}
+
+// Tree level 0: one CTA per front with at least two pivots.  Level-0 fronts have no children: the panel is the
+// front's own entries, and U = 0 - L21 D L21^T is written once.
+//   pivot block  right-looking, one barrier per pivot: every thread reads the pivot after the barrier and applies the
+//                sign test / regularisation itself; the columns are scaled (l = a / d) after the last pivot, since
+//                no later pivot reads them
+//   Schur        1 x 4 register tiles: a lane owns one row of U and four columns, a warp 32 rows
+//   inverse      L11^-1 of a wide front, from the panel before it is stored (pivot_inverse)
+// Inertia, regularisation, zero-pivot and non-finite flags: one atomic per counter per CTA.  Every entry receives
+// the same operations in the same order as in a column-by-column factorisation, so the bits do not depend on the
+// schedule.
 template <int NT>
 __global__ void __launch_bounds__(NT) k_factor_level(LDLDev d, int task_base, int smem_cap) {
   extern __shared__ double sm[];
-  __shared__ double s_inv;
   __shared__ double sD[CB_MAX_PANEL];
+  __shared__ double sInv[CB_MAX_PANEL];
   const int tid = threadIdx.x;
   const int lane = tid & 31, warp = tid >> 5, nwarp = NT >> 5;
   const int s = d.level_tasks[task_base + blockIdx.x];
@@ -97,91 +138,103 @@ __global__ void __launch_bounds__(NT) k_factor_level(LDLDev d, int task_base, in
   double* W = use_sm ? sm : P;
 
   for (long long i = tid; i < psz; i += NT) W[i] = 0.0;
-  for (int b = warp; b < nr; b += nwarp)
-    for (int a = b + lane; a < nr; a += 32) U[(long long)b * nr + a] = 0.0;
   __syncthreads();
-
   // original matrix entries (each lands in a distinct slot)
   for (long long e = d.asm_ptr[s] + tid; e < d.asm_ptr[s + 1]; e += NT)
     W[d.asm_dst[e]] = d.vals[d.asm_src[e]];
-  __syncthreads();
 
-  // extend-add of the children's update matrices, fixed child order
-  for (long long ci = d.child_ptr[s]; ci < d.child_ptr[s + 1]; ci++) {
-    const int c = d.child_list[ci];
-    const long long crp = d.sn_rowptr[c];
-    const int nrc = (int)(d.sn_rowptr[c + 1] - crp);
-    const double* __restrict__ Uc = d.U + d.upd_off[c];
-    const int* __restrict__ relc = d.rel + crp;
-    for (int b = warp; b < nrc; b += nwarp) {
-      const int rb = relc[b];
-      for (int a = b + lane; a < nrc; a += 32) {
-        const int ra = relc[a];
-        const double v = Uc[(long long)b * nrc + a];
-        if (rb < ns) W[(long long)rb * ld + ra] += v;
-        else U[(long long)(rb - ns) * nr + (ra - ns)] += v;
-      }
-    }
-    __syncthreads();
-  }
-
-  // dense LDL^T of the panel, right-looking, pivot order = elimination order
+  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0;
   for (int j = 0; j < ns; j++) {
+    __syncthreads();    // column j is final: assembled, and updated by every earlier pivot
+    const double* __restrict__ cj = W + (long long)j * ld;
+    double dj = cj[j];
+    bool reg = false;
+    if (d.reg_enable) {
+      const double sg = (double)d.dsigns[f + j];
+      if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; reg = true; }
+    }
+    const double inv = 1.0 / dj;
     if (tid == 0) {
-      double dj = W[(long long)j * ld + j];
-      if (d.reg_enable) {
-        const double sg = (double)d.dsigns[f + j];
-        if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; atomicAdd(&d.status[ST_REGCOUNT], 1); }
-      }
-      if (dj == 0.0) atomicExch(&d.status[ST_ZEROPIV], 1);
-      if (dj > 0.0) atomicAdd(&d.status[ST_POSINERTIA], 1);
-      const double inv = 1.0 / dj;
-      if (!isfinite(inv)) atomicExch(&d.status[ST_NONFINITE], 1);
+      c_reg += reg ? 1 : 0;
+      c_pos += dj > 0.0 ? 1 : 0;
+      if (dj == 0.0) c_zero = 1;
+      if (!isfinite(inv)) c_nonf = 1;
       d.D[f + j] = dj;
       d.Dinv[f + j] = inv;
-      W[(long long)j * ld + j] = dj;
-      s_inv = inv;
       sD[j] = dj;
+      sInv[j] = inv;
     }
-    __syncthreads();
-    const double inv = s_inv;
-    const double* __restrict__ cj = W + (long long)j * ld;
     for (int k = j + 1 + warp; k < ns; k += nwarp) {
       const double wk = cj[k] * inv;
       double* __restrict__ ck = W + (long long)k * ld;
       for (int i = k + lane; i < ld; i += 32) ck[i] -= cj[i] * wk;
     }
-    __syncthreads();
-    double* cjw = W + (long long)j * ld;
-    for (int i = j + 1 + tid; i < ld; i += NT) cjw[i] *= inv;
+  }
+  __syncthreads();
+  for (int j = warp; j < ns; j += nwarp) {
+    double* __restrict__ cj = W + (long long)j * ld;
+    const double inv = sInv[j];
+    if (lane == 0) cj[j] = sD[j];
+    for (int i = j + 1 + lane; i < ld; i += 32) cj[i] *= inv;
+  }
+  if (tid == 0) {
+    if (c_reg) atomicAdd(&d.status[ST_REGCOUNT], c_reg);
+    if (c_pos) atomicAdd(&d.status[ST_POSINERTIA], c_pos);
+    if (c_zero) atomicExch(&d.status[ST_ZEROPIV], 1);
+    if (c_nonf) atomicExch(&d.status[ST_NONFINITE], 1);
   }
   __syncthreads();
 
-  // Schur update of the lower triangle of U
-  for (int b = warp; b < nr; b += nwarp) {
-    for (int a = b + lane; a < nr; a += 32) {
-      double acc = 0.0;
-      for (int k = 0; k < ns; k++) {
-        const double* __restrict__ ck = W + (long long)k * ld + ns;
-        acc += ck[a] * (ck[b] * sD[k]);
+  // Schur update of the lower triangle of U; warp items (column block of 4, 32-row chunk from the block's diagonal)
+  {
+    int it = 0;
+    for (int b0 = 0; b0 < nr; b0 += 4)
+      for (int a0 = b0; a0 < nr; a0 += 32, it++) {
+        if (it % nwarp != warp) continue;
+        const int a = a0 + lane;
+        const bool on = a < nr;
+        const int nb = min(4, nr - b0);      // columns b0 .. b0 + nb - 1; the others repeat the last one
+        double acc[4] = {0.0, 0.0, 0.0, 0.0};
+        const double* __restrict__ ck = W + ns;
+        for (int k = 0; k < ns; k++, ck += ld) {
+          const double la = on ? ck[a] : 0.0, dk = sD[k];
+#pragma unroll
+          for (int c = 0; c < 4; c++) acc[c] += la * (ck[b0 + min(c, nb - 1)] * dk);
+        }
+#pragma unroll
+        for (int c = 0; c < 4; c++)
+          if (on && b0 + c < nr && a >= b0 + c) U[(long long)(b0 + c) * nr + a] = 0.0 - acc[c];
       }
-      U[(long long)b * nr + a] -= acc;
-    }
+  }
+  // the Schur update reads rows ns.. only: the inverse of the pivot block needs no barrier before it
+  if (ns > CB_SOLVE_SMALL_NS) {
+    pivot_inverse<NT>(W, ld, ns);
+    __syncthreads();
+    pivot_inverse_place<NT>(W, ld, ns);
   }
   if (use_sm) {
+    __syncthreads();
     for (long long i = tid; i < psz; i += NT) P[i] = W[i];
   }
 }
 
 // Single-column leaves (no children: tree level 0; on KKT matrices these are the constraint rows eliminated first,
-// 5e5 of them on config C4): ONE THREAD per front instead of one CTA.  Same arithmetic as the fused kernel above does
-// for such a front: d = a_jj (sign test, regularisation), l = a_:j / d, U = 0 - l (l d)^T on the lower triangle.
-// The inertia / regularisation counters are aggregated per warp before they touch global memory.
-__global__ void __launch_bounds__(256) k_factor_leaf1(LDLDev d, int task_base, int count) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  const bool on = i < count;
-  int pos = 0, reg = 0;
-  if (on) {
+// 5e5 of them on config C4): ONE WARP per front instead of one CTA.  The column is assembled in a per-warp shared
+// buffer, then the lanes store the panel and U = 0 - l (l d)^T (lower triangle) with consecutive lanes on consecutive
+// addresses.  Same arithmetic as the fused kernel above does for such a front: d = a_jj (sign test, regularisation),
+// l = a_:j / d.  The inertia / regularisation counters are aggregated per CTA before they touch global memory.
+#define LEAF1_NT 256
+#define LEAF1_MAXLD 128    /* level-0 fronts that are not big have fewer than CB_BIG_NR rows */
+static_assert(LEAF1_MAXLD > CB_BIG_NR, "a level-0 column must fit the per-warp buffer");
+__global__ void __launch_bounds__(LEAF1_NT) k_factor_leaf1(LDLDev d, int task_base, int count) {
+  __shared__ double s_col[LEAF1_NT / 32][LEAF1_MAXLD];
+  __shared__ int s_pos, s_reg;
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const int i = blockIdx.x * (LEAF1_NT / 32) + warp;
+  if (threadIdx.x == 0) { s_pos = 0; s_reg = 0; }
+  __syncthreads();
+  if (i < count) {
+    double* col = s_col[warp];
     const int s = d.level_tasks[task_base + i];
     const int f = d.sn_first[s];
     const long long rp = d.sn_rowptr[s];
@@ -189,34 +242,46 @@ __global__ void __launch_bounds__(256) k_factor_leaf1(LDLDev d, int task_base, i
     const int ld = 1 + nr;
     double* __restrict__ P = d.L + d.panel_off[s];
     double* __restrict__ U = d.U + d.upd_off[s];
-    for (int a = 0; a < ld; a++) P[a] = 0.0;
-    for (long long e = d.asm_ptr[s]; e < d.asm_ptr[s + 1]; e++) P[d.asm_dst[e]] = d.vals[d.asm_src[e]];
-    double dj = P[0];
+    for (int a = lane; a < ld; a += 32) col[a] = 0.0;
+    __syncwarp();
+    for (long long e = d.asm_ptr[s] + lane; e < d.asm_ptr[s + 1]; e += 32) col[d.asm_dst[e]] = d.vals[d.asm_src[e]];
+    __syncwarp();
+    double dj = col[0];
+    bool reg = false;
     if (d.reg_enable) {
       const double sg = (double)d.dsigns[f];
-      if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; reg = 1; }
+      if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; reg = true; }
     }
-    if (dj == 0.0) atomicExch(&d.status[ST_ZEROPIV], 1);
-    pos = dj > 0.0 ? 1 : 0;
     const double inv = 1.0 / dj;
-    if (!isfinite(inv)) atomicExch(&d.status[ST_NONFINITE], 1);
-    d.D[f] = dj;
-    d.Dinv[f] = inv;
-    P[0] = dj;
-    for (int a = 1; a < ld; a++) P[a] *= inv;
-    for (int b = 0; b < nr; b++) {
-      const double t = P[1 + b] * dj;
-      for (int a = b; a < nr; a++) {
+    if (lane == 0) {
+      if (dj == 0.0) atomicExch(&d.status[ST_ZEROPIV], 1);
+      if (!isfinite(inv)) atomicExch(&d.status[ST_NONFINITE], 1);
+      if (dj > 0.0) atomicAdd(&s_pos, 1);
+      if (reg) atomicAdd(&s_reg, 1);
+      d.D[f] = dj;
+      d.Dinv[f] = inv;
+    }
+    __syncwarp();
+    for (int a = lane; a < ld; a += 32) {
+      const double v = a == 0 ? dj : col[a] * inv;
+      col[a] = v;
+      P[a] = v;
+    }
+    __syncwarp();
+    for (int idx = lane; idx < nr * nr; idx += 32) {
+      const int b = idx / nr, a = idx - b * nr;
+      if (a >= b) {
+        const double t = col[1 + b] * dj;
         double acc = 0.0;
-        acc += P[1 + a] * t;
-        U[(long long)b * nr + a] = 0.0 - acc;
+        acc += col[1 + a] * t;
+        U[idx] = 0.0 - acc;
       }
     }
   }
-  const unsigned mp = __ballot_sync(0xffffffffu, pos != 0), mr = __ballot_sync(0xffffffffu, reg != 0);
-  if ((threadIdx.x & 31) == 0) {
-    if (mp) atomicAdd(&d.status[ST_POSINERTIA], __popc(mp));
-    if (mr) atomicAdd(&d.status[ST_REGCOUNT], __popc(mr));
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (s_pos) atomicAdd(&d.status[ST_POSINERTIA], s_pos);
+    if (s_reg) atomicAdd(&d.status[ST_REGCOUNT], s_reg);
   }
 }
 
@@ -388,6 +453,13 @@ __device__ void dff_small(const LDLDev& d, int s, double* sm, int* s_flag) {
       }
       U[(long long)b * nr + a] -= acc;
     }
+  // the Schur update reads rows ns.. only: the inverse of the pivot block needs no barrier before it
+  if (ns > CB_SOLVE_SMALL_NS) {
+    pivot_inverse<DF_NT>(W, ld, ns);
+    __syncthreads();
+    pivot_inverse_place<DF_NT>(W, ld, ns);
+    __syncthreads();
+  }
   if (use_sm) for (long long i = tid; i < psz; i += DF_NT) P[i] = W[i];
 }
 
@@ -743,6 +815,22 @@ __device__ void dff_rows(const LDLDev& d, const DFFactor& q, const DFTask& tk, d
   }
 }
 
+// ---- the R task that finishes a wide big front: L11^-1 for the solves ----
+// L11 has to stay in the panel until every R task of the front has read it; the last one to finish still holds it
+// in shared memory (sA of dff_rows) and replaces it in the panel by its inverse.  T tasks and the parent never read
+// L11, so this is off the critical path.
+__device__ void dff_rows_invert(const LDLDev& d, const DFTask& tk, double* sm) {
+  double* sA = sm;                                     // [64][CB_PB_LD]  L11, as dff_rows left it
+  const int ns = tk.ns, ld = ns + tk.nr;
+  double* P = d.L + tk.poff;
+  pivot_inverse<DF_NT>(sA, CB_PB_LD, ns);
+  __syncthreads();
+  for (int idx = threadIdx.x; idx < ns * ns; idx += DF_NT) {
+    const int j = idx / ns, i = idx - j * ns;
+    if (i > j) P[(long long)j * ld + i] = sA[i * CB_PB_LD + j];
+  }
+}
+
 // ---- T: one 64x64 tile of the update matrix ----
 __device__ void dff_tile(const LDLDev& d, const DFFactor& q, const DFTask& tk, double* sm, int* s_desc, int* s_ed, double* s_ev) {
   double* sAt = sm;                      // [ns][TS]  L21 rows of tile-row I
@@ -920,6 +1008,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
   __shared__ __align__(16) int s_task[16];
   __shared__ int s_ed[DF_ENT_FAST];
   __shared__ double s_ev[DF_ENT_FAST];
+  __shared__ int s_last;
   const int tid = threadIdx.x;
   if (tid == 0) df_cur_qi = -1;
   for (;;) {
@@ -963,7 +1052,9 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
       __syncthreads();
       dff_rows(d, q, tk, dfsm, s_desc, s_ed, s_ev);
       __syncthreads();
-      if (tid == 0) { __threadfence(); atomicSub(q.rows_left + s, 1); }
+      if (tid == 0) { __threadfence(); s_last = atomicSub(q.rows_left + s, 1) == 1; }
+      __syncthreads();
+      if (s_last && tk.ns > CB_SOLVE_SMALL_NS) dff_rows_invert(d, tk, dfsm);
     } else {
       if (tid == 0) { df_wait_zero(q.rows_left + s); __threadfence(); if (q.trace) q.trace[10 * (size_t)qi + 1] = df_gtime(); }
       __syncthreads();
@@ -1164,14 +1255,12 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   // dataflow solves (ldl_solve.cuh)
   const int nt = (int)sp.tasks.size();
   sv_nwide = (int)sp.wide.size();
-  sv_wide_runs = std::move(sp.wide_runs);
   sv_nleaf1 = (int)sp.leaf1.size(); sv_nleafn = (int)sp.leafn.size(); sv_nleafw = (int)sp.leafw.size();
   sv_leafw_nrmax = sp.leafw_nrmax;
   sv_leafw_grid = sv_nleafw;      // one CTA per front (a loop over fronts inside fewer CTAs was slower: 312 vs 189 us forward on C4)
   sv_ntask_owned = sp.ntask_owned;
   CK(upload(&dev.gat_ptr, sp.gat_ptr));
   CK(upload(&dev.gat_src, sp.gat_src));
-  CK(upload(&d_sv_wide, sp.wide));
   CK(upload(&d_sv_leaf1, sp.leaf1));
   CK(upload(&d_sv_leafn, sp.leafn));
   CK(upload(&d_sv_leafw, sp.leafw));
@@ -1233,7 +1322,7 @@ void LDLObject::release() {
   fr(dev.rel); fr(dev.panel_off); fr(dev.upd_off); fr(dev.asm_ptr); fr(dev.asm_src);
   fr(dev.asm_dst); fr(dev.level_tasks); fr(dev.perm); fr(dev.dsigns); fr(dev.vals); fr(dev.L);
   fr(dev.U); fr(dev.D); fr(dev.Dinv); fr(dev.u); fr(dev.status); fr(d_xp); fr(d_bx);
-  fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_wide); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.recs); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
+  fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.recs); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
   if (h_status) cudaFreeHost(h_status);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
@@ -1251,7 +1340,7 @@ int LDLObject::refactor_level0() {
   CK(cudaMemsetAsync(dff.qhead, 0, sizeof(int), stream));
   g_launches += plan.size();
   for (const LaunchSeg& g : plan) {
-    if (g.leaf1) k_factor_leaf1<<<(g.count + 255) / 256, 256, 0, stream>>>(dev, g.base, g.count);
+    if (g.leaf1) k_factor_leaf1<<<(g.count + LEAF1_NT / 32 - 1) / (LEAF1_NT / 32), LEAF1_NT, 0, stream>>>(dev, g.base, g.count);
     else if (g.threads == 64)
       k_factor_level<64><<<g.count, 64, (size_t)g.smem_doubles * 8, stream>>>(dev, g.base, g.smem_doubles);
     else
@@ -1266,22 +1355,10 @@ int LDLObject::refactor_async() {
   if (int rc = refactor_level0()) return rc;
   g_launches++;
   k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, dff);
-  invert_pivots();
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h_status, dev.status, ST_COUNT * sizeof(int), cudaMemcpyDeviceToHost, stream));
   factored = true;
   return CLDL_OK;
-}
-
-// the solves multiply by the inverse of every wide pivot block (ldl_solve.cuh): strictly lower triangle replaced in place
-void LDLObject::invert_pivots() {
-  if (!sv_nwide) return;
-  g_launches++;
-  // the list is sorted by pivot count: launched in runs of equal width so that each run asks for just its own shared memory
-  for (size_t g = 0; g + 2 < sv_wide_runs.size(); g += 2) {
-    const int first = sv_wide_runs[g], cnt = sv_wide_runs[g + 2] - first, ns = sv_wide_runs[g + 1];
-    k_invert_pivots<<<cnt, 64, (size_t)ns * (ns + 1) * sizeof(double), stream>>>(dev, d_sv_wide + first, cnt);
-  }
 }
 
 int LDLObject::sync_status() {
@@ -1434,7 +1511,6 @@ int LDLObject::refactor_phase_async(int phase) {
   CK(cudaMemcpyAsync(dff.qhead, &h_phase_start[0], sizeof(int), cudaMemcpyHostToDevice, stream));
   g_launches++;
   k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, dff);
-  invert_pivots();
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h_status, dev.status, ST_COUNT * sizeof(int), cudaMemcpyDeviceToHost, stream));
   factored = true;
@@ -1770,6 +1846,26 @@ void cldl_info(const cldl_t* h, cldl_info_t* info) {
 int cldl_get_perm(const cldl_t* h, uint64_t* perm_out) {
   if (!h || !perm_out) return CLDL_E_ARG;
   for (int k = 0; k < h->obj.n; k++) perm_out[k] = (uint64_t)h->obj.S.perm[k];
+  return CLDL_OK;
+}
+
+int cldl_get_factor(const cldl_t* h, double* L_out, double* D_out, double* Dinv_out) {
+  if (!h || !L_out || !D_out || !Dinv_out) return CLDL_E_ARG;
+  const LDLObject& o = h->obj;
+  if (!o.factored) return CLDL_E_NOT_FACTORED;
+  if (cudaSetDevice(o.device) != cudaSuccess || cudaStreamSynchronize(o.stream) != cudaSuccess) return CLDL_E_CUDA;
+  std::vector<double> all((size_t)o.S.L_alloc);
+  if (cudaMemcpy(all.data(), o.dev.L, all.size() * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(D_out, o.dev.D, (size_t)o.n * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(Dinv_out, o.dev.Dinv, (size_t)o.n * sizeof(double), cudaMemcpyDeviceToHost) != cudaSuccess)
+    return CLDL_E_CUDA;
+  // panels start on 32-byte boundaries in device memory; the padding between them is never written
+  size_t pos = 0;
+  for (int s = 0; s < o.S.nsup; s++) {
+    const size_t ns = (size_t)(o.S.sn_first[s + 1] - o.S.sn_first[s]), nr = (size_t)(o.S.sn_rowptr[s + 1] - o.S.sn_rowptr[s]);
+    std::memcpy(L_out + pos, all.data() + o.S.panel_off[s], (ns + nr) * ns * sizeof(double));
+    pos += (ns + nr) * ns;
+  }
   return CLDL_OK;
 }
 

@@ -73,19 +73,17 @@ struct DFFactor {
 
 class LDLObject {
  public:
-  // triangular solves (ldl_solve.cuh): task queue, counters, level-0 leaf lists, wide fronts whose pivot block is inverted
+  // triangular solves (ldl_solve.cuh): task queue, counters, level-0 leaf lists
   SVPlan sv;
-  int *d_sv_init = nullptr, *d_sv_cnt = nullptr, *d_sv_wide = nullptr, *d_sv_leaf1 = nullptr, *d_sv_leafn = nullptr, *d_sv_leafw = nullptr;
+  int *d_sv_init = nullptr, *d_sv_cnt = nullptr, *d_sv_leaf1 = nullptr, *d_sv_leafn = nullptr, *d_sv_leafw = nullptr;
   size_t sv_ninit = 0, sv_nzero = 0, sv_smem[2] = {0, 0};
   int sv_cap = 0, sv_nwide = 0, sv_nleaf1 = 0, sv_nleafn = 0, sv_nleafw = 0, sv_leafw_nrmax = 0, sv_leafw_grid = 1, sv_ntask_owned = 0;
   std::vector<SVTask> h_sv_tasks;
-  std::vector<int> sv_wide_runs;   // (first, widest ns) pairs of the launches of k_invert_pivots, closed by (count, 0)
   int sv_configure();
   int sv_occupancy();
   int sv_reset();
   void sv_sweep(bool fwd, int nrhs, const SVPlan& q, const SVRhs& r);
   void sv_leaves(bool fwd, int nrhs, const SVRhs& r);
-  void invert_pivots();
   DFFactor dff;
   int *d_dff_init = nullptr, *d_dff_cnt = nullptr;
   std::vector<DFTask> h_dff_tasks;

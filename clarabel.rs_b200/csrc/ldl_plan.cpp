@@ -469,20 +469,9 @@ SolvePlan build_solve_plan(const Symbolic& S, const std::vector<int>& owner, int
     const int p = S.sn_parent[s];
     if (p >= 0 && f2t[s] >= 0 && chain_child[p] != s) pend[f2t[p]]++;   // leaves and other ranks' fronts are complete before the sweep starts
   }
-  // wide fronts whose pivot block is inverted after every refactorisation (all that this rank factors), sorted by pivot
-  // count and cut into at most 8 runs (each run is launched with the shared memory of its widest front)
+  // wide fronts whose pivot block the factorisation replaces by its inverse (all that this rank factors)
   const std::vector<char> mine = queued(queue, nsup);
   for (int s = 0; s < nsup; s++) if (wide(s) && mine[s]) P.wide.push_back(s);
-  std::stable_sort(P.wide.begin(), P.wide.end(), [&](int a, int b) { return ns_of(S, a) < ns_of(S, b); });
-  const int nwide = (int)P.wide.size();
-  const int bounds[] = {16, 24, 32, 40, 48, 56, CB_PB_MAXNS};
-  int pos = 0;
-  for (int bd : bounds) {
-    int e = pos;
-    while (e < nwide && ns_of(S, P.wide[e]) <= bd) e++;
-    if (e > pos) { P.wide_runs.push_back(pos); P.wide_runs.push_back(bd); pos = e; }
-  }
-  P.wide_runs.push_back(nwide); P.wide_runs.push_back(0);
   return P;
 }
 

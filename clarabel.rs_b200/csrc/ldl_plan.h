@@ -108,8 +108,7 @@ struct SolvePlan {
   std::vector<int> cnt_init;             // pend (ntask) | fleft (nsup) | bleft (nsup)
   std::vector<int> fronts, front2task;   // narrow batches' fronts; [nsup] head / batch task of a front or -1
   std::vector<int> leaf1, leafn, leafw;  // level-0 leaves solved by plain kernels: one column, narrow, wide
-  std::vector<int> wide;                 // wide fronts whose pivot block is inverted, sorted by pivot count
-  std::vector<int> wide_runs;            // (first, widest ns) pairs of the launches of k_invert_pivots, closed by (count, 0)
+  std::vector<int> wide;                 // wide fronts this rank factors: their pivot blocks hold L11^-1
   std::vector<int> gat_ptr, gat_src;     // per front slot, CSR of contributing child update-vector entries
   int nslots = 0, leafw_nrmax = 0;
   int ntask_owned = 0;

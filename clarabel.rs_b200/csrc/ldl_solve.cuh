@@ -5,7 +5,7 @@
 //
 // Layout the sweeps rely on.  A front s with ns pivots and nr rows below stores its panel (ns+nr) x ns column-major
 // in d.L.  For wide fronts (ns > CB_SOLVE_SMALL_NS) the strictly lower triangle of the pivot block holds
-// L11^-1 (unit diagonal implied), written by k_invert_pivots at the end of every refactorisation: the ns dependent
+// L11^-1 (unit diagonal implied), written by the factorisation where it has the pivot block: the ns dependent
 // substitution steps of a pivot block become one ns x ns matrix-vector product.  Narrow fronts keep L11.
 //
 // Schedule.  Tree level 0 has no dependencies: its narrow fronts are swept by plain kernels before (forward) and
@@ -331,61 +331,6 @@ __global__ void __launch_bounds__(SV_LEAF_NT) k_bwd_leafw(LDLDev d, const int* _
     for (int h = 0; h < NR; h++) { const double x = s0[h * CB_PB_MAXNS + tid]; r.xp[h][f + tid] = x; r.out[h][pf] = x; }
   }
   }
-}
-
-// ---- pivot-block inverses (end of every refactorisation) ----
-// One CTA of 64 threads per wide front: thread j builds column j of X = L11^-1 by forward substitution on e_j
-// (X[j][j] = 1, X[i][j] = -sum_{k=j..i-1} L[i][k] X[k][j]); the strictly lower triangle of X replaces that of L11.
-// Shared memory holds ONE ns x (ns+1) array (dynamic, sized by the widest front of the launch): L11 row-major in the
-// strictly lower triangle (sA[i][k], k < i), column j of X in ROW j of the upper triangle (sA[j][i], i > j) -- both
-// patterns are conflict-free.  The launch is ordered by ns (host side) so that co-resident CTAs have similar work.
-__global__ void __launch_bounds__(64) k_invert_pivots(LDLDev d, const int* __restrict__ wide, int count) {
-  extern __shared__ double sA[];
-  const int s = wide[blockIdx.x];
-  const int f = d.sn_first[s];
-  const int ns = d.sn_first[s + 1] - f;
-  const int ld = ns + (int)(d.sn_rowptr[s + 1] - d.sn_rowptr[s]);
-  double* __restrict__ P = d.L + d.panel_off[s];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int LDS = ns | 1;             // odd
-  // columns two per pass and warp (independent loads in flight), lanes down the column
-  for (int j0 = 0; j0 < ns; j0 += 8) {
-    double v[4][2];
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-      const int j = j0 + 2 * c + w;
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int i = lane + 32 * h;
-        v[c][h] = (j < ns && i > j && i < ns) ? P[(long long)j * ld + i] : 0.0;
-      }
-    }
-#pragma unroll
-    for (int c = 0; c < 4; c++) {
-      const int j = j0 + 2 * c + w;
-#pragma unroll
-      for (int h = 0; h < 2; h++) {
-        const int i = lane + 32 * h;
-        if (j < ns && i > j && i < ns) sA[i * LDS + j] = v[c][h];
-      }
-    }
-  }
-  __syncthreads();
-  if ((int)threadIdx.x < ns) {
-    const int j = threadIdx.x;
-    double* X = sA + j * LDS;          // X[i] = (L11^-1)[i][j] for i > j
-    for (int i = j + 1; i < ns; i++) {
-      const double* Li = sA + i * LDS;
-      double a0 = Li[j], a1 = 0.0;     // k = j term: L[i][j] * X[j][j], X[j][j] = 1
-      int k = j + 1;
-      for (; k + 1 < i; k += 2) { a0 += Li[k] * X[k]; a1 += Li[k + 1] * X[k + 1]; }
-      if (k < i) a0 += Li[k] * X[k];
-      X[i] = -(a0 + a1);
-    }
-  }
-  __syncthreads();
-  for (int j = w; j < ns; j += 2)
-    for (int i = j + 1 + lane; i < ns; i += 32) P[(long long)j * ld + i] = sA[j * LDS + i];
 }
 
 // ---- the dataflow sweep ----

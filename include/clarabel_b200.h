@@ -113,6 +113,12 @@ void cldl_info(const cldl_t *h, cldl_info_t *info);
  * it to the CPU oracle so both sides eliminate in the same order. */
 int cldl_get_perm(const cldl_t *h, uint64_t *perm_out);
 
+/* The stored factor after the last refactor, for inspection and tests: the front panels as the solves read them
+ * (info.nnzL_stored doubles, front after front in supernode order; pivot blocks wider than 8 columns hold L11^-1 in
+ * their strictly lower triangle), the pivots D and their reciprocals (n doubles each, permuted order).  On a sharded
+ * handle the fronts of other ranks are not this handle's and hold no values.  Synchronises the handle's stream. */
+int cldl_get_factor(const cldl_t *h, double *L_out, double *D_out, double *Dinv_out);
+
 /* ---- device-pointer twins (asynchronous on the handle's stream) ---- */
 int cldl_update_values_dev(cldl_t *h, const int32_t *d_index, const double *d_values, uint64_t len);
 int cldl_set_values_dev(cldl_t *h, const double *d_nzval);   /* whole array, caller order */

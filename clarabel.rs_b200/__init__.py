@@ -142,6 +142,7 @@ EXPORTED_SYMBOLS = [
     "cldl_info", "cldl_get_perm", "cldl_update_values_dev", "cldl_set_values_dev",
     "cldl_refactor_dev", "cldl_solve_dev", "cldl_sync_status", "cldl_stream",
     "cldl_values_dev", "cldl_time_refactor_ms", "cldl_time_solve_ms",
+    "cldl_selected_inverse", "cldl_selected_inverse_dev",
 ]
 
 
@@ -279,6 +280,7 @@ class CudaLDLSolver:
                            _p(pm, C.c_uint64) if pm is not None else None)
         _check(rc, "cldl_create")
         self._h = h
+        self._pattern = (cp, rv)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -337,6 +339,26 @@ class CudaLDLSolver:
         p = np.empty(self.n, dtype=np.uint64)
         _check(self._L.cldl_get_perm(self._h, _p(p, C.c_uint64)), "get_perm")
         return p.astype(np.int64)
+
+    def selected_inverse(self):
+        """Selected inversion: the entries of (K + E)^-1 at the stored entries of the upper-triangular matrix passed
+        to the constructor, diagonal included, as a ``scipy.sparse.csc_matrix`` with that pattern.  K + E is the
+        matrix the last ``refactor()`` factored, E its dynamic regularisation (``regularize_count`` pivots).
+
+        Valid after a ``refactor()`` that returned True; raises BackendError (NotFactored) otherwise and
+        (BadArgument) on a sharded handle.  Computed on the GPU in one pass over the factor, about the work of a
+        refactor.  The first call allocates device memory that stays until ``close()``: one more array of
+        ``nnzL_stored`` doubles (the inverse in the factor's panel layout), the gather maps (about 12 bytes per row
+        index of the factor plus the segment positions) and nnzA doubles and int64s for the caller-order map and
+        result.  The factor and later solves are unchanged."""
+        import scipy.sparse as sps
+        f = self._L.cldl_selected_inverse
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        cp, rv = self._pattern
+        out = np.empty(rv.size, np.float64)
+        _check(f(self._h, _p(out, C.c_double)), "selected_inverse")
+        return sps.csc_matrix((out, rv.astype(np.int64), cp.astype(np.int64)), shape=(self.n, self.n))
 
     # --- device-side helpers (bench) ---
     def time_refactor_ms(self, reps):

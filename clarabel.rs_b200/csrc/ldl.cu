@@ -1068,6 +1068,8 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
   }
 }
 
+#include "ldl_selinv.cuh"
+
 __global__ void k_update_values(double* __restrict__ vals, const int* __restrict__ idx,
                                 const double* __restrict__ v, long long len) {
   long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1323,6 +1325,7 @@ void LDLObject::release() {
   fr(dev.asm_dst); fr(dev.level_tasks); fr(dev.perm); fr(dev.dsigns); fr(dev.vals); fr(dev.L);
   fr(dev.U); fr(dev.D); fr(dev.Dinv); fr(dev.u); fr(dev.status); fr(d_xp); fr(d_bx);
   fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.recs); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
+  fr(si.tasks); fr(si.col); fr(si.seg); fr(si.segpos); fr(si.Z); fr(d_si_pos); fr(d_si_init); fr(d_si_cnt); fr(d_si_out);
   if (h_status) cudaFreeHost(h_status);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
@@ -1352,12 +1355,52 @@ int LDLObject::refactor_level0() {
 int LDLObject::refactor_async() {
   if (sharded()) return has_transport() ? refactor_sharded() : CLDL_E_ARG;   // without a transport: the phase entry points
   CK(cudaSetDevice(device));
+  factor_ok = false;
   if (int rc = refactor_level0()) return rc;
   g_launches++;
   k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, dff);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h_status, dev.status, ST_COUNT * sizeof(int), cudaMemcpyDeviceToHost, stream));
   factored = true;
+  return CLDL_OK;
+}
+
+// the selected-inversion plan (ldl_plan.cpp) uploaded, Z panels and counters allocated: on the first call
+int LDLObject::selinv_setup() {
+  const SelinvPlan p = build_selinv_plan(S);
+  si.ntask = (int)p.tasks.size();
+  CK(upload(&si.tasks, p.tasks));
+  CK(upload(&si.col, p.col));
+  CK(upload(&si.seg, p.seg));
+  CK(upload(&si.segpos, p.segpos));
+  CK(upload(&d_si_pos, p.caller_pos));
+  CK(upload(&d_si_init, p.rows_left));
+  CK(cudaMalloc((void**)&d_si_cnt, (2 * (size_t)S.nsup + 1) * sizeof(int)));
+  si.rows_left = d_si_cnt; si.done = d_si_cnt + S.nsup; si.qhead = d_si_cnt + 2 * (size_t)S.nsup;
+  CK(cudaMalloc((void**)&si.Z, ((size_t)(S.L_alloc ? S.L_alloc : 1)) * sizeof(double)));
+  CK(cudaFuncSetAttribute(k_selinv, cudaFuncAttributeMaxDynamicSharedMemorySize, SI_SMEM_DOUBLES * 8));
+  int occ = 0, nsm = 0;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_selinv, SI_NT, (size_t)SI_SMEM_DOUBLES * 8));
+  CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+  if (occ < 1) return CLDL_E_CUDA;
+  si_grid = nsm * occ;    // every CTA resident: a task only waits for tasks queued before it
+  CK(cudaDeviceSynchronize());      // pageable uploads have landed before `stream` reads them
+  return CLDL_OK;
+}
+
+int LDLObject::selected_inverse_async(double* d_out) {
+  if (sharded()) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  CK(cudaSetDevice(device));
+  if (!si.Z) {
+    if (int rc = selinv_setup()) return rc;
+  }
+  CK(cudaMemcpyAsync(si.rows_left, d_si_init, (size_t)S.nsup * sizeof(int), cudaMemcpyDeviceToDevice, stream));
+  CK(cudaMemsetAsync(si.done, 0, ((size_t)S.nsup + 1) * sizeof(int), stream));
+  g_launches += 2;
+  if (si.ntask) k_selinv<<<si_grid, SI_NT, (size_t)SI_SMEM_DOUBLES * 8, stream>>>(dev, si);
+  if (nnzA) k_selinv_gather<<<(unsigned)((nnzA + 255) / 256), 256, 0, stream>>>(d_si_pos, si.Z, d_out, (long long)nnzA);
+  CK(cudaGetLastError());
   return CLDL_OK;
 }
 
@@ -1378,6 +1421,7 @@ int LDLObject::sync_status() {
     }
   }
   if (h_status[ST_ZEROPIV] && !dev.reg_enable) return CLDL_E_ZERO_PIVOT;
+  factor_ok = factored && !h_status[ST_NONFINITE];
   return h_status[ST_NONFINITE] ? 0 : 1;
 }
 
@@ -1867,6 +1911,26 @@ int cldl_get_factor(const cldl_t* h, double* L_out, double* D_out, double* Dinv_
     pos += (ns + nr) * ns;
   }
   return CLDL_OK;
+}
+
+int cldl_selected_inverse(cldl_t* h, double* nzval_out) {
+  if (!h || !nzval_out) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (!o.sharded() && o.factor_ok && !o.d_si_out) {
+    if (cudaSetDevice(o.device) != cudaSuccess ||
+        cudaMalloc((void**)&o.d_si_out, (size_t)(o.nnzA ? o.nnzA : 1) * sizeof(double)) != cudaSuccess)
+      return CLDL_E_CUDA;
+  }
+  int rc = o.selected_inverse_async(o.d_si_out);
+  if (rc) return rc;
+  if (cudaMemcpyAsync(nzval_out, o.d_si_out, (size_t)o.nnzA * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
+}
+int cldl_selected_inverse_dev(cldl_t* h, double* d_nzval_out) {
+  if (!h || !d_nzval_out) return CLDL_E_ARG;
+  return h->obj.selected_inverse_async(d_nzval_out);
 }
 
 int cldl_update_values_dev(cldl_t* h, const int32_t* d_index, const double* d_values, uint64_t len) {

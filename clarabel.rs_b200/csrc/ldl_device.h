@@ -70,6 +70,19 @@ struct DFFactor {
   unsigned long long* trace = nullptr;  // optional [ntask][4]: grab, ready, end (globaltimer ns), smid
 };
 
+// selected-inversion plan on the device (see k_selinv in ldl_selinv.cuh, SelinvPlan in ldl_plan.h)
+struct SIPlan {
+  int ntask = 0;
+  const int4* tasks = nullptr;      // 3 x int4 per task: SITask
+  const long long* col = nullptr;   // indexed like sn_rows
+  const long long* seg = nullptr;
+  const int* segpos = nullptr;
+  int* rows_left = nullptr;         // [nsup] row tasks still running
+  int* done = nullptr;              // [nsup] 1 when the front's Z panel is complete
+  int* qhead = nullptr;
+  double* Z = nullptr;              // panels of (K + E)^-1, laid out like the factor's
+};
+
 
 class LDLObject {
  public:
@@ -113,7 +126,16 @@ class LDLObject {
   size_t tmp_cap = 0;
   std::vector<int> h_idx;
   bool factored = false;
+  bool factor_ok = false;                // the last refactor's status was collected and it returned 1
   uint64_t regularize_count = 0, positive_inertia = 0;
+  // selected inversion: plan, Z panels and counters, allocated by the first call
+  SIPlan si;
+  long long* d_si_pos = nullptr;         // [nnzA] caller entry -> offset in si.Z
+  int *d_si_init = nullptr, *d_si_cnt = nullptr;
+  double* d_si_out = nullptr;            // [nnzA] staging of the host-pointer call
+  int si_grid = 0;
+  int selinv_setup();
+  int selected_inverse_async(double* d_out);
   // ---- one factorisation on several GPUs: this object is one rank (see ShardPlan in symbolic.h) ----
   int shard_nranks = 1, shard_rank = 0;
   ShardPlan shard;                       // owner[front] = rank or -1 (replicated top)

@@ -475,4 +475,89 @@ SolvePlan build_solve_plan(const Symbolic& S, const std::vector<int>& owner, int
   return P;
 }
 
+// Selected inversion (k_selinv): the queue runs the levels from the root down, as the backward sweep does.  The
+// gather maps follow every front's rows up the tree: `cur` holds their positions in the current ancestor's front; the
+// rows that are pivots of that ancestor form the next segment (rows are ascending, so segments are contiguous and
+// come in path order), the others move on to its parent through its `rel`.  Host threads take ranges of fronts.
+SelinvPlan build_selinv_plan(const Symbolic& S) {
+  SelinvPlan P;
+  const int nsup = S.nsup;
+  const size_t nrows = S.sn_rows.size();
+  P.col.assign(nrows, 0);
+  P.seg.assign(nrows, 0);
+  {
+    const unsigned nth = nsup < 20000 ? 1u : std::max(1u, std::min(16u, host_threads()));
+    std::vector<std::vector<int>> part(nth);
+    std::vector<std::thread> th;
+    auto walk = [&](unsigned t, int s0, int s1) {
+      std::vector<int>& sp = part[t];
+      std::vector<int> cur;
+      for (int s = s0; s < s1; s++) {
+        const int nr = nr_of(S, s);
+        const int64_t rp = S.sn_rowptr[s];
+        if (nr == 0) continue;
+        cur.assign(S.rel.begin() + rp, S.rel.begin() + rp + nr);
+        int a = S.sn_parent[s], i0 = 0;
+        while (i0 < nr) {
+          const int nsa = ns_of(S, a);
+          int k1 = i0;
+          while (k1 < nr && cur[k1] < nsa) k1++;
+          if (k1 > i0) {
+            const long long base = (long long)sp.size();
+            sp.insert(sp.end(), cur.begin() + i0, cur.end());
+            for (int k = i0; k < k1; k++) {
+              P.col[rp + k] = (long long)S.panel_off[a] + (long long)cur[k] * (nsa + nr_of(S, a));
+              P.seg[rp + k] = base - i0;     // local to this thread's part until the parts are joined
+            }
+          }
+          if (k1 < nr) {
+            const int64_t pa = S.sn_rowptr[a];
+            for (int i = k1; i < nr; i++) cur[i] = S.rel[pa + cur[i] - nsa];
+            a = S.sn_parent[a];
+          }
+          i0 = k1;
+        }
+      }
+    };
+    for (unsigned t = 0; t < nth; t++)
+      th.emplace_back(walk, t, (int)((int64_t)nsup * t / nth), (int)((int64_t)nsup * (t + 1) / nth));
+    for (auto& x : th) x.join();
+    size_t tot = 0;
+    for (auto& v : part) tot += v.size();
+    P.segpos.reserve(tot ? tot : 1);
+    for (unsigned t = 0; t < nth; t++) {
+      const long long off = (long long)P.segpos.size();
+      const int s0 = (int)((int64_t)nsup * t / nth), s1 = (int)((int64_t)nsup * (t + 1) / nth);
+      for (int64_t r = S.sn_rowptr[s0]; r < S.sn_rowptr[s1]; r++) P.seg[r] += off;
+      P.segpos.insert(P.segpos.end(), part[t].begin(), part[t].end());
+    }
+    if (P.segpos.empty()) P.segpos.push_back(0);
+  }
+  P.caller_pos.assign((size_t)S.nnzA, -1);
+  for (int s = 0; s < nsup; s++)
+    for (int64_t e = S.asm_ptr[s]; e < S.asm_ptr[s + 1]; e++)
+      P.caller_pos[S.asm_src[e]] = (long long)S.panel_off[s] + (long long)S.asm_dst[e];
+
+  const QueueOrder q = queue_order(S, {}, 0);
+  P.rows_left.assign(nsup, 0);
+  auto push = [&](int kind, int s, int r0, int r1) {
+    SITask t{};
+    t.kind = kind; t.s = s; t.r0 = r0; t.r1 = r1;
+    t.ns = ns_of(S, s); t.nr = nr_of(S, s); t.f = S.sn_first[s]; t.parent = S.sn_parent[s];
+    t.poff = S.panel_off[s]; t.rp = S.sn_rowptr[s];
+    P.tasks.push_back(t);
+  };
+  for (int l = S.nlevels - 1; l >= 0; l--) {
+    const std::vector<int>& lev = q[0][l];
+    for (int s : lev) {
+      const int nr = nr_of(S, s);
+      if (nr <= SI_RB) { push(0, s, 0, nr); continue; }
+      for (int r0 = 0; r0 < nr; r0 += SI_RB) push(1, s, r0, std::min(nr, r0 + SI_RB));
+      P.rows_left[s] = (nr + SI_RB - 1) / SI_RB;
+    }
+    for (int s : lev) if (nr_of(S, s) > SI_RB) push(2, s, 0, 0);
+  }
+  return P;
+}
+
 }  // namespace cb

@@ -23,6 +23,7 @@
 #define DF_RB 128           /* rows per R task */
 #define SV_NT 256
 #define SV_MAXROWS 256      /* rows of L21 in one slab (bounds the staged x / the per-thread row count) */
+#define SI_RB 64            /* selected inversion: rows of Z_RS per task (fronts with more rows get row tasks) */
 
 namespace cb {
 
@@ -115,5 +116,30 @@ struct SolvePlan {
 };
 // cap: doubles of the shared-memory slab of a sweep CTA
 SolvePlan build_solve_plan(const Symbolic& S, const std::vector<int>& owner, int rank, int cap);
+
+// One task of k_selinv (48 bytes = 3 x int4), queued root to leaves.  kind 0: a whole front with at most SI_RB rows
+// (its rows, then its pivot block); 1: rows [r0, r1) of Z_RS of a front with more rows; 2: the pivot block Z_SS of
+// such a front, after all of its row tasks.  Kinds 0 and 1 wait for the parent front's Z, kind 2 for its row tasks.
+struct SITask {
+  int kind, s, r0, r1;
+  int ns, nr, f, parent;    // pivots, rows below the pivot block, first column, parent front (-1: root)
+  long long poff, rp;       // panel_off[s], sn_rowptr[s]
+};
+static_assert(sizeof(SITask) == 48, "SITask is 3 x int4");
+static_assert(offsetof(SITask, ns) == 16 && offsetof(SITask, poff) == 32 && offsetof(SITask, rp) == 40, "SITask layout");
+
+// Selected inversion: Z = (K + E)^-1 in the layout of the factor's panels.  For the rows R of front s, entry
+// (R[i], R[k]) with i >= k lies in the panel of the front a that owns column R[k], at
+//     Z[col[rp + k] + segpos[seg[rp + k] + i]]
+// col: offset of column R[k] in a's panel; segpos: positions (0 .. ns_a + nr_a) in a's front of the rows R[k0 ..] of
+// the segment of R that a owns (rows k0 .. k1), the composition of `rel` along the path from s to a.
+struct SelinvPlan {
+  std::vector<SITask> tasks;
+  std::vector<int> rows_left;            // [nsup] row tasks of a front (0 for kind 0 fronts)
+  std::vector<long long> col, seg;       // indexed like sn_rows
+  std::vector<int> segpos;
+  std::vector<long long> caller_pos;     // [nnzA] offset in Z of the caller's entry p (triu, caller's CSC order)
+};
+SelinvPlan build_selinv_plan(const Symbolic& S);
 
 }  // namespace cb

@@ -119,6 +119,22 @@ int cldl_get_perm(const cldl_t *h, uint64_t *perm_out);
  * handle the fronts of other ranks are not this handle's and hold no values.  Synchronises the handle's stream. */
 int cldl_get_factor(const cldl_t *h, double *L_out, double *D_out, double *Dinv_out);
 
+/* Selected inversion: the entries of (K + E)^-1 at every stored entry of the upper triangle passed to cldl_create,
+ * diagonal included, in the caller's CSC order (nnzA doubles).  K + E is the matrix the last refactor factored: E is
+ * the dynamic regularisation it applied (cldl_info.regularize_count pivots), so with regularisation the result is the
+ * inverse of the regularised matrix, not of K.  Computed on the device in one pass over the factor from the root of
+ * the assembly tree to its leaves (about the work of one refactor).
+ *   - Valid after a refactor that returned 1 (cldl_refactor, or cldl_refactor_dev followed by cldl_sync_status).
+ *     Before any refactor, or after one that returned 0 or an error, the call returns CLDL_E_NOT_FACTORED.
+ *   - On a sharded handle the call returns CLDL_E_ARG.
+ *   - The first call builds the plan and allocates its device memory: panels of the inverse (info.nnzL_stored
+ *     doubles, plus alignment), the gather maps and the task queue.  cldl_destroy frees them.
+ *   - The factor, D, 1/D and every later solve are left bit for bit unchanged.
+ * cldl_selected_inverse writes a host buffer and synchronises; the _dev form writes a device buffer and is only
+ * enqueued on the handle's stream (cldl_stream). */
+int cldl_selected_inverse(cldl_t *h, double *nzval_out);
+int cldl_selected_inverse_dev(cldl_t *h, double *d_nzval_out);
+
 /* ---- device-pointer twins (asynchronous on the handle's stream) ---- */
 int cldl_update_values_dev(cldl_t *h, const int32_t *d_index, const double *d_values, uint64_t len);
 int cldl_set_values_dev(cldl_t *h, const double *d_nzval);   /* whole array, caller order */

@@ -143,6 +143,8 @@ EXPORTED_SYMBOLS = [
     "cldl_refactor_dev", "cldl_solve_dev", "cldl_sync_status", "cldl_stream",
     "cldl_values_dev", "cldl_time_refactor_ms", "cldl_time_solve_ms",
     "cldl_selected_inverse", "cldl_selected_inverse_dev",
+    "cldl_create_schur", "cldl_schur_complement", "cldl_schur_complement_dev", "cldl_schur_reduce",
+    "cldl_schur_reduce_dev", "cldl_schur_expand", "cldl_schur_expand_dev",
 ]
 
 
@@ -260,7 +262,10 @@ class CudaLDLSolver:
     def __init__(self, n, colptr, rowval, nzval, dsigns, *, perm=None,
                  regularize_eps=1e-13, regularize_delta=2e-7, regularize_enable=True,
                  amd_dense_scale=1.5, ordering=ORDER_BEST, device=0, max_panel=0, nd_leaf=0,
-                 shard_nranks=0, shard_rank=0):
+                 shard_nranks=0, shard_rank=0, schur=None):
+        """``schur``: a Schur set (caller indices, in the order the complement's rows and columns take) makes a Schur
+        complement handle: ``refactor()`` factors the other indices only, and ``schur_complement()``,
+        ``schur_reduce()`` and ``schur_expand()`` replace ``solve()`` (see cldl_create_schur)."""
         L = lib()
         self._L = L
         self.n = int(n)
@@ -275,10 +280,26 @@ class CudaLDLSolver:
         ds = np.ascontiguousarray(dsigns, dtype=np.int8)
         pm = _u64(perm) if perm is not None else None
         h = C.c_void_p()
-        rc = L.cldl_create(C.byref(h), self.n, _p(cp, C.c_uint64), _p(rv, C.c_uint64),
-                           _p(nz, C.c_double), _p(ds, C.c_int8), C.byref(o),
-                           _p(pm, C.c_uint64) if pm is not None else None)
-        _check(rc, "cldl_create")
+        self.nschur = 0
+        if schur is None:
+            rc = L.cldl_create(C.byref(h), self.n, _p(cp, C.c_uint64), _p(rv, C.c_uint64),
+                               _p(nz, C.c_double), _p(ds, C.c_int8), C.byref(o),
+                               _p(pm, C.c_uint64) if pm is not None else None)
+            _check(rc, "cldl_create")
+        else:
+            si = np.asarray(schur, dtype=np.int64).ravel()
+            if si.size == 0 or (si < 0).any():
+                raise BackendError("cldl_create_schur failed: BadArgument")
+            si = _u64(si)
+            f = L.cldl_create_schur
+            f.argtypes = [C.POINTER(C.c_void_p), C.c_uint64] + [C.POINTER(C.c_uint64)] * 2 + \
+                [C.POINTER(C.c_double), C.POINTER(C.c_int8), C.POINTER(cldl_opts), C.POINTER(C.c_uint64), C.c_uint64,
+                 C.POINTER(C.c_uint64)]
+            f.restype = C.c_int
+            rc = f(C.byref(h), self.n, _p(cp, C.c_uint64), _p(rv, C.c_uint64), _p(nz, C.c_double), _p(ds, C.c_int8),
+                   C.byref(o), _p(pm, C.c_uint64) if pm is not None else None, si.size, _p(si, C.c_uint64))
+            _check(rc, "cldl_create_schur")
+            self.nschur = int(si.size)
         self._h = h
         self._pattern = (cp, rv)
 
@@ -359,6 +380,42 @@ class CudaLDLSolver:
         out = np.empty(rv.size, np.float64)
         _check(f(self._h, _p(out, C.c_double)), "selected_inverse")
         return sps.csc_matrix((out, rv.astype(np.int64), cp.astype(np.int64)), shape=(self.n, self.n))
+
+    # --- Schur complement handles (constructed with schur=...) ---
+    def _schur_call(self, name, *args):
+        f = getattr(self._L, name)
+        f.argtypes = [C.c_void_p] + [C.POINTER(C.c_double)] * len(args)
+        f.restype = C.c_int
+        _check(f(self._h, *(_p(a, C.c_double) for a in args)), name[5:])
+
+    def schur_complement(self):
+        """The dense Schur complement K_SS - K_SB K_BB^-1 K_BS assembled by the last ``refactor()`` (which must have
+        returned True), as a (k, k) array in the order of the Schur set.  With regularisation it is the complement of
+        K + E_B, E_B the dynamic regularisation of B's pivots.  BackendError (NotFactored) before such a refactor,
+        (BadArgument) on a handle without a Schur set."""
+        k = self.nschur
+        out = np.empty(k * k, np.float64)
+        self._schur_call("cldl_schur_complement", out)
+        return out.reshape((k, k), order="F")
+
+    def schur_reduce(self, b):
+        """Condensation: w_S = b_S - K_SB K_BB^-1 b_B (b: n values in the caller's order; w_S in the Schur set's
+        order)."""
+        b = _f64(b)
+        assert b.size == self.n
+        w = np.empty(self.nschur, np.float64)
+        self._schur_call("cldl_schur_reduce", w, b)
+        return w
+
+    def schur_expand(self, xS):
+        """Expansion: the whole solution x (n values) from x_S solving Sc x_S = w_S, for the b of the last
+        ``schur_reduce``.  Each expansion consumes its condensation: BackendError (BadArgument) without one since the
+        last refactor or expansion."""
+        xS = _f64(xS)
+        assert xS.size == self.nschur
+        x = np.empty(self.n, np.float64)
+        self._schur_call("cldl_schur_expand", x, xS)
+        return x
 
     # --- device-side helpers (bench) ---
     def time_refactor_ms(self, reps):

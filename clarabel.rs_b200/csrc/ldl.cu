@@ -1069,6 +1069,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
 }
 
 #include "ldl_selinv.cuh"
+#include "ldl_schur.cuh"
 
 __global__ void k_update_values(double* __restrict__ vals, const int* __restrict__ idx,
                                 const double* __restrict__ v, long long len) {
@@ -1121,7 +1122,8 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   if (o.max_panel > 0) so.max_panel = o.max_panel > CB_PB_MAXNS ? CB_PB_MAXNS : o.max_panel;
   if (o.nd_leaf > 0) so.nd_leaf = o.nd_leaf;
   cb_tmark(nullptr);
-  int rc = analyse(n, Ap, Ai, perm_in, so, S);
+  schur = !schur_set.empty();
+  int rc = schur ? analyse_schur(n, Ap, Ai, perm_in, schur_set, so, S) : analyse(n, Ap, Ai, perm_in, so, S);
   cb_tmark("ldl: ordering + symbolic");
   if (rc == -2) return CLDL_E_EMPTY_COLUMN;
   if (rc == -3) return CLDL_E_NOT_TRIU;
@@ -1129,6 +1131,8 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   if (rc) return CLDL_E_ARG;
   shard_nranks = o.shard_nranks > 1 ? o.shard_nranks : 1;
   shard_rank = o.shard_rank;
+  if (schur && sharded()) return CLDL_E_ARG;
+  if (schur) shard_rank = 0;
   if (sharded()) {
     if (shard_rank < 0 || shard_rank >= shard_nranks) return CLDL_E_ARG;
     std::vector<int> par(S.sn_parent);
@@ -1142,6 +1146,8 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
       for (int j = S.sn_first[s]; j < S.sn_first[s + 1]; j++) shard_xidx[g].push_back(S.perm[j]);
     }
   }
+  // the plans' view of the fronts: a Schur handle is rank 0 of a split whose top part is S (never factored)
+  const std::vector<int> owner = schur ? schur_owner(S, n - (int)schur_set.size()) : shard.owner;
 
   CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
   CK(cudaStreamCreateWithFlags(&stream_a, cudaStreamNonBlocking));
@@ -1212,10 +1218,10 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     sv_cap = std::min(sv_cap, 16384);
   }
   SolvePlan sp;
-  std::thread th_solve([&]() { sp = build_solve_plan(S, shard.owner, shard_rank, sv_cap); });
+  std::thread th_solve([&]() { sp = build_solve_plan(S, owner, shard_rank, sv_cap); });
   struct ThJoin { std::thread& t; ~ThJoin() { if (t.joinable()) t.join(); } } th_solve_guard{th_solve};
-  Level0Plan l0 = build_level0_plan(S, shard.owner, shard_rank, level_cap);
-  FactorPlan fp = build_factor_plan(S, shard.owner, shard_rank);
+  Level0Plan l0 = build_level0_plan(S, owner, shard_rank, level_cap);
+  FactorPlan fp = build_factor_plan(S, owner, shard_rank);
   th_solve.join();
   cb_tmark("ldl: plans");
 
@@ -1302,6 +1308,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     for (int w = 0; w < 2; w++) { d_shard_segs[w].assign(shard_nranks, nullptr); shard_nsegs[w].assign(shard_nranks, 0); }
     for (int g = 0; g < shard_nranks; g++) CK(upload(&d_shard_xidx[g], shard_xidx[g]));
   }
+  if (schur && (rc = schur_setup(sp))) return rc;
   if (big_alloc.joinable()) big_alloc.join();
   if (big_alloc_rc) { std::fprintf(stderr, "[clarabel_b200] device allocation of the factor storage failed\n"); return CLDL_E_CUDA; }
   cb_tmark("ldl: big allocations joined");
@@ -1326,6 +1333,8 @@ void LDLObject::release() {
   fr(dev.U); fr(dev.D); fr(dev.Dinv); fr(dev.u); fr(dev.status); fr(d_xp); fr(d_bx);
   fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.recs); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
   fr(si.tasks); fr(si.col); fr(si.seg); fr(si.segpos); fr(si.Z); fr(d_si_pos); fr(d_si_init); fr(d_si_cnt); fr(d_si_out);
+  fr(sv_bwd.tasks); fr(sv_bwd.parent); fr(d_sc_spos); fr(d_sc_kss_src); fr(d_sc_rec_ptr); fr(d_sc_kss_ptr); fr(d_sc_kss_dst);
+  fr(d_sc_recs); fr(d_sc_out); fr(d_sc_vec);
   if (h_status) cudaFreeHost(h_status);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
@@ -1356,9 +1365,20 @@ int LDLObject::refactor_async() {
   if (sharded()) return has_transport() ? refactor_sharded() : CLDL_E_ARG;   // without a transport: the phase entry points
   CK(cudaSetDevice(device));
   factor_ok = false;
+  schur_fwd = false;
   if (int rc = refactor_level0()) return rc;
   g_launches++;
-  k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, dff);
+  if (schur) {    // B's tasks only (they come first in the queue), then the complement from the cut roots
+    DFFactor q = dff;
+    q.ntask = dff_ntask_owned;
+    k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, q);
+    g_launches++;
+    k_schur_assemble<<<schur_k, SC_NT, 0, stream>>>(dev.vals, dev.U, dev.sn_rows, schur_first, schur_k, d_sc_spos,
+                                                     d_sc_kss_ptr, d_sc_kss_dst, d_sc_kss_src, d_sc_rec_ptr, d_sc_recs,
+                                                     d_sc_out);
+  } else {
+    k_factor_df<<<dff_grid, DF_NT, (size_t)DF_SMEM_DOUBLES * 8, stream>>>(dev, dff);
+  }
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(h_status, dev.status, ST_COUNT * sizeof(int), cudaMemcpyDeviceToHost, stream));
   factored = true;
@@ -1389,7 +1409,7 @@ int LDLObject::selinv_setup() {
 }
 
 int LDLObject::selected_inverse_async(double* d_out) {
-  if (sharded()) return CLDL_E_ARG;
+  if (sharded() || schur) return CLDL_E_ARG;
   if (!factor_ok) return CLDL_E_NOT_FACTORED;
   CK(cudaSetDevice(device));
   if (!si.Z) {
@@ -1401,6 +1421,75 @@ int LDLObject::selected_inverse_async(double* d_out) {
   if (si.ntask) k_selinv<<<si_grid, SI_NT, (size_t)SI_SMEM_DOUBLES * 8, stream>>>(dev, si);
   if (nnzA) k_selinv_gather<<<(unsigned)((nnzA + 255) / 256), 256, 0, stream>>>(d_si_pos, si.Z, d_out, (long long)nnzA);
   CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+// the Schur plan (ldl_plan.cpp) uploaded and the complement allocated, at the end of init
+int LDLObject::schur_setup(const SolvePlan& sp) {
+  const SchurPlan p = build_schur_plan(S, schur_set, sp);
+  schur_k = p.k;
+  schur_first = p.first;
+  for (int c : p.cut)     // their update matrices and vectors must hold S rows only
+    if (S.sn_rowptr[c + 1] > S.sn_rowptr[c] && S.sn_rows[S.sn_rowptr[c]] < schur_first) return CLDL_E_ARG;
+  const size_t kk = (size_t)schur_k * (size_t)schur_k;
+  if (cudaMalloc((void**)&d_sc_out, kk * sizeof(double)) != cudaSuccess) {
+    cudaGetLastError();
+    d_sc_out = nullptr;
+    std::fprintf(stderr, "[clarabel_b200] a Schur set of %d needs %zu bytes for the complement\n", schur_k, kk * sizeof(double));
+    return CLDL_E_ARG;
+  }
+  CK(cudaMalloc((void**)&d_sc_vec, 2 * (size_t)schur_k * sizeof(double)));
+  CK(upload(&d_sc_spos, p.spos));
+  CK(upload(&d_sc_kss_ptr, p.kss_ptr));
+  CK(upload(&d_sc_kss_dst, p.kss_dst));
+  CK(upload(&d_sc_kss_src, p.kss_src));
+  CK(upload(&d_sc_rec_ptr, p.rec_ptr));
+  CK(upload(&d_sc_recs, p.recs));
+  sv_bwd = sv;
+  sv_bwd.ntask = (int)p.bwd.size();
+  sv_bwd.tasks = nullptr;
+  sv_bwd.parent = nullptr;
+  sv_bwd.trace = nullptr;
+  CK(upload(&sv_bwd.tasks, p.bwd.empty() ? std::vector<SVTask>(1) : p.bwd));
+  CK(upload(&sv_bwd.parent, p.bparent));
+  return CLDL_OK;
+}
+
+// condensation: permute b, forward over B (leaf kernels and the owned phase of the sweep), then w_S
+int LDLObject::schur_reduce_async(double* d_wS, const double* d_b) {
+  if (!schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  CK(cudaSetDevice(device));
+  SVRhs r;
+  r.xp[0] = r.xp[1] = d_xp; r.u[0] = r.u[1] = dev.u; r.out[0] = r.out[1] = d_xp;
+  g_launches += 2;
+  k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, d_b, d_xp);
+  if (int rc = sv_reset()) return rc;
+  sv_leaves(true, 1, r);
+  SVPlan qv = sv;
+  qv.ntask = sv_ntask_owned;
+  sv_sweep(true, 1, qv, r);
+  k_schur_reduce<<<(schur_k + 255) / 256, 256, 0, stream>>>(schur_first, schur_k, d_sc_spos, d_sc_rec_ptr, d_sc_recs,
+                                                             d_xp, dev.u, d_wS);
+  CK(cudaGetLastError());
+  schur_fwd = true;
+  return CLDL_OK;
+}
+
+// expansion: x_S into the work vector (B's forward state from the last condensation), backward over B alone
+int LDLObject::schur_expand_async(double* d_x, const double* d_xS) {
+  if (!schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if (!schur_fwd) return CLDL_E_ARG;
+  CK(cudaSetDevice(device));
+  SVRhs r;
+  r.xp[0] = r.xp[1] = d_xp; r.u[0] = r.u[1] = dev.u; r.out[0] = r.out[1] = d_x;
+  g_launches++;
+  k_schur_expand_in<<<(schur_k + 255) / 256, 256, 0, stream>>>(schur_first, schur_k, d_sc_spos, dev.perm, d_xS, d_xp, d_x);
+  if (sv_bwd.ntask) sv_sweep(false, 1, sv_bwd, r);
+  sv_leaves(false, 1, r);
+  CK(cudaGetLastError());
+  schur_fwd = false;     // the backward sweep overwrote the forward state
   return CLDL_OK;
 }
 
@@ -1496,6 +1585,7 @@ int LDLObject::solve_async(double* d_x, const double* d_b, double* d_x1, const d
     if (rc || nrhs == 1) return rc;
     return solve_sharded(d_x1, d_b1);
   }
+  if (schur) return CLDL_E_ARG;   // S is never factored: schur_reduce_async / schur_expand_async
   if (!factored) return CLDL_E_NOT_FACTORED;
   CK(cudaSetDevice(device));
   SVRhs r;
@@ -1847,6 +1937,7 @@ int cldl_refactor(cldl_t* h) {
 int cldl_solve(cldl_t* h, double* x, const double* b) {
   if (!h || !x || !b) return CLDL_E_ARG;
   LDLObject& o = h->obj;
+  if (o.schur) return CLDL_E_ARG;
   if (!o.factored) return CLDL_E_NOT_FACTORED;
   if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
   size_t bytes = (size_t)o.n * sizeof(double);
@@ -1916,7 +2007,7 @@ int cldl_get_factor(const cldl_t* h, double* L_out, double* D_out, double* Dinv_
 int cldl_selected_inverse(cldl_t* h, double* nzval_out) {
   if (!h || !nzval_out) return CLDL_E_ARG;
   LDLObject& o = h->obj;
-  if (!o.sharded() && o.factor_ok && !o.d_si_out) {
+  if (!o.sharded() && !o.schur && o.factor_ok && !o.d_si_out) {
     if (cudaSetDevice(o.device) != cudaSuccess ||
         cudaMalloc((void**)&o.d_si_out, (size_t)(o.nnzA ? o.nnzA : 1) * sizeof(double)) != cudaSuccess)
       return CLDL_E_CUDA;
@@ -1931,6 +2022,112 @@ int cldl_selected_inverse(cldl_t* h, double* nzval_out) {
 int cldl_selected_inverse_dev(cldl_t* h, double* d_nzval_out) {
   if (!h || !d_nzval_out) return CLDL_E_ARG;
   return h->obj.selected_inverse_async(d_nzval_out);
+}
+
+int cldl_create_schur(cldl_t** out, uint64_t n, const uint64_t* colptr, const uint64_t* rowval,
+                      const double* nzval, const int8_t* dsigns, const cldl_opts* opts,
+                      const uint64_t* perm_or_null, uint64_t nschur, const uint64_t* schur_idx) {
+  if (!out) return CLDL_E_ARG;
+  *out = nullptr;
+  if (!colptr || !rowval || !nzval || n == 0 || n > 0x7fffffffu) return CLDL_E_DIM;
+  if (!schur_idx || nschur == 0 || nschur >= n) return CLDL_E_ARG;
+  if (opts && opts->shard_nranks > 1) return CLDL_E_ARG;
+  const uint64_t nnz = colptr[n];
+  if (nnz > 0x7fffffffu) return CLDL_E_DIM;
+  std::vector<int64_t> Ap(n + 1);
+  std::vector<int32_t> Ai(nnz);
+  for (uint64_t j = 0; j <= n; j++) Ap[j] = (int64_t)colptr[j];
+  for (uint64_t p = 0; p < nnz; p++) {
+    if (rowval[p] >= n) return CLDL_E_DIM;
+    Ai[p] = (int32_t)rowval[p];
+  }
+  std::vector<int> perm;
+  if (perm_or_null) {
+    perm.resize(n);
+    for (uint64_t k = 0; k < n; k++) {
+      if (perm_or_null[k] >= n) return CLDL_E_BAD_PERM;
+      perm[k] = (int)perm_or_null[k];
+    }
+  }
+  std::vector<int> sidx(nschur);
+  for (uint64_t i = 0; i < nschur; i++) {
+    if (schur_idx[i] >= n) return CLDL_E_ARG;
+    sidx[i] = (int)schur_idx[i];
+  }
+  cldl_opts o;
+  if (opts) o = *opts; else cldl_default_opts(&o);
+  cldl_handle* h = new (std::nothrow) cldl_handle();
+  if (!h) return CLDL_E_ARG;
+  h->obj.schur_set = std::move(sidx);
+  int rc = h->obj.init((int)n, Ap.data(), Ai.data(), nzval, dsigns, o, perm_or_null ? perm.data() : nullptr);
+  if (rc != CLDL_OK) {
+    h->obj.release();
+    delete h;
+    return rc;
+  }
+  *out = h;
+  return CLDL_OK;
+}
+
+int cldl_schur_complement_dev(cldl_t* h, double* d_out) {
+  if (!h || !d_out) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (!o.schur) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t bytes = (size_t)o.schur_k * (size_t)o.schur_k * sizeof(double);
+  return cudaMemcpyAsync(d_out, o.d_sc_out, bytes, cudaMemcpyDeviceToDevice, o.stream) == cudaSuccess ? CLDL_OK : CLDL_E_CUDA;
+}
+int cldl_schur_complement(cldl_t* h, double* out) {
+  if (!h || !out) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (!o.schur) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t bytes = (size_t)o.schur_k * (size_t)o.schur_k * sizeof(double);
+  if (cudaMemcpyAsync(out, o.d_sc_out, bytes, cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
+}
+int cldl_schur_reduce_dev(cldl_t* h, double* d_wS, const double* d_b) {
+  if (!h || !d_wS || !d_b) return CLDL_E_ARG;
+  return h->obj.schur_reduce_async(d_wS, d_b);
+}
+int cldl_schur_reduce(cldl_t* h, double* wS, const double* b) {
+  if (!h || !wS || !b) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (!o.schur) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t k = (size_t)o.schur_k;
+  if (cudaMemcpyAsync(o.d_bx, b, (size_t)o.n * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess) return CLDL_E_CUDA;
+  int rc = o.schur_reduce_async(o.d_sc_vec, o.d_bx);
+  if (rc) return rc;
+  if (cudaMemcpyAsync(wS, o.d_sc_vec, k * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
+}
+int cldl_schur_expand_dev(cldl_t* h, double* d_x, const double* d_xS) {
+  if (!h || !d_x || !d_xS) return CLDL_E_ARG;
+  return h->obj.schur_expand_async(d_x, d_xS);
+}
+int cldl_schur_expand(cldl_t* h, double* x, const double* xS) {
+  if (!h || !x || !xS) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (!o.schur) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  if (!o.schur_fwd) return CLDL_E_ARG;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t k = (size_t)o.schur_k;
+  if (cudaMemcpyAsync(o.d_sc_vec + k, xS, k * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess) return CLDL_E_CUDA;
+  int rc = o.schur_expand_async(o.d_bx + o.n, o.d_sc_vec + k);
+  if (rc) return rc;
+  if (cudaMemcpyAsync(x, o.d_bx + o.n, (size_t)o.n * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
 }
 
 int cldl_update_values_dev(cldl_t* h, const int32_t* d_index, const double* d_values, uint64_t len) {

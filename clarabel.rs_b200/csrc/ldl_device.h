@@ -136,6 +136,20 @@ class LDLObject {
   int si_grid = 0;
   int selinv_setup();
   int selected_inverse_async(double* d_out);
+  // Schur complement handle (cldl_create_schur; SchurPlan in ldl_plan.h): B's fronts are factored, S's never
+  std::vector<int> schur_set;            // non-empty: a Schur complement handle
+  bool schur = false;
+  bool schur_fwd = false;                // a condensation since the last expansion / refactor left the forward state
+  int schur_k = 0, schur_first = 0;
+  SVPlan sv_bwd;                         // the B-only backward queue (counters shared with sv)
+  int *d_sc_spos = nullptr, *d_sc_kss_src = nullptr, *d_sc_rec_ptr = nullptr;
+  long long *d_sc_kss_ptr = nullptr, *d_sc_kss_dst = nullptr;
+  SchurRec* d_sc_recs = nullptr;
+  double* d_sc_out = nullptr;            // [k * k] the complement of the last refactor
+  double* d_sc_vec = nullptr;            // [2 k] staging of the host-pointer partial solves
+  int schur_setup(const SolvePlan& sp);
+  int schur_reduce_async(double* d_wS, const double* d_b);
+  int schur_expand_async(double* d_x, const double* d_xS);
   // ---- one factorisation on several GPUs: this object is one rank (see ShardPlan in symbolic.h) ----
   int shard_nranks = 1, shard_rank = 0;
   ShardPlan shard;                       // owner[front] = rank or -1 (replicated top)
@@ -183,6 +197,7 @@ class LDLObject {
   int refactor_sharded();
   int solve_sharded(double* d_x, const double* d_b);
 
+  // a Schur complement handle sets schur_set (caller indices, in output order) before init
   int init(int n, const int64_t* Ap, const int32_t* Ai, const double* Ax, const int8_t* dsigns,
            const cldl_opts& o, const int* perm_in);
   void release();

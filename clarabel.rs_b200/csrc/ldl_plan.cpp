@@ -38,12 +38,15 @@ QueueOrder queue_order(const Symbolic& S, const std::vector<int>& owner, int ran
 
 // Tree level 0 (leaves: no dependencies) is factored by plain launches before k_factor_df.  Single-column fronts take
 // one thread each (k_factor_leaf1), the others one fused CTA each (k_factor_level), grouped by the shared-memory class
-// of their panel.  Big fronts (k_factor_df's tasks) and fronts this rank does not handle are parked at the end.
+// of their panel.  Big fronts (k_factor_df's tasks) and fronts outside the first phase are parked at the end (a
+// sharded top part has no leaves; a Schur handle's S fronts are never factored).
 Level0Plan build_level0_plan(const Symbolic& S, const std::vector<int>& owner, int rank, int smem_cap) {
   Level0Plan P;
   P.level_tasks = S.level_tasks;
   if (S.nlevels == 0) return P;
-  const std::vector<char> mine = queued(queue_order(S, owner, rank), S.nsup);
+  QueueOrder q = queue_order(S, owner, rank);
+  q.resize(1);
+  const std::vector<char> mine = queued(q, S.nsup);
   const long long classes[3] = {1024, 5632, smem_cap};  // 8 KB, 44 KB, ~225 KB panels
   const int b = S.level_ptr[0], e = S.level_ptr[1];
   std::vector<int> order[4], order1, big, not_mine;
@@ -383,8 +386,9 @@ SolvePlan build_solve_plan(const Symbolic& S, const std::vector<int>& owner, int
     std::vector<std::vector<int>> lev_small(S.nlevels), lev_big(S.nlevels);
     for (int l = 0; l < S.nlevels; l++)
       for (int s : queue[ph][l]) {
-        if (!wide(s) && !has_kids(s)) { (ns_of(S, s) == 1 ? P.leaf1 : P.leafn).push_back(s); continue; }
-        if (wide(s) && !has_kids(s) && nr_of(S, s) <= 1024) {
+        // leaves of the first phase only (a sharded top part has none; a Schur handle's S fronts are never solved)
+        if (ph == 0 && !wide(s) && !has_kids(s)) { (ns_of(S, s) == 1 ? P.leaf1 : P.leafn).push_back(s); continue; }
+        if (ph == 0 && wide(s) && !has_kids(s) && nr_of(S, s) <= 1024) {
           P.leafw.push_back(s);
           P.leafw_nrmax = std::max(P.leafw_nrmax, nr_of(S, s));
           continue;
@@ -557,6 +561,79 @@ SelinvPlan build_selinv_plan(const Symbolic& S) {
     }
     for (int s : lev) if (nr_of(S, s) > SI_RB) push(2, s, 0, 0);
   }
+  return P;
+}
+
+std::vector<int> schur_owner(const Symbolic& S, int first) {
+  std::vector<int> owner(S.nsup, 0);
+  for (int s = 0; s < S.nsup; s++) if (S.sn_first[s] >= first) owner[s] = -1;
+  return owner;
+}
+
+SchurPlan build_schur_plan(const Symbolic& S, const std::vector<int>& schur, const SolvePlan& sp) {
+  SchurPlan P;
+  const int nsup = S.nsup, n = S.n, k = (int)schur.size();
+  P.k = k;
+  P.first = n - k;
+  const int sf = P.first;
+  P.owner = schur_owner(S, sf);
+  for (int s = 0; s < nsup; s++)
+    if (P.owner[s] == 0 && S.sn_parent[s] >= 0 && P.owner[S.sn_parent[s]] < 0) P.cut.push_back(s);
+  std::vector<int> out_of(n, -1);        // caller index -> output index
+  for (int i = 0; i < k; i++) out_of[schur[i]] = i;
+  P.spos.resize(k);
+  for (int j = 0; j < k; j++) P.spos[j] = out_of[S.perm[sf + j]];
+
+  // K_SS: bucket by the lower permuted column, then sort each bucket by output position (stable: caller order
+  // among duplicates)
+  P.kss_ptr.assign(k + 1, 0);
+  struct E { long long dst; int src; int col; };
+  std::vector<E> ents;
+  {
+    // the K_SS entries are the original entries assembled into S fronts (the analysis keeps no copy of the caller's
+    // pattern; the assembly map gives each entry's front and panel position)
+    for (int s = 0; s < nsup; s++) {
+      if (P.owner[s] == 0) continue;
+      const int f = S.sn_first[s], ns = ns_of(S, s), nr = nr_of(S, s), ld = ns + nr;
+      for (int64_t e = S.asm_ptr[s]; e < S.asm_ptr[s + 1]; e++) {
+        const int64_t d = S.asm_dst[e];
+        const int lc = (int)(d / ld), lr = (int)(d % ld);
+        const int jc = f + lc - sf;
+        const int jr = (lr < ns ? f + lr : S.sn_rows[S.sn_rowptr[s] + lr - ns]) - sf;
+        ents.push_back(E{(long long)P.spos[jc] * k + P.spos[jr], S.asm_src[e], jc});
+      }
+    }
+    for (const E& x : ents) P.kss_ptr[x.col + 1]++;
+    for (int j = 0; j < k; j++) P.kss_ptr[j + 1] += P.kss_ptr[j];
+    std::vector<E> w(ents.size());
+    std::vector<long long> pos(P.kss_ptr.begin(), P.kss_ptr.end() - 1);
+    for (const E& x : ents) w[pos[x.col]++] = x;
+    for (int j = 0; j < k; j++)
+      std::stable_sort(w.begin() + P.kss_ptr[j], w.begin() + P.kss_ptr[j + 1], [](const E& a, const E& b) { return a.dst < b.dst; });
+    P.kss_dst.resize(w.size() ? w.size() : 1, 0);
+    P.kss_src.resize(w.size() ? w.size() : 1, 0);
+    for (size_t i = 0; i < w.size(); i++) { P.kss_dst[i] = w[i].dst; P.kss_src[i] = w[i].src; }
+  }
+
+  // cut roots per permuted S column, ascending
+  P.rec_ptr.assign(k + 1, 0);
+  for (int c : P.cut)
+    for (int64_t t = S.sn_rowptr[c]; t < S.sn_rowptr[c + 1]; t++) P.rec_ptr[S.sn_rows[t] - sf + 1]++;
+  for (int j = 0; j < k; j++) P.rec_ptr[j + 1] += P.rec_ptr[j];
+  P.recs.resize(P.rec_ptr[k] ? P.rec_ptr[k] : 1);
+  {
+    std::vector<int> pos(P.rec_ptr.begin(), P.rec_ptr.end() - 1);
+    for (int c : P.cut)
+      for (int64_t t = S.sn_rowptr[c]; t < S.sn_rowptr[c + 1]; t++)
+        P.recs[pos[S.sn_rows[t] - sf]++] = SchurRec{(long long)S.upd_off[c], (long long)S.sn_rowptr[c], nr_of(S, c),
+                                                     (int)(t - S.sn_rowptr[c])};
+  }
+
+  // B-only backward queue: the owned tasks, with the waits on S fronts dropped
+  P.bwd.assign(sp.tasks.begin(), sp.tasks.begin() + sp.ntask_owned);
+  for (SVTask& t : P.bwd) if (t.kind != 0 && t.bowner >= 0 && P.owner[t.bowner] < 0) t.bowner = -1;
+  P.bparent = S.sn_parent;
+  for (int c : P.cut) P.bparent[c] = -1;
   return P;
 }
 

@@ -142,4 +142,32 @@ struct SelinvPlan {
 };
 SelinvPlan build_selinv_plan(const Symbolic& S);
 
+// Schur complement handle (S.schur_first >= 0): the fronts of B are rank 0's owned subtrees and the fronts of S the
+// top part, which is never factored.  The output is the k x k complement, column-major, in the caller's order of the
+// Schur set; permuted S column j (column schur_first + j) is output column spos[j].
+struct SchurRec {           // cut root whose local row b is the permuted S column of the list it is in
+  long long uoff, rp;       // upd_off[c], sn_rowptr[c]
+  int nr, b;
+};
+static_assert(sizeof(SchurRec) == 24, "SchurRec is 6 ints");
+struct SchurPlan {
+  int first = 0, k = 0;                  // schur_first, |S|
+  std::vector<int> owner;                // [nsup] 0: front of B, -1: front of S
+  std::vector<int> cut;                  // cut roots (fronts of B whose parent is in S), ascending
+  std::vector<int> spos;                 // [k] output index of permuted S column j
+  // original K_SS entries per permuted S column j (the lower one of the pair): caller CSC position and output position
+  // (spos[j] * k + spos[i]), sorted by output position so that duplicates are adjacent
+  std::vector<long long> kss_ptr, kss_dst;
+  std::vector<int> kss_src;
+  std::vector<int> rec_ptr;              // [k + 1] per permuted S column: the cut roots whose rows contain it, ascending
+  std::vector<SchurRec> recs;
+  // expansion: the backward sweep over B's tasks alone, waiting on no S front (x_S is preset in the work vector)
+  std::vector<SVTask> bwd;
+  std::vector<int> bparent;              // sn_parent with the cut roots' parents replaced by -1
+};
+// schur: the caller's Schur set, in output order; sp: the solve plan built with `owner`
+SchurPlan build_schur_plan(const Symbolic& S, const std::vector<int>& schur, const SolvePlan& sp);
+// the owner vector above, for the plan builders (first: S.schur_first)
+std::vector<int> schur_owner(const Symbolic& S, int first);
+
 }  // namespace cb

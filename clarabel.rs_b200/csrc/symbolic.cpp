@@ -167,6 +167,18 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
   etree_upper(n, Up, Ui, parent0);
   TMARK("sym:   etree");
   postorder(n, parent0, post);
+  const int sf = opt.schur_first;
+  std::vector<int> post_cc;   // Schur set: the post-order of the whole tree, for the column counts
+  if (sf >= 0) {
+    // S columns are the last ones and their parents are S columns.  The subtrees of B that hang below S become roots
+    // of their own, the forest is post-ordered and its B trees are moved ahead of its S trees: every B column stays
+    // ahead of every S column and the numbering is still topological.
+    std::vector<int> pB(parent0);
+    for (int j = 0; j < sf; j++) if (pB[j] >= sf) pB[j] = -1;
+    post_cc.swap(post);
+    postorder(n, pB, post);
+    std::stable_partition(post.begin(), post.end(), [&](int v) { return v < sf; });
+  }
   S.perm.resize(n);
   S.iperm.resize(n);
   for (int k = 0; k < n; k++) S.perm[k] = perm0[post[k]];
@@ -184,30 +196,47 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
 
   // strictly-lower pattern by columns of the post-ordered matrix, straight from the caller's entries (the column
   // counts and the row-structure unions below do not depend on the order inside a column)
-  std::vector<int64_t> Lo_ptr(n + 1, 0);
-  for (int c = 0; c < n; c++) {
-    const int b = S.iperm[c];
-    for (int64_t p = Ap[c]; p < Ap[c + 1]; p++) {
-      const int a = S.iperm[Ai[p]];
-      if (a != b) Lo_ptr[(a < b ? a : b) + 1]++;
+  auto lower_pattern = [&](const std::vector<int>& ip, std::vector<int64_t>& Lo_ptr, std::vector<int>& Lo_idx) {
+    Lo_ptr.assign(n + 1, 0);
+    for (int c = 0; c < n; c++) {
+      const int b = ip[c];
+      for (int64_t p = Ap[c]; p < Ap[c + 1]; p++) {
+        const int a = ip[Ai[p]];
+        if (a != b) Lo_ptr[(a < b ? a : b) + 1]++;
+      }
     }
-  }
-  for (int j = 0; j < n; j++) Lo_ptr[j + 1] += Lo_ptr[j];
-  std::vector<int> Lo_idx(Lo_ptr[n]);
-  {
+    for (int j = 0; j < n; j++) Lo_ptr[j + 1] += Lo_ptr[j];
+    Lo_idx.resize(Lo_ptr[n]);
     std::vector<int64_t> pos(Lo_ptr.begin(), Lo_ptr.end() - 1);
     for (int c = 0; c < n; c++) {
-      const int b = S.iperm[c];
+      const int b = ip[c];
       for (int64_t p = Ap[c]; p < Ap[c + 1]; p++) {
-        const int a = S.iperm[Ai[p]];
+        const int a = ip[Ai[p]];
         if (a != b) Lo_idx[pos[a < b ? a : b]++] = a < b ? b : a;
       }
     }
-  }
+  };
+  std::vector<int64_t> Lo_ptr;
+  std::vector<int> Lo_idx;
+  lower_pattern(S.iperm, Lo_ptr, Lo_idx);
   std::vector<int64_t>().swap(Up);
   std::vector<int>().swap(Ui);
   TMARK("sym:   lower pattern");
-  colcounts_postordered(n, parent, Lo_ptr, Lo_idx, S.colcount);
+  if (post_cc.empty()) {
+    colcounts_postordered(n, parent, Lo_ptr, Lo_idx, S.colcount);
+  } else {
+    // every topological order of the tree has the same filled graph, so the counts are those of the post-order
+    // (which the counting algorithm needs), relabelled
+    std::vector<int> icc(n), pcc(n, -1), cc2;
+    for (int k = 0; k < n; k++) icc[perm0[post_cc[k]]] = k;
+    for (int j = 0; j < n; j++) if (parent0[j] >= 0) pcc[icc[perm0[j]]] = icc[perm0[parent0[j]]];
+    std::vector<int64_t> Lp2;
+    std::vector<int> Li2;
+    lower_pattern(icc, Lp2, Li2);
+    colcounts_postordered(n, pcc, Lp2, Li2, cc2);
+    S.colcount.resize(n);
+    for (int j = 0; j < n; j++) S.colcount[j] = cc2[icc[S.perm[j]]];
+  }
   TMARK("sym:   column counts");
   S.nnzL_simplicial = 0;
   S.flops_simplicial = 0;
@@ -226,13 +255,16 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
     //     the contiguous column range [r - size(r) + 1, r] and every row it reaches beyond r is in
     //     struct(L(:,r)), so the merged front is size(r) pivots by colcount[r] rows.  This trades a few
     //     explicit zeros at the leaves for far fewer fronts / children / tree levels.
+    //     With a Schur set, B's subtrees below S count as whole trees: a merged subtree is all B or all S.
+    std::vector<int> pcut(parent);
+    if (sf >= 0) for (int j = 0; j < sf; j++) if (pcut[j] >= sf) pcut[j] = -1;
     std::vector<int> sub(n, 1);
-    for (int j = 0; j < n; j++) if (parent[j] >= 0) sub[parent[j]] += sub[j];
+    for (int j = 0; j < n; j++) if (pcut[j] >= 0) sub[pcut[j]] += sub[j];
     std::vector<char> in_small(n, 0), small_root(n, 0);
     if (opt.relax_subtree > 1)
       for (int r = 0; r < n; r++) {
         const bool fits = sub[r] <= opt.relax_subtree;
-        const bool top = parent[r] < 0 || sub[parent[r]] > opt.relax_subtree;
+        const bool top = pcut[r] < 0 || sub[pcut[r]] > opt.relax_subtree;
         if (fits && top && sub[r] > 1) {
           small_root[r] = 1;
           for (int j = r - sub[r] + 1; j <= r; j++) in_small[j] = 1;
@@ -244,6 +276,7 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
       bool join = j > 0 && parent[j - 1] == j && cc[j] == cc[j - 1] - 1;
       if (in_small[j]) join = !(j == 0 || !in_small[j - 1] || small_root[j - 1]);
       else if (j > 0 && in_small[j - 1]) join = false;
+      if (j == sf) join = false;          // the first S column starts a supernode
       if (!join) fs.push_back(j);
     }
     int nf = (int)fs.size();
@@ -258,7 +291,7 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
     for (int p = 0; p < nf; p++) {
       int lastcol = fs[p + 1] - 1;
       int nr_p = cc[lastcol];
-      while (start[p] > 0) {
+      while (start[p] > 0 && start[p] != sf) {   // a B supernode never merges into an S one
         int c = col2f[start[p] - 1];        // supernode ending right before p
         int c_last = fs[c + 1] - 1;
         if (parent[c_last] < start[p] || parent[c_last] > lastcol) break;  // not a child of p
@@ -281,7 +314,8 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
     for (int s = 0; s < nf; s++) {
       if (dead[s]) continue;
       int b = start[s], e = fs[s + 1];
-      // split into panels of at most max_panel columns (balanced widths)
+      // split into panels of at most max_panel columns (balanced widths); a supernode lies in B or in S, so its
+      // panels do too
       int w = e - b;
       int np = (w + opt.max_panel - 1) / opt.max_panel;
       for (int k = 0; k < np; k++) sfirst.push_back(b + (int)((int64_t)w * k / np));
@@ -356,7 +390,7 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
     double wtot = 0.0;
     for (int s = 0; s < nsup; s++) {
       const int last = S.sn_first[s + 1] - 1;
-      if (parent[last] >= 0) gpar[s] = S.col2sn[parent[last]];
+      if (parent[last] >= 0 && !(last < sf && parent[last] >= sf)) gpar[s] = S.col2sn[parent[last]];   // B's trees are cut from S
       for (int j = S.sn_first[s]; j <= last; j++) wsub[s] += (double)cc[j] + 1.0;
       wtot += wsub[s];
     }
@@ -368,7 +402,7 @@ static int build(int n, const int64_t* Ap, const int32_t* Ai, const std::vector<
     for (int s = 0; s < nsup; s++) {
       const bool fits = wsub[s] <= thr;
       const bool top = gpar[s] < 0 || wsub[gpar[s]] > thr;
-      if (fits && top && cntsub[s] > 1) {
+      if (fits && top && cntsub[s] > 1 && !(sf >= 0 && S.sn_first[s] >= sf)) {   // S fronts: after the chunks
         Chunk c; c.first = s - cntsub[s] + 1; c.last = s;
         for (int t = c.first; t <= c.last; t++) chunk_of[t] = (int)chunks.size();
         chunks.push_back(std::move(c));
@@ -811,6 +845,59 @@ int analyse(int n, const int64_t* Ap, const int32_t* Ai, const int* perm_in,
     else { perm0.swap(pa); kind = ORDER_AMD; }
   }
   if ((int)perm0.size() != n) return -6;
+  S.ordering_used = kind;
+  return build(n, Ap, Ai, perm0, opt, S, false);
+}
+
+int analyse_schur(int n, const int64_t* Ap, const int32_t* Ai, const int* perm_in, const std::vector<int>& schur,
+                  const SymbolicOptions& opt_in, Symbolic& S) {
+  if (n <= 0) return -1;
+  const int k = (int)schur.size();
+  if (k < 1 || k >= n) return -4;
+  std::vector<char> in_s(n, 0);
+  for (int v : schur) {
+    if (v < 0 || v >= n || in_s[v]) return -4;
+    in_s[v] = 1;
+  }
+  for (int j = 0; j < n; j++) {
+    if (!(Ap[j] < Ap[j + 1])) return -2;
+    for (int64_t p = Ap[j]; p < Ap[j + 1]; p++)
+      if (Ai[p] > j || Ai[p] < 0) return -3;
+  }
+  std::vector<int> perm0;
+  int kind = ORDER_GIVEN;
+  if (perm_in) {
+    perm0.assign(perm_in, perm_in + n);
+    std::vector<char> seen(n, 0);
+    for (int q = 0; q < n; q++) {
+      if (perm0[q] < 0 || perm0[q] >= n || seen[perm0[q]]) return -5;
+      seen[perm0[q]] = 1;
+      if ((q >= n - k) != (in_s[perm0[q]] != 0)) return -5;
+    }
+  } else {
+    // B's own ordering on the subgraph it induces (diagonal added: a B column may hold entries in S rows only)
+    std::vector<int> bidx, bpos(n, -1);
+    for (int v = 0; v < n; v++) if (!in_s[v]) { bpos[v] = (int)bidx.size(); bidx.push_back(v); }
+    const int nb = (int)bidx.size();
+    std::vector<int64_t> Bp(nb + 1, 0);
+    std::vector<int32_t> Bi;
+    for (int c = 0; c < nb; c++) {
+      const int v = bidx[c];
+      for (int64_t p = Ap[v]; p < Ap[v + 1]; p++) if (bpos[Ai[p]] >= 0 && Ai[p] != v) Bi.push_back(bpos[Ai[p]]);
+      Bi.push_back(c);
+      Bp[c + 1] = (int64_t)Bi.size();
+    }
+    SymbolicOptions ob = opt_in;
+    ob.schur_first = -1;
+    Symbolic SB;
+    if (int rc = analyse(nb, Bp.data(), Bi.data(), nullptr, ob, SB)) return rc;
+    for (int q = 0; q < nb; q++) perm0.push_back(bidx[SB.perm[q]]);
+    perm0.insert(perm0.end(), schur.begin(), schur.end());
+    kind = SB.ordering_used;
+  }
+  SymbolicOptions opt = opt_in;
+  if (const char* e = std::getenv("CB_RELAX_SUBTREE")) opt.relax_subtree = std::atoi(e);
+  opt.schur_first = n - k;
   S.ordering_used = kind;
   return build(n, Ap, Ai, perm0, opt, S, false);
 }

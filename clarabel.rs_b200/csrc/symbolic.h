@@ -39,6 +39,10 @@ struct SymbolicOptions {
   int relax_subtree = 64; // merge every etree subtree with at most this many columns into one front (C2 sweep: 16/32/64 -> solve 1.76/1.66/1.58 ms)
   int relax_small = 8;    // always merge a child chain if the merged width stays <= this
   double relax_zeros = 0.25;  // otherwise merge when added explicit zeros / merged size <= this
+  // Schur complement handles: the first permuted column of the Schur set S, whose columns are the last n -
+  // schur_first of the given permutation.  B and S are post-ordered separately and no front holds columns of both.
+  // -1: no Schur set.
+  int schur_first = -1;
 };
 
 // One "task" = one supernode panel = one front of the multifrontal method.
@@ -96,6 +100,12 @@ int order_with_groups(int n, const int64_t* Ap, const int32_t* Ai, const int* gr
 // Returns 0 on success, negative on structural error.
 int analyse(int n, const int64_t* Ap, const int32_t* Ai, const int* perm_in,
             const SymbolicOptions& opt, Symbolic& S);
+
+// The analysis of a Schur complement handle: the columns outside `schur` (B) are ordered first, by opt.ordering on the
+// subgraph B induces (or perm_in, whose last schur.size() entries must be the Schur set: -5 otherwise), then the Schur
+// set S.  opt.schur_first is set to n - |S|.  -4: an empty, duplicate or out-of-range Schur set, or |S| = n.
+int analyse_schur(int n, const int64_t* Ap, const int32_t* Ai, const int* perm_in, const std::vector<int>& schur,
+                  const SymbolicOptions& opt, Symbolic& S);
 
 // ---- multi-GPU: subtree-to-rank mapping of one factorisation (SURVEY section 8e) ----
 // Independent subtrees of the assembly tree factor and solve independently; the fronts above the cut (the "top"

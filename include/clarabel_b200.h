@@ -135,6 +135,35 @@ int cldl_get_factor(const cldl_t *h, double *L_out, double *D_out, double *Dinv_
 int cldl_selected_inverse(cldl_t *h, double *nzval_out);
 int cldl_selected_inverse_dev(cldl_t *h, double *d_nzval_out);
 
+/* Schur complement: a handle over the same matrix as cldl_create plus a Schur set S of nschur caller indices
+ * (schur_idx, any order, 1 <= nschur < n: a set of all n indices is refused).  The rest, B, is eliminated and S never
+ * is: B is ordered first (by opts->ordering on the subgraph B induces, or by perm_or_null, whose last nschur entries
+ * must be exactly S, else CLDL_E_BAD_PERM), then S.  Every refactor factors B alone and assembles
+ *     Sc = K_SS - K_SB K_BB^-1 K_BS
+ * on the device: nschur x nschur doubles, column-major, both triangles, rows and columns in the order of schur_idx.
+ * With dynamic regularisation, Sc is the complement of K + E_B: E_B the regularisation of B's pivots, the only pivots
+ * factored (cldl_info.regularize_count / positive_inertia and the refactor's verdict cover B alone).  Value updates
+ * reach Sc at the next refactor.  Every sum has a fixed order: repeated refactors give the same bits.
+ *   - cldl_schur_reduce (condensation): w_S = b_S - K_SB K_BB^-1 b_B, nschur doubles in the order of schur_idx, from b
+ *     (n doubles, caller's order).
+ *   - cldl_schur_expand (expansion): given x_S (schur_idx order) solving Sc x_S = w_S, writes the whole x (n doubles,
+ *     x_B = K_BB^-1 (b_B - K_BS x_S) and x_S) for the b of the last condensation, whose forward state it consumes:
+ *     every expansion needs a condensation after the last refactor and after the previous expansion, else CLDL_E_ARG.
+ *   - Refusals: an empty, duplicate or out-of-range Schur set, or opts->shard_nranks > 1, at create: CLDL_E_ARG; a set
+ *     whose complement the device cannot allocate: CLDL_E_ARG.  The Schur calls before a refactor that returned 1:
+ *     CLDL_E_NOT_FACTORED.  cldl_solve(_dev), cldl_selected_inverse(_dev) and the shard entry points on a Schur handle,
+ *     and the Schur calls on any other handle: CLDL_E_ARG.
+ * The host-pointer forms synchronise; the _dev forms are only enqueued on the handle's stream (cldl_stream). */
+int cldl_create_schur(cldl_t **out, uint64_t n, const uint64_t *colptr, const uint64_t *rowval, const double *nzval,
+                      const int8_t *dsigns, const cldl_opts *opts, const uint64_t *perm_or_null, uint64_t nschur,
+                      const uint64_t *schur_idx);
+int cldl_schur_complement(cldl_t *h, double *out);
+int cldl_schur_complement_dev(cldl_t *h, double *d_out);
+int cldl_schur_reduce(cldl_t *h, double *wS, const double *b);
+int cldl_schur_reduce_dev(cldl_t *h, double *d_wS, const double *d_b);
+int cldl_schur_expand(cldl_t *h, double *x, const double *xS);
+int cldl_schur_expand_dev(cldl_t *h, double *d_x, const double *d_xS);
+
 /* ---- device-pointer twins (asynchronous on the handle's stream) ---- */
 int cldl_update_values_dev(cldl_t *h, const int32_t *d_index, const double *d_values, uint64_t len);
 int cldl_set_values_dev(cldl_t *h, const double *d_nzval);   /* whole array, caller order */

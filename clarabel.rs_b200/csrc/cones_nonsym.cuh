@@ -172,21 +172,37 @@ CB_HD bool pow_dual_feasible(const double* z, double a) {
   return z[0] > 0.0 && z[1] > 0.0 &&
          (exp(2.0 * a * lsafe(z[0] / a) + 2.0 * (1.0 - a) * lsafe(z[1] / (1.0 - a))) - z[2] * z[2]) > 0.0;
 }
+// Start of the one-sided Newton iterations of the power and generalised power cones' primal gradients: a point left
+// of the root x of  r (phi(x) - x^2) = 2x,  r = |w| the norm of the cone's w-part, psi = 1 / sum(alpha_i^2).  It is
+// genpowcone.rs:451-459's  -1/r + (psi r + sqrt((phi/r^2 + psi^2 - 1) phi)) / (phi - r^2)  with the -1/r cancelled
+// against the square root, which otherwise leaves 0 or a negative start for r below about 1e-9 sqrt(phi).
+CB_HD double newton_start(double r, double phi, double psi) {
+  const double p1 = psi * psi - 1.0;
+  return r * (psi + 1.0 + p1 / (1.0 + sqrt(1.0 + p1 * r * r / phi))) / (phi - r * r);
+}
+// Newton stopping rule shared by both cones (nonsymmetric_common.rs:191-219 stops BEFORE taking a step below
+// sqrt(eps) relative, which leaves an error of that size): a step that is not positive is rounding noise and is not
+// taken; a step below sqrt(eps) relative is taken and ends the iteration, the convergence being quadratic.
+CB_HD bool newton_step(double& x, double dx, double f1) {
+  if (!(dx >= EPS * x) || fabs(f1) < EPS) return false;
+  x += dx;
+  return dx >= SQRT_EPS * x;
+}
 // third component of the primal gradient: root of a scalar equation by a one-sided Newton iteration started to
-// the left of it (powcone.rs:440-490, nonsymmetric_common.rs:191-219)
+// the left of it (powcone.rs:440-490, nonsymmetric_common.rs:191-219).  The start is the generalised power cone's
+// with psi = 1 / (a^2 + (1-a)^2): powcone.rs:446 fixes psi = 2, which is left of the root only at a = 1/2.
 CB_HD double pow_newton(double s3, double phi, double a) {
-  double x = -1.0 / s3 + (2.0 * s3 + sqrt(phi * phi / (s3 * s3) + 3.0 * phi)) / (phi - s3 * s3);
-  const double t0 = -2.0 * a * lsafe(a) - 2.0 * (1.0 - a) * lsafe(1.0 - a);
-  const double lphi = lsafe(phi), b = 1.0 - a;
+  const double b = 1.0 - a;
+  double x = newton_start(s3, phi, 1.0 / (a * a + b * b));
+  const double t0 = -2.0 * a * lsafe(a) - 2.0 * b * lsafe(b);
+  const double lphi = lsafe(phi);
   for (int it = 0; it < 100; it++) {
     const double t1 = x * x, t2 = 2.0 * x / s3;
     const double f1 = 2.0 * a * a / (a * x + (1.0 + a) / s3) + 2.0 * b * b / (b * x + (2.0 - a) / s3) -
                       2.0 * (x + 1.0 / s3) / (t1 + t2);
     const double f0 = 2.0 * a * lsafe(2.0 * a * t1 + (1.0 + a) * t2) + 2.0 * b * lsafe(2.0 * b * t1 + (2.0 - a) * t2) -
                       lphi - lsafe(t1 + t2) - 2.0 * lsafe(t2) + t0;
-    const double dx = -f0 / f1;
-    if (dx < EPS || fabs(dx / x) < SQRT_EPS || fabs(f1) < EPS) break;
-    x += dx;
+    if (!newton_step(x, -f0 / f1, f1)) break;
   }
   return x;
 }
@@ -642,9 +658,10 @@ CB_HD double barrier_dual_at(const double* al, const double* q, const double* dq
   for (int i = d1; i < n; i++) { const double v = q[i] + a * dq[i]; ss += v * v; }
   return -lsafe(exp(res) - ss) - extra;
 }
-// primal barrier at s + a*ds = -f*(-g(s)) - degree (genpowcone.rs:310-331, 404-485).  The w-part of the primal
-// gradient uses the cone's stored Hessian vector r (genpowcone.rs:426), exactly like the reference.
-CB_HD double barrier_primal_at(const View& c, int k, const double* s, const double* ds, double a) {
+// The primal gradient at s + a*ds (genpowcone.rs:404-485) is g = (-(1 + al_i + al_i x |w|) / u_i, (x / |w|) w) for
+// (u, w) = s + a*ds, with x = 0 when |w| <= eps and otherwise the root of a scalar equation, found by a one-sided
+// Newton iteration (genpowcone.rs:451-485, nonsymmetric_common.rs:191-219).  Returns x, and |w| in *norm_w.
+CB_HD double primal_grad_scalar(const View& c, int k, const double* s, const double* ds, double a, double* norm_w) {
   const int id = c.list[k], o = c.off[id], n = c.dim[id], d1 = c.dim1[k];
   const double* al = c.alpha + o;
   double phi = 1.0;
@@ -657,24 +674,28 @@ CB_HD double barrier_primal_at(const View& c, int k, const double* s, const doub
     for (int i = d1; i < n; i++) { const double t = (s[o + i] + a * ds[o + i]) / mx; ss += t * t; }
     norm_r = mx * sqrt(ss);
   }
-  double g1 = 0.0;
-  const bool far = norm_r > EPS;
-  if (far) {   // one-sided Newton iteration (genpowcone.rs:451-485, nonsymmetric_common.rs:191-219)
-    const double psi = c.psi[k];
-    double x = -1.0 / norm_r + (psi * norm_r + sqrt((phi / norm_r / norm_r + psi * psi - 1.0) * phi)) / (phi - norm_r * norm_r);
-    for (int it = 0; it < 100; it++) {
-      double f1 = -(2.0 * x + 2.0 / norm_r) / (x * x + 2.0 * x / norm_r);
-      double f0 = -lsafe(2.0 * x / norm_r + x * x);
-      for (int i = 0; i < d1; i++) {
-        f1 += 2.0 * al[i] * norm_r / (norm_r * x + (1.0 + al[i]) / al[i]);
-        f0 += 2.0 * al[i] * (lsafe(x * norm_r + (1.0 + al[i]) / al[i]) - lsafe(s[o + i] + a * ds[o + i]));
-      }
-      const double dx = -f0 / f1;
-      if (dx < EPS || fabs(dx / x) < SQRT_EPS || fabs(f1) < EPS) break;
-      x += dx;
+  *norm_w = norm_r;
+  if (!(norm_r > EPS)) return 0.0;
+  double x = ns3::newton_start(norm_r, phi, c.psi[k]);
+  for (int it = 0; it < 100; it++) {
+    double f1 = -(2.0 * x + 2.0 / norm_r) / (x * x + 2.0 * x / norm_r);
+    double f0 = -lsafe(2.0 * x / norm_r + x * x);
+    for (int i = 0; i < d1; i++) {
+      f1 += 2.0 * al[i] * norm_r / (norm_r * x + (1.0 + al[i]) / al[i]);
+      f0 += 2.0 * al[i] * (lsafe(x * norm_r + (1.0 + al[i]) / al[i]) - lsafe(s[o + i] + a * ds[o + i]));
     }
-    g1 = x;
+    if (!ns3::newton_step(x, -f0 / f1, f1)) break;
   }
+  return x;
+}
+// primal barrier at s + a*ds = -f*(-g(s)) - degree (genpowcone.rs:310-331).  The w-part of g is formed from the
+// argument's own w-part; genpowcone.rs:426 takes the cone's stored Hessian vector r there, a shadowed name.
+CB_HD double barrier_primal_at(const View& c, int k, const double* s, const double* ds, double a) {
+  const int id = c.list[k], o = c.off[id], n = c.dim[id], d1 = c.dim1[k];
+  const double* al = c.alpha + o;
+  double norm_r;
+  const double g1 = primal_grad_scalar(c, k, s, ds, a, &norm_r);
+  const bool far = norm_r > EPS;
   // -f*(-g): dual barrier of the negated gradient, streamed
   double res = 0.0, extra = 0.0, ss = 0.0;
   for (int i = 0; i < d1; i++) {
@@ -683,7 +704,7 @@ CB_HD double barrier_primal_at(const View& c, int k, const double* s, const doub
     res += 2.0 * al[i] * lsafe(-gi / al[i]);
     extra += lsafe(-gi) * (1.0 - al[i]);
   }
-  if (far) for (int i = d1; i < n; i++) { const double gi = (g1 / norm_r) * c.qr[o + i]; ss += gi * gi; }
+  if (far) for (int i = d1; i < n; i++) { const double gi = (g1 / norm_r) * (s[o + i] + a * ds[o + i]); ss += gi * gi; }
   const double bd = -lsafe(exp(res) - ss) - extra;
   return -bd - (double)(d1 + 1);
 }

@@ -213,6 +213,23 @@ static int pow_is_dual_feasible(const double *z, double a)
     }
     return 0;
 }
+/* Start of the one-sided Newton iterations of the power and generalised power cones: genpowcone.rs:451-459's
+   -1/r + (psi r + sqrt((phi/r^2 + psi^2 - 1) phi)) / (phi - r^2) with the -1/r cancelled against the square root,
+   which otherwise gives 0 or a negative start for r below about 1e-9 sqrt(phi). */
+static double newton_onesided_start(double r, double phi, double psi)
+{
+    double p1 = psi * psi - 1.0;
+    return r * (psi + 1.0 + p1 / (1.0 + sqrt(1.0 + p1 * r * r / phi))) / (phi - r * r);
+}
+/* Stopping rule of nonsymmetric_common.rs:191-219, except that a step below sqrt(eps) relative is taken before the
+   iteration ends (the reference stops before it and keeps an error of that size), and a step is rounding noise when
+   it is below eps relative rather than absolute. */
+static int newton_onesided_step(double *x, double dx, double f1)
+{
+    if (!(dx >= NS_EPS * *x) || fabs(f1) < NS_EPS) return 0;
+    *x += dx;
+    return dx >= sqrt(NS_EPS) * *x;
+}
 /* nonsymmetric_common.rs:191-219 */
 static double newton_raphson_onesided_pow(double x0, double s3, double phi, double a, double t0)
 {
@@ -228,16 +245,15 @@ static double newton_raphson_onesided_pow(double x0, double s3, double phi, doub
         double f0 = 2.0 * a * logsafe(2.0 * a * u1 + (1.0 + a) * u2)
                   + 2.0 * (1.0 - a) * logsafe(2.0 * (1.0 - a) * u1 + (2.0 - a) * u2)
                   - logsafe(phi) - logsafe(u1 + u2) - 2.0 * logsafe(u2) + t0;
-        double dx = -f0 / dfdx;
-        if ((dx < NS_EPS) || (fabs(dx / x) < sqrt(NS_EPS)) || (fabs(dfdx) < NS_EPS)) break;
-        x += dx;
+        if (!newton_onesided_step(&x, -f0 / dfdx, dfdx)) break;
     }
     return x;
 }
-/* powcone.rs:440-490 */
+/* powcone.rs:440-490, started like the generalised power cone with psi = 1 / (a^2 + (1-a)^2); powcone.rs:446 fixes
+   psi = 2, which starts left of the root only at a = 1/2 */
 static double newton_raphson_powcone(double s3, double phi, double a)
 {
-    double x0 = -1.0 / s3 + (s3 * 2.0 + sqrt((phi * phi) / (s3 * s3) + phi * 3.0)) / (phi - s3 * s3);
+    double x0 = newton_onesided_start(s3, phi, 1.0 / (a * a + (1.0 - a) * (1.0 - a)));
     double t0 = -2.0 * a * logsafe(a) - 2.0 * (1.0 - a) * logsafe(1.0 - a);
     return newton_raphson_onesided_pow(x0, s3, phi, a, t0);
 }
@@ -411,20 +427,18 @@ static double gp_barrier_dual(const gp_t *K, const double *z)
 /* genpowcone.rs:451-485 + nonsymmetric_common.rs:191-219 */
 static double gp_newton_raphson(double norm_r, const double *p, double phi, const double *alpha, idx dim1, double psi)
 {
-    double x = -1.0 / norm_r + (psi * norm_r + sqrt((phi / norm_r / norm_r + psi * psi - 1.0) * phi)) / (phi - norm_r * norm_r);
+    double x = newton_onesided_start(norm_r, phi, psi);
     for (int iter = 0; iter < 100; iter++) {
         double f1 = -(2.0 * x + 2.0 / norm_r) / (x * x + 2.0 * x / norm_r);
         for (idx i = 0; i < dim1; i++) f1 = f1 + 2.0 * alpha[i] * norm_r / (norm_r * x + (1.0 + alpha[i]) / alpha[i]);
         double f0 = -logsafe(2.0 * x / norm_r + x * x);
         for (idx i = 0; i < dim1; i++) f0 = f0 + 2.0 * alpha[i] * (logsafe(x * norm_r + (1.0 + alpha[i]) / alpha[i]) - logsafe(p[i]));
-        double dx = -f0 / f1;
-        if ((dx < NS_EPS) || (fabs(dx / x) < sqrt(NS_EPS)) || (fabs(f1) < NS_EPS)) break;
-        x += dx;
+        if (!newton_onesided_step(&x, -f0 / f1, f1)) break;
     }
     return x;
 }
-/* genpowcone.rs:404-441.  NB the w-part of the gradient is formed from the cone's stored Hessian vector data.r,
-   not from the argument's own w-part (genpowcone.rs:426) -- restated as written. */
+/* genpowcone.rs:404-441, with the w-part of the gradient formed from the argument's own w-part: genpowcone.rs:426
+   takes the cone's stored Hessian vector data.r there (a shadowed name), which is the gradient only when w || r. */
 static void gp_gradient_primal(const gp_t *K, double *g, const double *s)
 {
     idx dim1 = K->dim1, dim2 = K->dim2;
@@ -433,7 +447,7 @@ static void gp_gradient_primal(const gp_t *K, double *g, const double *s)
     double norm_r = vnorm(s + dim1, dim2);
     if (norm_r > NS_EPS) {
         double g1 = gp_newton_raphson(norm_r, s, phi, K->alpha, dim1, K->psi);
-        for (idx i = 0; i < dim2; i++) g[dim1 + i] = (g1 / norm_r) * K->r[i];
+        for (idx i = 0; i < dim2; i++) g[dim1 + i] = (g1 / norm_r) * s[dim1 + i];
         for (idx i = 0; i < dim1; i++) g[i] = -(1.0 + K->alpha[i] + K->alpha[i] * g1 * norm_r) / s[i];
     } else {
         for (idx i = 0; i < dim2; i++) g[dim1 + i] = 0.0;

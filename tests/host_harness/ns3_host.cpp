@@ -81,6 +81,13 @@ double ns3h_barrier(ns3h* h, const double* z, const double* s, const double* dz,
   return b;
 }
 double ns3h_wright_omega(double z) { return wright_omega(z); }
+// the primal gradient update_scaling forms at the rows of every exponential / power cone (g is m long)
+void ns3h_grad_primal(ns3h* h, const double* s, double* g) {
+  for (int k = 0; k < h->v.n; k++) {
+    const int id = h->list[k], o = h->off[id];
+    if (h->type[id] == KIND_EXP) exp_grad_primal(s + o, g + o); else pow_grad_primal(s + o, h->alpha[k], g + o);
+  }
+}
 
 // ---------------------------------------------------------------- generalised power cones (namespace cb::gp)
 struct gph {
@@ -148,6 +155,21 @@ double gph_barrier(gph* h, const double* z, const double* s, const double* dz, c
   double b = 0.0;
   for (int k = 0; k < h->v.n; k++) b += cb::gp::body_barrier(h->v, k, z, s, dz, ds, al);
   return b;
+}
+// the primal gradient the primal barrier is formed from, at the rows of every generalised power cone (g is m long)
+void gph_grad_primal(gph* h, const double* s, double* g) {
+  std::vector<double> zero(h->m, 0.0);
+  for (int k = 0; k < h->v.n; k++) {
+    const int id = h->list[k], o = h->off[id], n = h->dim[id], d1 = h->dim1[k];
+    double nw;
+    const double x = cb::gp::primal_grad_scalar(h->v, k, s, zero.data(), 0.0, &nw);
+    const bool far = nw > EPS;
+    for (int i = 0; i < d1; i++) {
+      const double a = h->alpha[o + i];
+      g[o + i] = far ? -(1.0 + a + a * x * nw) / s[o + i] : -(1.0 + a) / s[o + i];
+    }
+    for (int i = d1; i < n; i++) g[o + i] = far ? (x / nw) * s[o + i] : 0.0;
+  }
 }
 // values the three expansion columns and their diagonals would receive: out_qr[m], out_p[m], out_D[3*n]
 void gph_kkt_values(gph* h, double* out_qr, double* out_p, double* out_D) {

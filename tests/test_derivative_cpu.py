@@ -9,7 +9,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMU_FULL = os.path.join(ROOT, "tests", "emu", "libclarabel_emu_full.so")
 
 
-def test_derivative_cases_on_the_emulated_build():
+def test_derivative_module_on_the_emulated_build():
     assert os.path.exists(EMU_FULL), "tests/emu/libclarabel_emu_full.so missing: run `make`"
     env = dict(os.environ, CLARABEL_EMU="1", CLARABEL_EMU_FULL="1")
     cmd = [sys.executable, "-m", "pytest", "-q", "-m", "gpu", "-p", "no:cacheprovider", "tests/test_zz_derivative_gpu.py",

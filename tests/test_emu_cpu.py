@@ -16,7 +16,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 MODULES = ["tests/test_cones_gpu.py", "tests/test_psd_gpu.py", "tests/test_ipm_gpu.py", "tests/test_zz_nonsym_gpu.py",
            "tests/test_zz_golden.py", "tests/test_zz_psd_large_gpu.py", "tests/test_zz_equilibration_gpu.py",
-           "tests/test_zz_data_updating_gpu.py", "tests/test_zz_algebra_gpu.py", "tests/test_cone_shapes_gpu.py"]
+           "tests/test_zz_data_updating_gpu.py", "tests/test_zz_algebra_gpu.py", "tests/test_cone_shapes_gpu.py",
+           "tests/test_nonsym_shapes_gpu.py"]
 # lists of tests/cone_shapes.py whose KKT matrix exceeds the dense stand-in's cap (PSD 64 and up, the 1e5 SOC, the
 # nonnegative pass boundaries); the full build runs PSD(64, 65)
 CONE_SHAPES_BIG = ["psd-n96-97", "psd-n128", "soc-long", "nonneg-75775", "nonneg-75776", "nonneg-75777", "nonneg-300000"]
@@ -31,6 +32,12 @@ _SHAPE_BIG = [f"tests/test_cone_shapes_gpu.py::{t}[{n}-{r}]" for n in CONE_SHAPE
              [f"tests/test_cone_shapes_gpu.py::test_margins[{n}-{r}]" for n in CONE_SHAPES_BIG for r in ("opening", "late", "indefinite")] + \
              [f"tests/test_cone_shapes_gpu.py::test_nonnegative_pass_boundaries[{n}]" for n in CONE_SHAPES_BIG]
 TOO_BIG += _SHAPE_BIG + [t.replace("[psd-n96-97", "[psd-n64-65") for t in _SHAPE_BIG if "psd-n96-97" in t]
+# the list of tests/nonsym_shapes.py with more exp / pow cones than one grid-stride pass of the barrier sum
+_NS_BIG = [f"tests/test_nonsym_shapes_gpu.py::test_update_scaling_Hs_and_secant[ns-big-{r}-{s}]"
+           for r in ("opening", "late", "late-off", "edge") for s in ("primal-dual", "dual")] + \
+          [f"tests/test_nonsym_shapes_gpu.py::test_barrier[ns-big-{r}]" for r in ("opening", "late", "late-off", "edge")] + \
+          [f"tests/test_nonsym_shapes_gpu.py::test_step_length[ns-big-{r}]" for r in ("opening", "late")]
+TOO_BIG += _NS_BIG
 
 
 # ---- the whole product, multifrontal kernels included (tests/emu/libclarabel_emu_full.so) ----
@@ -46,7 +53,7 @@ FULL_SKIP = [
     # amplified past the test's 1e-7; both thread orders agree bitwise with each other and the regularisation counts
     # equal the oracle's
     "tests/test_ldl_gpu.py::test_dynamic_regularisation_counts",
-] + _SHAPE_BIG
+] + _SHAPE_BIG + _NS_BIG
 
 
 

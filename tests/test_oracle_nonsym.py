@@ -193,19 +193,26 @@ def test_genpow_equals_powcone_when_dim_is_3():
 
 
 # ---- how much "same iteration count" means for nonsymmetric cones ----
-def test_iteration_count_is_sensitive_to_last_bit_noise():
+def test_iteration_count_under_last_bit_noise():
     """ORACLE_JITTER perturbs the outputs of the exponential / power cone arithmetic, here by at most 1 ulp
-    (ORACLE_JITTER_ULP; what a different libm or FMA contraction does).  Status and optimum do not move; the iteration count does (the backtracking searches
-    and scaling fall-backs are discrete decisions on quantities that reach a cone boundary at the solution).  This is
-    why the GPU parity tests for nonsymmetric problems compare status, optimum and the opening iterations, not counts."""
+    (ORACLE_JITTER_ULP; what a different libm or FMA contraction does).  Status and optimum do not move; on the
+    450-cone entropy / power mix the iteration count does (the backtracking searches and scaling fall-backs are discrete
+    decisions on quantities that reach a cone boundary at the solution).  This is why the GPU parity tests for
+    nonsymmetric problems compare status, optimum and the opening iterations, not counts.  tests/mixed_conic.rs with
+    the dual strategy moved too (7..16 iterations) while the power cone's primal gradient was off by up to 3e-2 for
+    alpha != 1/2; with the gradient converged it takes 6 iterations under every perturbation."""
     import json, os, subprocess, sys
     code = r'''
 import sys, json, numpy as np
 sys.path.insert(0, %r); sys.path.insert(0, %r)
 import oracle, test_oracle_nonsym as t
+from helpers import workloads
 ipm = oracle.IPM(*t.mixed_conic_data(), settings=oracle.default_settings(min_switch_step_length=0.999))
 ipm.set_perm(np.arange(ipm.N)); r = ipm.solve()
-print(json.dumps([r["status"], r["iterations"], r["obj_val"], ipm.trace[:2, 0].tolist()]))
+pr = workloads.entropy_power_mix(300, 150, n_eq=5, seed=6)
+mix = oracle.IPM(pr["P"], pr["q"], pr["A"], pr["b"], pr["cones"])
+mix.set_perm(np.arange(mix.N)); rm = mix.solve()
+print(json.dumps([r["status"], r["iterations"], r["obj_val"], rm["status"], rm["iterations"], rm["obj_val"]]))
 ''' % (os.path.dirname(os.path.dirname(os.path.abspath(__file__))), os.path.dirname(os.path.abspath(__file__)))
     runs = []
     for seed in [None, 1, 2, 3, 4, 5, 6]:
@@ -218,7 +225,9 @@ print(json.dumps([r["status"], r["iterations"], r["obj_val"], ipm.trace[:2, 0].t
         assert out.returncode == 0, out.stderr[-2000:]
         runs.append(json.loads(out.stdout.strip().splitlines()[-1]))
     base = runs[0]
-    assert base[0] == "Solved" and base[1] == 8                                          # the unperturbed oracle: the reference's answer
+    # the unperturbed oracle on mixed_conic.rs reaches the reference's answer (the reference itself takes 8 iterations)
+    assert base[0] == "Solved" and base[1] == 6
     assert all(abs(r[2]) <= 1e-8 for r in runs)                                          # every run reaches the optimum
-    assert all(r[0] in ("Solved", "AlmostSolved", "InsufficientProgress") for r in runs)  # ... the status label can flip
-    assert len({r[1] for r in runs}) > 1                                                # ... and the count does not survive
+    assert all(r[0] == "Solved" and r[1] == 6 for r in runs)                             # ... in the same count
+    assert all(r[3] == "Solved" and abs(r[5] - base[5]) <= 1e-8 * abs(base[5]) for r in runs)
+    assert len({r[4] for r in runs}) > 1                                                # the mix's count does not survive

@@ -2,6 +2,8 @@
 adjoint_derivative, clarabel.rs_b200/autograd.py) against an independent dense reference, the exact active-set
 derivative, central finite differences of the solver itself, and each other.  tests/test_derivative_cpu.py runs this
 module against the CUDA-on-CPU emulated build."""
+import os
+
 import numpy as np
 import pytest
 import scipy.sparse as sp
@@ -276,8 +278,11 @@ IDENTITY_TOL = {                 # measured on the H100 / on the emulated build 
     "basic_socp": 3e-7,          # 8.4e-8 / 5.1e-8 (3.0e11)
     "basic_expcone": 5e-8,       # 9.1e-9 / 1.0e-8 (6.8e12)
     "basic_sdp": 3e-8,           # 7.1e-9 / 1.3e-10 (1.2e10)
-    "basic_powcone": 5e-9,       # 1.3e-9 / 5.7e-10 (6.2e8)
+    "basic_powcone": 5e-9,       # 3.3e-9 / 5.6e-9 (9.5e17; 1.3e-9 / 5.7e-10 at cond 6.2e8, where the solve ended
+                                 # while the power cone's primal gradient stopped at its Newton start)
 }
+# the emulated build (another FMA contraction and libm than nvcc's) where it exceeds the device's bound
+EMU_IDENTITY_TOL = {"basic_powcone": 2e-8}
 
 
 @pytest.mark.parametrize("name", list(PROBLEMS))
@@ -289,6 +294,8 @@ def test_adjoint_is_the_transpose_of_the_forward_derivative(name):
     data, dev, r = solved(name)
     rng = np.random.default_rng(4)
     tol = IDENTITY_TOL.get(name, 1e-10)
+    if os.environ.get("CLARABEL_EMU") == "1":
+        tol = EMU_IDENTITY_TOL.get(name, tol)
     for _ in range(2):
         tl, tr = pair_products(dev, data, rng)
         scale = max(np.abs(tl).sum(), np.abs(tr).sum())

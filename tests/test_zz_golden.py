@@ -50,7 +50,7 @@ def test_device_reaches_the_reference_answer(path):
     dev = cb.CudaSolver(d["P"], d["q"], d["A"], d["b"], d["cones"], settings=cb.default_settings(**d["settings"]) if d["settings"] else None)
     r = dev.solve()
     if os.path.basename(path) == "mixed_conic_dual_strategy.json":
-        # knife-edge problem (see tests/test_oracle_nonsym.py::test_iteration_count_is_sensitive_to_last_bit_noise):
+        # the apex of every cone is the optimum (see tests/test_oracle_nonsym.py::test_iteration_count_under_last_bit_noise):
         # the optimum must be reached, the status label is not stable under last-bit differences
         assert r["status"] in ("Solved", "AlmostSolved", "InsufficientProgress") and abs(r["info"].cost_primal - exp["obj"]) <= 1e-6
         return
@@ -63,5 +63,5 @@ def test_device_reaches_the_reference_answer(path):
         assert r["iterations"] == ro["iterations"]          # symmetric cones: identical iteration counts
     else:
         # nonsymmetric cones: the iteration count is not stable under last-bit differences of the cone arithmetic
-        # (tests/test_oracle_nonsym.py::test_iteration_count_is_sensitive_to_last_bit_noise)
+        # (tests/test_oracle_nonsym.py::test_iteration_count_under_last_bit_noise)
         assert r["iterations"] <= 2 * ro["iterations"] + 10

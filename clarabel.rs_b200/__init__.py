@@ -145,6 +145,7 @@ EXPORTED_SYMBOLS = [
     "cldl_selected_inverse", "cldl_selected_inverse_dev",
     "cldl_create_schur", "cldl_schur_complement", "cldl_schur_complement_dev", "cldl_schur_reduce",
     "cldl_schur_reduce_dev", "cldl_schur_expand", "cldl_schur_expand_dev",
+    "cldl_logdet", "cldl_adjoint_solve", "cldl_adjoint_solve_dev",
 ]
 
 
@@ -381,6 +382,36 @@ class CudaLDLSolver:
         _check(f(self._h, _p(out, C.c_double)), "selected_inverse")
         return sps.csc_matrix((out, rv.astype(np.int64), cp.astype(np.int64)), shape=(self.n, self.n))
 
+    def slogdet(self):
+        """(sign, logabsdet) of K + E, the matrix the last ``refactor()`` factored (E its dynamic regularisation), from
+        the factor's pivots: logabsdet = sum log|d_k|, sign = (-1)^(negative pivots).  On a Schur handle, of
+        K_BB + E_B.  BackendError (NotFactored) before a refactor that returned True, (BadArgument) on a sharded
+        handle (see cldl_logdet)."""
+        f = self._L.cldl_logdet
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int32)]
+        f.restype = C.c_int
+        ld, sg = C.c_double(), C.c_int32()
+        _check(f(self._h, C.byref(ld), C.byref(sg)), "logdet")
+        return int(sg.value), float(ld.value)
+
+    def adjoint_solve(self, g, x):
+        """The adjoint of x = K^-1 b for an output gradient g: (gb, gvals) with gb = (K + E)^-1 g (n values) and gvals
+        the gradient of <g, x> with respect to the stored upper-triangle values, -(gb_i x_j + x_i gb_j) off the
+        diagonal and -gb_i x_i on it, as a ``scipy.sparse.csc_matrix`` with the constructor's pattern.  ``x`` is the
+        solution being differentiated (``solve(b)`` on the current factor).  BackendError (NotFactored) before a
+        refactor that returned True, (BadArgument) on a Schur or sharded handle (see cldl_adjoint_solve)."""
+        import scipy.sparse as sps
+        f = self._L.cldl_adjoint_solve
+        f.argtypes = [C.c_void_p] + [C.POINTER(C.c_double)] * 4
+        f.restype = C.c_int
+        g, x = _f64(g), _f64(x)
+        assert g.size == self.n and x.size == self.n
+        cp, rv = self._pattern
+        gb, gv = np.empty(self.n, np.float64), np.empty(rv.size, np.float64)
+        _check(f(self._h, _p(g, C.c_double), _p(x, C.c_double), _p(gb, C.c_double), _p(gv, C.c_double)),
+               "adjoint_solve")
+        return gb, sps.csc_matrix((gv, rv.astype(np.int64), cp.astype(np.int64)), shape=(self.n, self.n))
+
     # --- Schur complement handles (constructed with schur=...) ---
     def _schur_call(self, name, *args):
         f = getattr(self._L, name)
@@ -435,6 +466,20 @@ class CudaLDLSolver:
 
     def set_values_dev(self, d_ptr):
         _check(self._L.cldl_set_values_dev(self._h, C.c_void_p(d_ptr)), "set_values_dev")
+
+    def selected_inverse_dev(self, d_out_ptr):
+        f = self._L.cldl_selected_inverse_dev
+        f.argtypes = [C.c_void_p, C.c_void_p]
+        f.restype = C.c_int
+        _check(f(self._h, C.c_void_p(d_out_ptr)), "selected_inverse_dev")
+
+    def adjoint_solve_dev(self, d_g_ptr, d_x_ptr, d_gb_ptr, d_gvals_ptr):
+        """device pointers; d_x_ptr / d_gvals_ptr may be None (gb only)"""
+        f = self._L.cldl_adjoint_solve_dev
+        f.argtypes = [C.c_void_p] * 5
+        f.restype = C.c_int
+        _check(f(self._h, C.c_void_p(d_g_ptr), C.c_void_p(d_x_ptr), C.c_void_p(d_gb_ptr), C.c_void_p(d_gvals_ptr)),
+               "adjoint_solve_dev")
 
     def stream_ptr(self):
         return self._L.cldl_stream(self._h)

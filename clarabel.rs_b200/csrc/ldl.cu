@@ -1176,6 +1176,8 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     CK(upload(&dev.dsigns, ds));
   }
   nnzA = Ap[n];
+  h_colptr.assign(Ap, Ap + n + 1);
+  h_rowval.assign(Ai, Ai + nnzA);
   CK(cudaMalloc((void**)&dev.vals, (size_t)(nnzA ? nnzA : 1) * sizeof(double)));
   CK(cudaMemcpy(dev.vals, Ax, (size_t)nnzA * sizeof(double), cudaMemcpyHostToDevice));
   // The factor panels, the update-matrix arena and the update vectors are gigabytes (C4: 1.7 + 2.8 + 0.25 GB) and
@@ -1335,6 +1337,7 @@ void LDLObject::release() {
   fr(si.tasks); fr(si.col); fr(si.seg); fr(si.segpos); fr(si.Z); fr(d_si_pos); fr(d_si_init); fr(d_si_cnt); fr(d_si_out);
   fr(sv_bwd.tasks); fr(sv_bwd.parent); fr(d_sc_spos); fr(d_sc_kss_src); fr(d_sc_rec_ptr); fr(d_sc_kss_ptr); fr(d_sc_kss_dst);
   fr(d_sc_recs); fr(d_sc_out); fr(d_sc_vec);
+  fr(d_adj_cp); fr(d_adj_rv); fr(d_adj_buf); fr(d_ld_ws); fr(d_ld_cnt);
   if (h_status) cudaFreeHost(h_status);
   if (ev0) cudaEventDestroy(ev0);
   if (ev1) cudaEventDestroy(ev1);
@@ -1421,6 +1424,52 @@ int LDLObject::selected_inverse_async(double* d_out) {
   if (si.ntask) k_selinv<<<si_grid, SI_NT, (size_t)SI_SMEM_DOUBLES * 8, stream>>>(dev, si);
   if (nnzA) k_selinv_gather<<<(unsigned)((nnzA + 255) / 256), 256, 0, stream>>>(d_si_pos, si.Z, d_out, (long long)nnzA);
   CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+// log|det(K + E)| as one deterministic sum of log|d_k| over the factored pivots (B's alone on a Schur handle); the sign
+// from the negative-pivot count the refactor collected
+int LDLObject::logdet(double* logabsdet, int32_t* sign) {
+  if (sharded()) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  CK(cudaSetDevice(device));
+  if (!d_ld_ws) {
+    CK(cudaMalloc((void**)&d_ld_ws, (RED_BLOCKS + 1) * sizeof(double)));
+    CK(cudaMalloc((void**)&d_ld_cnt, sizeof(unsigned)));
+    CK(cudaMemsetAsync(d_ld_cnt, 0, sizeof(unsigned), stream));   // k_sum's last block leaves it at 0 again
+  }
+  const int nf = schur ? schur_first : n;
+  const double* D = dev.D;
+  double* out = d_ld_ws + RED_BLOCKS;
+  g_launches++;
+  k_sum<<<red_grid(nf), RED_THREADS, 0, stream>>>(nf, [=] __device__(int k) { return log(fabs(D[k])); },
+                                                  ReduceWS{d_ld_ws, d_ld_cnt}, out);
+  CK(cudaGetLastError());
+  double v = 0.0;
+  CK(cudaMemcpyAsync(&v, out, sizeof(double), cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));
+  *logabsdet = v;
+  *sign = (((uint64_t)nf - positive_inertia) & 1) ? -1 : 1;
+  return CLDL_OK;
+}
+
+// gb = (K + E)^-1 g by the solve's launch sequence, then (d_gvals non-null) the gradient of <g, x> on the caller's
+// pattern by k_grad_P
+int LDLObject::adjoint_async(const double* d_g, const double* d_x, double* d_gb, double* d_gvals) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  CK(cudaSetDevice(device));
+  if (d_gvals && !d_adj_cp) {
+    CK(upload(&d_adj_cp, h_colptr));
+    CK(upload(&d_adj_rv, h_rowval));
+    CK(cudaDeviceSynchronize());      // pageable uploads have landed before `stream` reads them
+  }
+  if (int rc = solve_async(d_gb, d_g)) return rc;
+  if (d_gvals && nnzA) {
+    g_launches++;
+    k_grad_P<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(n, d_adj_cp, d_adj_rv, d_x, d_gb, d_gvals);   // a warp per column
+    CK(cudaGetLastError());
+  }
   return CLDL_OK;
 }
 
@@ -2022,6 +2071,39 @@ int cldl_selected_inverse(cldl_t* h, double* nzval_out) {
 int cldl_selected_inverse_dev(cldl_t* h, double* d_nzval_out) {
   if (!h || !d_nzval_out) return CLDL_E_ARG;
   return h->obj.selected_inverse_async(d_nzval_out);
+}
+
+int cldl_logdet(cldl_t* h, double* logabsdet, int32_t* sign) {
+  if (!h || !logabsdet || !sign) return CLDL_E_ARG;
+  return h->obj.logdet(logabsdet, sign);
+}
+
+int cldl_adjoint_solve(cldl_t* h, const double* g, const double* x, double* gb, double* gvals) {
+  if (!h || !g || !gb || (gvals && !x)) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (o.sharded() || o.schur) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t n = (size_t)o.n, nnz = (size_t)o.nnzA;
+  if (!o.d_adj_buf && cudaMalloc((void**)&o.d_adj_buf, (3 * n + (nnz ? nnz : 1)) * sizeof(double)) != cudaSuccess) {
+    o.d_adj_buf = nullptr;
+    return CLDL_E_CUDA;
+  }
+  double *dg = o.d_adj_buf, *dx = dg + n, *dgb = dx + n, *dv = dgb + n;
+  if (cudaMemcpyAsync(dg, g, n * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess ||
+      (gvals && cudaMemcpyAsync(dx, x, n * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess))
+    return CLDL_E_CUDA;
+  int rc = o.adjoint_async(dg, dx, dgb, gvals ? dv : nullptr);
+  if (rc) return rc;
+  if (cudaMemcpyAsync(gb, dgb, n * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      (gvals && cudaMemcpyAsync(gvals, dv, nnz * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess) ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
+}
+int cldl_adjoint_solve_dev(cldl_t* h, const double* d_g, const double* d_x, double* d_gb, double* d_gvals) {
+  if (!h || !d_g || !d_gb || (d_gvals && !d_x)) return CLDL_E_ARG;
+  return h->obj.adjoint_async(d_g, d_x, d_gb, d_gvals);
 }
 
 int cldl_create_schur(cldl_t** out, uint64_t n, const uint64_t* colptr, const uint64_t* rowval,

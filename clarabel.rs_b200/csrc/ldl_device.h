@@ -136,6 +136,14 @@ class LDLObject {
   int si_grid = 0;
   int selinv_setup();
   int selected_inverse_async(double* d_out);
+  // log-determinant and adjoint solves (cldl_logdet, cldl_adjoint_solve): buffers allocated by the first call of each
+  std::vector<int> h_colptr, h_rowval;   // the caller's pattern, int32 CSC (kept by init for the pattern gradient)
+  int *d_adj_cp = nullptr, *d_adj_rv = nullptr;   // the same on the device, uploaded by the first adjoint call
+  double* d_adj_buf = nullptr;           // [3 n + nnzA] staging of the host-pointer adjoint: g, x, gb, gvals
+  double* d_ld_ws = nullptr;             // [RED_BLOCKS + 1] partial sums of the log-determinant, then its value
+  unsigned* d_ld_cnt = nullptr;          // the reduction's block counter
+  int logdet(double* logabsdet, int32_t* sign);
+  int adjoint_async(const double* d_g, const double* d_x, double* d_gb, double* d_gvals);
   // Schur complement handle (cldl_create_schur; SchurPlan in ldl_plan.h): B's fronts are factored, S's never
   std::vector<int> schur_set;            // non-empty: a Schur complement handle
   bool schur = false;

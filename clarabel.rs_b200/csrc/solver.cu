@@ -517,18 +517,6 @@ __global__ void k_grad_A(int n, const int* __restrict__ colptr, const int* __res
     g[p] = -(z[i] * uj + w[i] * xj);
   }
 }
-// gradient on the stored upper triangle of P (CSC, the caller's order): -(u_i x_j + x_i u_j) off the diagonal, -u_i x_i
-// on it; one warp per column
-__global__ void k_grad_P(int n, const int* __restrict__ colptr, const int* __restrict__ rowval,
-                         const double* __restrict__ x, const double* __restrict__ u, double* __restrict__ g) {
-  const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-  if (j >= n) return;
-  const double xj = x[j], uj = u[j];
-  for (int p = colptr[j] + lane; p < colptr[j + 1]; p += 32) {
-    const int i = rowval[p];
-    g[p] = i == j ? -(u[i] * xj) : -(u[i] * xj + x[i] * uj);
-  }
-}
 
 // ------------------------------------------------------------------ the IPM
 enum { IST_UNSOLVED = 0, IST_SOLVED, IST_PINF, IST_DINF, IST_ALMOST_SOLVED, IST_ALMOST_PINF, IST_ALMOST_DINF,

@@ -198,6 +198,21 @@ __global__ void k_map(int n, F f) {
   if (i < n) f(i);
 }
 
+// gradient of <g, x> with respect to the stored upper triangle of a symmetric matrix K (CSC, the caller's order), with
+// x = K^-1 b and u = K^-1 g: -(u_i x_j + x_i u_j) off the diagonal, -u_i x_i on it; one warp per column.  Used by the
+// interior-point adjoint (P's gradient, solver.cu) and by cldl_adjoint_solve (ldl.cu); static, so that each translation
+// unit has its own copy of the one definition.
+static __global__ void k_grad_P(int n, const int* __restrict__ colptr, const int* __restrict__ rowval,
+                                const double* __restrict__ x, const double* __restrict__ u, double* __restrict__ g) {
+  const int j = (int)((blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+  if (j >= n) return;
+  const double xj = x[j], uj = u[j];
+  for (int p = colptr[j] + lane; p < colptr[j + 1]; p += 32) {
+    const int i = rowval[p];
+    g[p] = i == j ? -(u[i] * xj) : -(u[i] * xj + x[i] * uj);
+  }
+}
+
 inline int red_grid(int n) {
   int g = (n + RED_THREADS - 1) / RED_THREADS;
   return g < 1 ? 1 : (g > RED_BLOCKS ? RED_BLOCKS : g);

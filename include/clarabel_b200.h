@@ -164,6 +164,38 @@ int cldl_schur_reduce_dev(cldl_t *h, double *d_wS, const double *d_b);
 int cldl_schur_expand(cldl_t *h, double *x, const double *xS);
 int cldl_schur_expand_dev(cldl_t *h, double *d_x, const double *d_xS);
 
+/* Log-determinant: log|det(K + E)| and its sign (-1)^(number of negative pivots), from the pivots D of the last refactor.
+ * E is the dynamic regularisation that refactor applied (cldl_info.regularize_count pivots), so with regularisation
+ * the result is the determinant of the regularised matrix, not of K.  One device sum of log|d_k| in a fixed order,
+ * then an 8-byte read; the sign comes from the refactor's positive_inertia count.
+ *   - Valid after a refactor that returned 1 (cldl_refactor, or cldl_refactor_dev followed by cldl_sync_status);
+ *     otherwise CLDL_E_NOT_FACTORED.
+ *   - On a Schur handle: log|det(K_BB + E_B)|, over B's pivots only (the first n - nschur in the permuted order),
+ *     which are the pivots the verdict and the counters cover.
+ *   - On a sharded handle: CLDL_E_ARG.
+ *   - Synchronises the handle's stream.  The first call allocates a few kilobytes of reduction workspace. */
+int cldl_logdet(cldl_t *h, double *logabsdet, int32_t *sign);
+
+/* Adjoint solve: the adjoint of x = K^-1 b.  For an output gradient g (n doubles):
+ *     gb = (K + E)^-1 g
+ * and, when gvals is not NULL, the gradient of <g, x> with respect to the stored values of the upper triangle passed
+ * to cldl_create (caller's CSC order, nnzA doubles):
+ *     gvals = -(gb_i x_j + x_i gb_j) off the diagonal, -gb_i x_i on it,
+ * where x is the solution being differentiated (cldl_solve(b) on the current factor).  NULL gvals computes gb only,
+ * and x may then be NULL.  E is the refactor's dynamic regularisation, as for cldl_logdet: with
+ * regularize_count > 0 these are the derivatives of the solve with K + E.  gb is the solve's launch sequence on g; the
+ * gradient is one kernel with a warp per column.
+ *   - Valid after a refactor that returned 1; otherwise CLDL_E_NOT_FACTORED.
+ *   - On a Schur handle (no cldl_solve there) and on a sharded handle: CLDL_E_ARG.
+ *   - The first call with gvals uploads the caller's pattern as int32 colptr / rowval ((n + 1 + nnzA) * 4 bytes); the
+ *     first host-pointer call allocates (3 n + nnzA) doubles of staging.  cldl_destroy frees them.
+ *   - No floating-point atomics: repeated calls give the same bits.
+ * For both calls the factor, D, 1/D and every later solve are left bit for bit unchanged.  cldl_adjoint_solve reads
+ * and writes host buffers and synchronises; the _dev form takes device buffers and is only enqueued on the handle's
+ * stream (cldl_stream). */
+int cldl_adjoint_solve(cldl_t *h, const double *g, const double *x, double *gb, double *gvals);
+int cldl_adjoint_solve_dev(cldl_t *h, const double *d_g, const double *d_x, double *d_gb, double *d_gvals);
+
 /* ---- device-pointer twins (asynchronous on the handle's stream) ---- */
 int cldl_update_values_dev(cldl_t *h, const int32_t *d_index, const double *d_values, uint64_t len);
 int cldl_set_values_dev(cldl_t *h, const double *d_nzval);   /* whole array, caller order */

@@ -382,20 +382,20 @@ int ConeSet::init(const ConeLayout& layout, cudaStream_t st) {
       row2blk[off[k] + i] = boff[k] + i;  // valid for diagonal-block cones
     }
   dev.ncones = nc; dev.m = m; dev.nsoc = (int)soc_list.size();
-  CCK(upload(&dev.type, type)); CCK(upload(&dev.off, off)); CCK(upload(&dev.dim, dim)); CCK(upload(&dev.boff, boff));
-  CCK(upload(&dev.sparse, sparse_flag)); CCK(upload(&dev.soc_list, soc_list)); CCK(upload(&dev.rowtag, tag));
-  CCK(upload(&row2blk_dev, row2blk));
+  CCK(own.upload(&dev.type, type)); CCK(own.upload(&dev.off, off)); CCK(own.upload(&dev.dim, dim)); CCK(own.upload(&dev.boff, boff));
+  CCK(own.upload(&dev.sparse, sparse_flag)); CCK(own.upload(&dev.soc_list, soc_list)); CCK(own.upload(&dev.rowtag, tag));
+  CCK(own.upload(&row2blk_dev, row2blk));
   const size_t mm = (size_t)(m ? m : 1), cc = (size_t)(nc ? nc : 1);
-  CCK(cudaMalloc((void**)&dev.w, mm * 8)); CCK(cudaMalloc((void**)&dev.lam, mm * 8));
-  CCK(cudaMalloc((void**)&dev.u, mm * 8)); CCK(cudaMalloc((void**)&dev.v, mm * 8));
-  CCK(cudaMalloc((void**)&dev.eta, cc * 8)); CCK(cudaMalloc((void**)&dev.dd, cc * 8));
-  CCK(cudaMalloc((void**)&dev.fail, sizeof(int)));
+  CCK(own.alloc(&dev.w, mm)); CCK(own.alloc(&dev.lam, mm));
+  CCK(own.alloc(&dev.u, mm)); CCK(own.alloc(&dev.v, mm));
+  CCK(own.alloc(&dev.eta, cc)); CCK(own.alloc(&dev.dd, cc));
+  CCK(own.alloc(&dev.fail, 1));
   CCK(cudaMemset(dev.w, 0, mm * 8)); CCK(cudaMemset(dev.lam, 0, mm * 8));
   CCK(cudaMemset(dev.u, 0, mm * 8)); CCK(cudaMemset(dev.v, 0, mm * 8));
   CCK(cudaMemset(dev.eta, 0, cc * 8)); CCK(cudaMemset(dev.dd, 0, cc * 8));
   CCK(cudaMemset(dev.fail, 0, sizeof(int)));
-  CCK(cudaMalloc((void**)&ws.partials, (size_t)(RED_BLOCKS + 64) * 4 * 8));
-  CCK(cudaMalloc((void**)&ws.counter, sizeof(unsigned)));
+  CCK(own.alloc(&ws.partials, (size_t)(RED_BLOCKS + 64) * 4));
+  CCK(own.alloc(&ws.counter, 1));
   CCK(cudaMemset(ws.counter, 0, sizeof(unsigned)));
   {
     std::vector<int> pn(nc, 0);
@@ -409,11 +409,11 @@ int ConeSet::init(const ConeLayout& layout, cudaStream_t st) {
         if (cs[k].dim > psd_numel_max) psd_numel_max = cs[k].dim;
       }
     dev.npsd = (int)psd_list.size();
-    CCK(upload(&dev.psd_list, psd_list)); CCK(upload(&dev.psd_n, pn)); CCK(upload(&dev.psd_moff, mo));
-    const size_t tb = (size_t)(tot ? tot : 1) * 8;
+    CCK(own.upload(&dev.psd_list, psd_list)); CCK(own.upload(&dev.psd_n, pn)); CCK(own.upload(&dev.psd_moff, mo));
+    const size_t tn = (size_t)(tot ? tot : 1), tb = tn * 8;
     psd_mat_total = tot;
-    CCK(cudaMalloc((void**)&dev.psd_R, tb)); CCK(cudaMalloc((void**)&dev.psd_Rinv, tb)); CCK(cudaMalloc((void**)&dev.psd_RRt, tb));
-    CCK(cudaMalloc((void**)&dev.psd_bar, tb));
+    CCK(own.alloc(&dev.psd_R, tn)); CCK(own.alloc(&dev.psd_Rinv, tn)); CCK(own.alloc(&dev.psd_RRt, tn));
+    CCK(own.alloc(&dev.psd_bar, tn));
     CCK(cudaMemset(dev.psd_R, 0, tb)); CCK(cudaMemset(dev.psd_Rinv, 0, tb)); CCK(cudaMemset(dev.psd_RRt, 0, tb));
     if (dev.npsd && psd_prepare()) return -20;
   }
@@ -424,18 +424,8 @@ int ConeSet::init(const ConeLayout& layout, cudaStream_t st) {
     if (gp_prepare()) return -20;
   }
   const size_t np = (size_t)RED_BLOCKS + soc_list.size() + psd_list.size() + 8;
-  CCK(cudaMalloc((void**)&d_pmin, np * 8)); CCK(cudaMalloc((void**)&d_psum, np * 8));
+  CCK(own.alloc(&d_pmin, np)); CCK(own.alloc(&d_psum, np));
   return 0;
-}
-
-void ConeSet::release() {
-  auto fr = [](const void* p) { if (p) cudaFree((void*)p); };
-  fr(dev.type); fr(dev.off); fr(dev.dim); fr(dev.boff); fr(dev.sparse); fr(dev.soc_list); fr(dev.rowtag);
-  fr(dev.w); fr(dev.lam); fr(dev.u); fr(dev.v); fr(dev.eta); fr(dev.dd); fr(dev.fail);
-  fr(ws.partials); fr(ws.counter); fr(row2blk_dev); fr(d_pmin); fr(d_psum);
-  fr(dev.psd_list); fr(dev.psd_n); fr(dev.psd_moff); fr(dev.psd_R); fr(dev.psd_Rinv); fr(dev.psd_RRt); fr(dev.psd_ws); fr(dev.psd_bar);
-  ns_release();
-  gp_release();
 }
 
 #define EW_GRID ((m + 255) / 256)

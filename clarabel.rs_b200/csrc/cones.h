@@ -66,6 +66,7 @@ struct ConeDev {
 // the device half of a cone layout
 class ConeSet : public ConeLayout {
  public:
+  DevOwner own;       // every buffer behind dev, ws and the scratch below
   ConeDev dev;
   cudaStream_t stream = nullptr;
   ReduceWS ws;
@@ -74,7 +75,6 @@ class ConeSet : public ConeLayout {
   double* d_psum = nullptr;
 
   int init(const ConeLayout& layout, cudaStream_t st);   // uploads the layout
-  void release();
 
   void set_identity_scaling();
   // failure -> dev.fail; mu and the scaling strategy only matter to the nonsymmetric cones
@@ -92,12 +92,10 @@ class ConeSet : public ConeLayout {
 
   // nonsymmetric pieces (cones_nonsym.cu)
   int gp_prepare();
-  void gp_release();
   // the three KKT columns + diagonal entries of every generalised power cone (datamaps.rs:314-337)
   void gp_kkt_fill(double* vals, const int* map_qr, const int* map_p, const int* map_D);
   double ns_amin = 1e-4, ns_step = 0.8;   // min_terminate_step_length, linesearch_backtrack_step
   int ns_prepare(const std::vector<double>& alpha_per_cone);
-  void ns_release();
   void unit_initialization(double* z, double* s);
   void ns_update_scaling(const double* s, const double* z, double mu, int strategy);
   void ns_get_Hs(double* Hs, double sign);

@@ -134,18 +134,14 @@ int ConeSet::ns_prepare(const std::vector<double>& alpha_per_cone) {
   if (dev.nns == 0) return 0;
   std::vector<double> al(ns_list.size());
   for (size_t k = 0; k < ns_list.size(); k++) al[k] = alpha_per_cone[ns_list[k]];
-  int* l = nullptr; double* a = nullptr;
-  NCK(cudaMalloc((void**)&l, ns_list.size() * sizeof(int)));
-  NCK(cudaMemcpy(l, ns_list.data(), ns_list.size() * sizeof(int), cudaMemcpyHostToDevice));
-  NCK(cudaMalloc((void**)&a, al.size() * 8));
-  NCK(cudaMemcpy(a, al.data(), al.size() * 8, cudaMemcpyHostToDevice));
-  dev.ns_list = l; dev.ns_alpha = a;
+  NCK(own.upload(&dev.ns_list, ns_list));
+  NCK(own.upload(&dev.ns_alpha, al));
   const size_t n = ns_list.size();
-  NCK(cudaMalloc((void**)&dev.ns_Hd, 6 * n * 8)); NCK(cudaMalloc((void**)&dev.ns_Hs, 6 * n * 8));
-  NCK(cudaMalloc((void**)&dev.ns_grad, 3 * n * 8)); NCK(cudaMalloc((void**)&dev.ns_z, 3 * n * 8));
+  NCK(own.alloc(&dev.ns_Hd, 6 * n)); NCK(own.alloc(&dev.ns_Hs, 6 * n));
+  NCK(own.alloc(&dev.ns_grad, 3 * n)); NCK(own.alloc(&dev.ns_z, 3 * n));
   NCK(cudaMemset(dev.ns_Hd, 0, 6 * n * 8)); NCK(cudaMemset(dev.ns_Hs, 0, 6 * n * 8));
   NCK(cudaMemset(dev.ns_grad, 0, 3 * n * 8)); NCK(cudaMemset(dev.ns_z, 0, 3 * n * 8));
-  NCK(cudaMalloc((void**)&dev.ns_jmax, sizeof(int)));
+  NCK(own.alloc(&dev.ns_jmax, 1));
   NCK(cudaMemset(dev.ns_jmax, 0, sizeof(int)));
   return 0;
 }
@@ -163,34 +159,19 @@ int ConeSet::gp_prepare() {
     for (size_t i = 0; i < c.alphas.size(); i++) { al[off[gp_list[k]] + i] = c.alphas[i]; sq += c.alphas[i] * c.alphas[i]; }
     psi[k] = 1.0 / sq;                       // genpowcone.rs:56
   }
-  int *l = nullptr, *dd = nullptr; double *a = nullptr, *ps = nullptr;
-  NCK(cudaMalloc((void**)&l, n * sizeof(int))); NCK(cudaMemcpy(l, gp_list.data(), n * sizeof(int), cudaMemcpyHostToDevice));
-  NCK(cudaMalloc((void**)&dd, n * sizeof(int))); NCK(cudaMemcpy(dd, d1.data(), n * sizeof(int), cudaMemcpyHostToDevice));
-  NCK(cudaMalloc((void**)&a, mm * 8)); NCK(cudaMemcpy(a, al.data(), mm * 8, cudaMemcpyHostToDevice));
-  NCK(cudaMalloc((void**)&ps, n * 8)); NCK(cudaMemcpy(ps, psi.data(), n * 8, cudaMemcpyHostToDevice));
-  dev.gp_list = l; dev.gp_dim1 = dd; dev.gp_alpha = a; dev.gp_psi = ps;
+  NCK(own.upload(&dev.gp_list, gp_list)); NCK(own.upload(&dev.gp_dim1, d1));
+  NCK(own.upload(&dev.gp_alpha, al)); NCK(own.upload(&dev.gp_psi, psi));
   for (double** q : {&dev.gp_grad, &dev.gp_p, &dev.gp_qr, &dev.gp_d1, &dev.gp_zc}) {
-    NCK(cudaMalloc((void**)q, mm * 8)); NCK(cudaMemset(*q, 0, mm * 8));
+    NCK(own.alloc(q, mm)); NCK(cudaMemset(*q, 0, mm * 8));
   }
-  for (double** q : {&dev.gp_d2, &dev.gp_mu}) { NCK(cudaMalloc((void**)q, n * 8)); NCK(cudaMemset(*q, 0, n * 8)); }
-  if (!dev.ns_jmax) { NCK(cudaMalloc((void**)&dev.ns_jmax, sizeof(int))); NCK(cudaMemset(dev.ns_jmax, 0, sizeof(int))); }
+  for (double** q : {&dev.gp_d2, &dev.gp_mu}) { NCK(own.alloc(q, n)); NCK(cudaMemset(*q, 0, n * 8)); }
+  if (!dev.ns_jmax) { NCK(own.alloc(&dev.ns_jmax, 1)); NCK(cudaMemset(dev.ns_jmax, 0, sizeof(int))); }
   return 0;
-}
-void ConeSet::gp_release() {
-  auto fr = [](const void* p) { if (p) cudaFree((void*)p); };
-  fr(dev.gp_list); fr(dev.gp_dim1); fr(dev.gp_alpha); fr(dev.gp_psi); fr(dev.gp_grad); fr(dev.gp_p); fr(dev.gp_qr);
-  fr(dev.gp_d1); fr(dev.gp_zc); fr(dev.gp_d2); fr(dev.gp_mu);
 }
 void ConeSet::gp_kkt_fill(double* vals, const int* map_qr, const int* map_p, const int* map_D) {
   if (!dev.ngp) return;
   g_launches++;
   k_gp_kkt_fill<<<GP_GRID, 128, 0, stream>>>(dev, vals, map_qr, map_p, map_D);
-}
-
-void ConeSet::ns_release() {
-  auto fr = [](const void* p) { if (p) cudaFree((void*)p); };
-  fr(dev.ns_list); fr(dev.ns_alpha); fr(dev.ns_Hd); fr(dev.ns_Hs); fr(dev.ns_grad); fr(dev.ns_z); fr(dev.ns_jmax);
-  dev.ns_jmax = nullptr;
 }
 
 // Cone::unit_initialization of the whole composite cone (compositecone.rs:217-221): zero everything, add the

@@ -1149,57 +1149,57 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   // the plans' view of the fronts: a Schur handle is rank 0 of a split whose top part is S (never factored)
   const std::vector<int> owner = schur ? schur_owner(S, n - (int)schur_set.size()) : shard.owner;
 
-  CK(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&stream_a, cudaStreamNonBlocking));
-  CK(cudaStreamCreateWithFlags(&stream_b, cudaStreamNonBlocking));
-  for (auto& e : ev_leaf) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  CK(cudaEventCreate(&ev0));
-  CK(cudaEventCreate(&ev1));
-  CK(cudaMallocHost((void**)&h_status, ST_COUNT * sizeof(int)));
+  CK(own.stream(&stream, cudaStreamNonBlocking));
+  CK(own.stream(&stream_a, cudaStreamNonBlocking));
+  CK(own.stream(&stream_b, cudaStreamNonBlocking));
+  for (auto& e : ev_leaf) CK(own.event(&e, cudaEventDisableTiming));
+  CK(own.event(&ev0));
+  CK(own.event(&ev1));
+  CK(own.alloc_host(&h_status, ST_COUNT));
 
   auto to_ll = [](const std::vector<int64_t>& v) { return std::vector<long long>(v.begin(), v.end()); };
-  CK(upload(&dev.sn_first, S.sn_first));
-  CK(upload(&dev.sn_rowptr, to_ll(S.sn_rowptr)));
-  CK(upload(&dev.sn_rows, S.sn_rows));
-  CK(upload(&dev.child_ptr, to_ll(S.child_ptr)));
-  CK(upload(&dev.child_list, S.child_list));
-  CK(upload(&dev.rel, S.rel));
-  CK(upload(&dev.panel_off, to_ll(S.panel_off)));
-  CK(upload(&dev.upd_off, to_ll(S.upd_off)));
-  CK(upload(&dev.asm_ptr, to_ll(S.asm_ptr)));
-  CK(upload(&dev.asm_src, S.asm_src));
-  CK(upload(&dev.asm_dst, to_ll(S.asm_dst)));
-  CK(upload(&dev.perm, S.perm));
+  CK(own.upload(&dev.sn_first, S.sn_first));
+  CK(own.upload(&dev.sn_rowptr, to_ll(S.sn_rowptr)));
+  CK(own.upload(&dev.sn_rows, S.sn_rows));
+  CK(own.upload(&dev.child_ptr, to_ll(S.child_ptr)));
+  CK(own.upload(&dev.child_list, S.child_list));
+  CK(own.upload(&dev.rel, S.rel));
+  CK(own.upload(&dev.panel_off, to_ll(S.panel_off)));
+  CK(own.upload(&dev.upd_off, to_ll(S.upd_off)));
+  CK(own.upload(&dev.asm_ptr, to_ll(S.asm_ptr)));
+  CK(own.upload(&dev.asm_src, S.asm_src));
+  CK(own.upload(&dev.asm_dst, to_ll(S.asm_dst)));
+  CK(own.upload(&dev.perm, S.perm));
   {
     std::vector<signed char> ds(n);
     for (int k = 0; k < n; k++) ds[k] = dsigns ? (signed char)dsigns[S.perm[k]] : (signed char)1;
-    CK(upload(&dev.dsigns, ds));
+    CK(own.upload(&dev.dsigns, ds));
   }
   nnzA = Ap[n];
   h_colptr.assign(Ap, Ap + n + 1);
   h_rowval.assign(Ai, Ai + nnzA);
-  CK(cudaMalloc((void**)&dev.vals, (size_t)(nnzA ? nnzA : 1) * sizeof(double)));
+  CK(own.alloc(&dev.vals, (size_t)nnzA));
   CK(cudaMemcpy(dev.vals, Ax, (size_t)nnzA * sizeof(double), cudaMemcpyHostToDevice));
   // The factor panels, the update-matrix arena and the update vectors are gigabytes (C4: 1.7 + 2.8 + 0.25 GB) and
-  // cudaMalloc of that size takes a few tenths of a second: a helper thread allocates them while this one builds and
-  // uploads the plans below (nothing in init touches these buffers; the first refactor does).  Joined before init returns.
+  // a device allocation of that size takes a few tenths of a second: a helper thread allocates them while this one builds
+  // and uploads the plans below (nothing in init touches these buffers; the first refactor does).  Joined before init returns.
   big_alloc_rc = 0;
   big_alloc = std::thread([this]() {
     if (cudaSetDevice(device) != cudaSuccess) { big_alloc_rc = 1; return; }
     const size_t nu = S.sn_rows.size() ? S.sn_rows.size() : 1;
-    if (cudaMalloc((void**)&dev.L, ((size_t)(S.L_alloc ? S.L_alloc : 1) + 8) * sizeof(double)) != cudaSuccess ||   // + slack: a bulk copy of the last panel is rounded up to 16 bytes
-        cudaMalloc((void**)&dev.U, (size_t)(S.upd_total ? S.upd_total : 1) * sizeof(double)) != cudaSuccess ||
-        cudaMalloc((void**)&dev.u, nu * sizeof(double)) != cudaSuccess ||
-        cudaMalloc((void**)&d_u2, nu * sizeof(double)) != cudaSuccess)
+    if (own.alloc(&dev.L, (size_t)(S.L_alloc ? S.L_alloc : 1) + 8) != cudaSuccess ||   // + slack: a bulk copy of the last panel is rounded up to 16 bytes
+        own.alloc(&dev.U, (size_t)S.upd_total) != cudaSuccess ||
+        own.alloc(&dev.u, nu) != cudaSuccess ||
+        own.alloc(&d_u2, nu) != cudaSuccess)
       big_alloc_rc = 1;
   });
   struct BigJoin { std::thread& t; ~BigJoin() { if (t.joinable()) t.join(); } } big_join{big_alloc};
-  CK(cudaMalloc((void**)&dev.D, (size_t)n * sizeof(double)));
-  CK(cudaMalloc((void**)&dev.Dinv, (size_t)n * sizeof(double)));
-  CK(cudaMalloc((void**)&d_xp, (size_t)n * sizeof(double)));
-  CK(cudaMalloc((void**)&d_xp2, (size_t)n * sizeof(double)));
-  CK(cudaMalloc((void**)&d_bx, (size_t)2 * n * sizeof(double)));
-  CK(cudaMalloc((void**)&dev.status, ST_COUNT * sizeof(int)));
+  CK(own.alloc(&dev.D, (size_t)n));
+  CK(own.alloc(&dev.Dinv, (size_t)n));
+  CK(own.alloc(&d_xp, (size_t)n));
+  CK(own.alloc(&d_xp2, (size_t)n));
+  CK(own.alloc(&d_bx, (size_t)2 * n));
+  CK(own.alloc(&dev.status, ST_COUNT));
   CK(cudaMemset(dev.status, 0, ST_COUNT * sizeof(int)));
   dev.reg_enable = o.regularize_enable;
   dev.reg_eps = o.regularize_eps;
@@ -1230,27 +1230,27 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   // tree level 0: plain launches
   CK(cudaFuncSetAttribute(k_factor_level<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, level_cap * 8));
   plan = std::move(l0.segs);
-  CK(upload(&dev.level_tasks, l0.level_tasks));
+  CK(own.upload(&dev.level_tasks, l0.level_tasks));
 
   // dataflow factorisation (k_factor_df)
-  CK(upload(&dev.sc_panel_src, fp.sc_panel_src));
-  CK(upload(&dev.sc_panel_dst, fp.sc_panel_dst));
-  CK(upload(&dev.sc_tile_src, fp.sc_tile_src));
-  CK(upload(&dev.sc_tile_dst, fp.sc_tile_dst));
+  CK(own.upload(&dev.sc_panel_src, fp.sc_panel_src));
+  CK(own.upload(&dev.sc_panel_dst, fp.sc_panel_dst));
+  CK(own.upload(&dev.sc_tile_src, fp.sc_tile_src));
+  CK(own.upload(&dev.sc_tile_dst, fp.sc_tile_dst));
   if (std::getenv("CB_TIMING")) std::fprintf(stderr, "[cb timing]     factor plan: %zu tasks, %zu child records, %zu big fronts, %zu tiles\n",
                                               fp.tasks.size(), fp.recs.size(), fp.sc_panel_ptr.size() - 1, fp.sc_tile_ptr.size() - 1);
   dff.ntask = (int)fp.tasks.size();
   dff_ntask_owned = fp.ntask_owned;
-  CK(upload(&dff.tasks, fp.tasks));
-  CK(upload(&dff.recs, fp.recs));
-  CK(upload(&d_dff_init, fp.cnt_init));
-  CK(cudaMalloc((void**)&d_dff_cnt, fp.cnt_init.size() * sizeof(int) + 16));
+  CK(own.upload(&dff.tasks, fp.tasks));
+  CK(own.upload(&dff.recs, fp.recs));
+  CK(own.upload(&d_dff_init, fp.cnt_init));
+  CK(own.alloc(&d_dff_cnt, fp.cnt_init.size() + 4));
   dff.pend = d_dff_cnt; dff.diag_done = d_dff_cnt + S.nsup; dff.rows_left = d_dff_cnt + 2 * (size_t)S.nsup;
   dff.tiles_left = d_dff_cnt + 3 * (size_t)S.nsup;
-  CK(cudaMalloc((void**)&dff.qhead, sizeof(int)));
-  CK(upload(&dff.parent, S.sn_parent));
-  CK(upload(&dff.big_pos, fp.big_pos));
-  CK(upload(&dff.tile_base, fp.tile_base));
+  CK(own.alloc(&dff.qhead, 1));
+  CK(own.upload(&dff.parent, S.sn_parent));
+  CK(own.upload(&dff.big_pos, fp.big_pos));
+  CK(own.upload(&dff.tile_base, fp.tile_base));
   CK(cudaFuncSetAttribute(k_factor_df, cudaFuncAttributeMaxDynamicSharedMemorySize, DF_SMEM_DOUBLES * 8));
   int occ = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_factor_df, DF_NT, (size_t)DF_SMEM_DOUBLES * 8));
@@ -1258,7 +1258,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   dff_nsup4 = 4 * (size_t)S.nsup;
   if (std::getenv("CB_DF_TRACE") && dff.ntask > 0) {
     h_dff_tasks = fp.tasks;
-    CK(cudaMalloc((void**)&dff.trace, (size_t)dff.ntask * 10 * sizeof(unsigned long long)));
+    CK(own.alloc(&dff.trace, (size_t)dff.ntask * 10));
     CK(cudaMemset(dff.trace, 0, (size_t)dff.ntask * 10 * sizeof(unsigned long long)));
   }
 
@@ -1269,25 +1269,25 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   sv_leafw_nrmax = sp.leafw_nrmax;
   sv_leafw_grid = sv_nleafw;      // one CTA per front (a loop over fronts inside fewer CTAs was slower: 312 vs 189 us forward on C4)
   sv_ntask_owned = sp.ntask_owned;
-  CK(upload(&dev.gat_ptr, sp.gat_ptr));
-  CK(upload(&dev.gat_src, sp.gat_src));
-  CK(upload(&d_sv_leaf1, sp.leaf1));
-  CK(upload(&d_sv_leafn, sp.leafn));
-  CK(upload(&d_sv_leafw, sp.leafw));
-  CK(upload(&sv.fronts, sp.fronts));
-  CK(upload(&sv.front2task, sp.front2task));
-  CK(upload(&sv.parent, S.sn_parent));
-  CK(upload(&sv.tasks, sp.tasks));
+  CK(own.upload(&dev.gat_ptr, sp.gat_ptr));
+  CK(own.upload(&dev.gat_src, sp.gat_src));
+  CK(own.upload(&d_sv_leaf1, sp.leaf1));
+  CK(own.upload(&d_sv_leafn, sp.leafn));
+  CK(own.upload(&d_sv_leafw, sp.leafw));
+  CK(own.upload(&sv.fronts, sp.fronts));
+  CK(own.upload(&sv.front2task, sp.front2task));
+  CK(own.upload(&sv.parent, S.sn_parent));
+  CK(own.upload(&sv.tasks, sp.tasks));
   // counters: [pend(nt) | fleft(nsup) | bleft(nsup)] are copied from their initial values before every solve,
   // [tdone(nt) | ydone(nsup) | done(nsup) | qhead(2)] are cleared
   sv_ninit = sp.cnt_init.size();
   sv_nzero = (size_t)nt + 2 * (size_t)S.nsup + 2;
-  CK(upload(&d_sv_init, sp.cnt_init));
-  CK(cudaMalloc((void**)&d_sv_cnt, (sv_ninit + sv_nzero) * sizeof(int)));
+  CK(own.upload(&d_sv_init, sp.cnt_init));
+  CK(own.alloc(&d_sv_cnt, sv_ninit + sv_nzero));
   sv.pend = d_sv_cnt; sv.fleft = d_sv_cnt + nt; sv.bleft = sv.fleft + S.nsup;
   sv.tdone = d_sv_cnt + sv_ninit; sv.ydone = sv.tdone + nt; sv.done = sv.ydone + S.nsup; sv.qhead = sv.done + S.nsup;
   sv.bpart_stride = (long long)(sp.nslots ? sp.nslots : 1) * CB_PB_MAXNS;
-  CK(cudaMalloc((void**)&sv.bpart, (size_t)2 * sv.bpart_stride * sizeof(double)));
+  CK(own.alloc(&sv.bpart, (size_t)2 * sv.bpart_stride));
   sv.ntask = nt;
   // launch geometry: dynamic shared memory = slab + vectors for one or two right-hand sides
   for (int nr2 = 1; nr2 <= 2; nr2++)
@@ -1298,7 +1298,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   sv_grid = nsm * sv_occ;
   use_dataflow = true;
   if (std::getenv("CB_DF_TRACE_SOLVE") && nt > 0) {
-    CK(cudaMalloc((void**)&sv.trace, (size_t)nt * 8 * sizeof(unsigned long long)));
+    CK(own.alloc(&sv.trace, (size_t)nt * 8));
     CK(cudaMemset(sv.trace, 0, (size_t)nt * 8 * sizeof(unsigned long long)));
     h_sv_tasks = sp.tasks;
   }
@@ -1308,7 +1308,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   if (sharded()) {
     d_shard_xidx.assign(shard_nranks, nullptr);
     for (int w = 0; w < 2; w++) { d_shard_segs[w].assign(shard_nranks, nullptr); shard_nsegs[w].assign(shard_nranks, 0); }
-    for (int g = 0; g < shard_nranks; g++) CK(upload(&d_shard_xidx[g], shard_xidx[g]));
+    for (int g = 0; g < shard_nranks; g++) CK(own.upload(&d_shard_xidx[g], shard_xidx[g]));
   }
   if (schur && (rc = schur_setup(sp))) return rc;
   if (big_alloc.joinable()) big_alloc.join();
@@ -1321,30 +1321,7 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
 
 void LDLObject::release() {
   cudaSetDevice(device);
-  for (auto& w : d_shard_segs) for (auto& p : w) if (p) { cudaFree(p); p = nullptr; }
-  for (int* p : d_shard_xidx) if (p) cudaFree(p);
-  d_shard_xidx.clear();
   if (nccl_comm) { if (NcclApi* a = nccl_api(nullptr)) a->CommDestroy((cb_ncclComm_t)nccl_comm); nccl_comm = nullptr; }
-  if (d_xsend) { cudaFree(d_xsend); d_xsend = nullptr; }
-  if (d_xrecv) { cudaFree(d_xrecv); d_xrecv = nullptr; }
-  xbuf_cap = 0;
-  auto fr = [](const void* p) { if (p) cudaFree((void*)p); };
-  fr(dev.sn_first); fr(dev.sn_rowptr); fr(dev.sn_rows); fr(dev.child_ptr); fr(dev.child_list);
-  fr(dev.rel); fr(dev.panel_off); fr(dev.upd_off); fr(dev.asm_ptr); fr(dev.asm_src);
-  fr(dev.asm_dst); fr(dev.level_tasks); fr(dev.perm); fr(dev.dsigns); fr(dev.vals); fr(dev.L);
-  fr(dev.U); fr(dev.D); fr(dev.Dinv); fr(dev.u); fr(dev.status); fr(d_xp); fr(d_bx);
-  fr(d_tmp_idx); fr(d_tmp_val); fr(d_tmp_sgn); fr(sv.tasks); fr(sv.fronts); fr(sv.front2task); fr(sv.parent); fr(sv.bpart); fr(sv.trace); fr(d_sv_cnt); fr(d_sv_init); fr(d_sv_leaf1); fr(d_sv_leafn); fr(d_sv_leafw); fr(d_xp2); fr(d_u2); fr(dff.tasks); fr(dff.recs); fr(d_dff_init); fr(d_dff_cnt); fr(dff.qhead); fr(dff.parent); fr(dff.big_pos); fr(dff.tile_base); fr(dff.trace); fr(dev.gat_ptr); fr(dev.gat_src); fr(dev.sc_panel_src); fr(dev.sc_panel_dst); fr(dev.sc_tile_src); fr(dev.sc_tile_dst);
-  fr(si.tasks); fr(si.col); fr(si.seg); fr(si.segpos); fr(si.Z); fr(d_si_pos); fr(d_si_init); fr(d_si_cnt); fr(d_si_out);
-  fr(sv_bwd.tasks); fr(sv_bwd.parent); fr(d_sc_spos); fr(d_sc_kss_src); fr(d_sc_rec_ptr); fr(d_sc_kss_ptr); fr(d_sc_kss_dst);
-  fr(d_sc_recs); fr(d_sc_out); fr(d_sc_vec);
-  fr(d_adj_cp); fr(d_adj_rv); fr(d_adj_buf); fr(d_ld_ws); fr(d_ld_cnt);
-  if (h_status) cudaFreeHost(h_status);
-  if (ev0) cudaEventDestroy(ev0);
-  if (ev1) cudaEventDestroy(ev1);
-  for (auto& e : ev_leaf) if (e) { cudaEventDestroy(e); e = nullptr; }
-  if (stream_a) { cudaStreamDestroy(stream_a); stream_a = nullptr; }
-  if (stream_b) { cudaStreamDestroy(stream_b); stream_b = nullptr; }
-  if (stream) cudaStreamDestroy(stream);
 }
 
 // the start of every refactor: status, counters and queue head of k_factor_df reset, tree level 0 factored by the
@@ -1392,15 +1369,15 @@ int LDLObject::refactor_async() {
 int LDLObject::selinv_setup() {
   const SelinvPlan p = build_selinv_plan(S);
   si.ntask = (int)p.tasks.size();
-  CK(upload(&si.tasks, p.tasks));
-  CK(upload(&si.col, p.col));
-  CK(upload(&si.seg, p.seg));
-  CK(upload(&si.segpos, p.segpos));
-  CK(upload(&d_si_pos, p.caller_pos));
-  CK(upload(&d_si_init, p.rows_left));
-  CK(cudaMalloc((void**)&d_si_cnt, (2 * (size_t)S.nsup + 1) * sizeof(int)));
+  CK(own.upload(&si.tasks, p.tasks));
+  CK(own.upload(&si.col, p.col));
+  CK(own.upload(&si.seg, p.seg));
+  CK(own.upload(&si.segpos, p.segpos));
+  CK(own.upload(&d_si_pos, p.caller_pos));
+  CK(own.upload(&d_si_init, p.rows_left));
+  CK(own.alloc(&d_si_cnt, 2 * (size_t)S.nsup + 1));
   si.rows_left = d_si_cnt; si.done = d_si_cnt + S.nsup; si.qhead = d_si_cnt + 2 * (size_t)S.nsup;
-  CK(cudaMalloc((void**)&si.Z, ((size_t)(S.L_alloc ? S.L_alloc : 1)) * sizeof(double)));
+  CK(own.alloc(&si.Z, (size_t)S.L_alloc));
   CK(cudaFuncSetAttribute(k_selinv, cudaFuncAttributeMaxDynamicSharedMemorySize, SI_SMEM_DOUBLES * 8));
   int occ = 0, nsm = 0;
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_selinv, SI_NT, (size_t)SI_SMEM_DOUBLES * 8));
@@ -1416,7 +1393,8 @@ int LDLObject::selected_inverse_async(double* d_out) {
   if (!factor_ok) return CLDL_E_NOT_FACTORED;
   CK(cudaSetDevice(device));
   if (!si.Z) {
-    if (int rc = selinv_setup()) return rc;
+    const size_t mk = own.mark();
+    if (int rc = selinv_setup()) { own.release_since(mk); si.Z = nullptr; return rc; }
   }
   CK(cudaMemcpyAsync(si.rows_left, d_si_init, (size_t)S.nsup * sizeof(int), cudaMemcpyDeviceToDevice, stream));
   CK(cudaMemsetAsync(si.done, 0, ((size_t)S.nsup + 1) * sizeof(int), stream));
@@ -1434,9 +1412,11 @@ int LDLObject::logdet(double* logabsdet, int32_t* sign) {
   if (!factor_ok) return CLDL_E_NOT_FACTORED;
   CK(cudaSetDevice(device));
   if (!d_ld_ws) {
-    CK(cudaMalloc((void**)&d_ld_ws, (RED_BLOCKS + 1) * sizeof(double)));
-    CK(cudaMalloc((void**)&d_ld_cnt, sizeof(unsigned)));
-    CK(cudaMemsetAsync(d_ld_cnt, 0, sizeof(unsigned), stream));   // k_sum's last block leaves it at 0 again
+    const size_t mk = own.mark();
+    if (own.alloc(&d_ld_ws, RED_BLOCKS + 1) || own.alloc(&d_ld_cnt, 1) ||
+        cudaMemsetAsync(d_ld_cnt, 0, sizeof(unsigned), stream)) {   // k_sum's last block leaves it at 0 again
+      own.release_since(mk); d_ld_ws = nullptr; return CLDL_E_CUDA;
+    }
   }
   const int nf = schur ? schur_first : n;
   const double* D = dev.D;
@@ -1460,9 +1440,11 @@ int LDLObject::adjoint_async(const double* d_g, const double* d_x, double* d_gb,
   if (!factor_ok) return CLDL_E_NOT_FACTORED;
   CK(cudaSetDevice(device));
   if (d_gvals && !d_adj_cp) {
-    CK(upload(&d_adj_cp, h_colptr));
-    CK(upload(&d_adj_rv, h_rowval));
-    CK(cudaDeviceSynchronize());      // pageable uploads have landed before `stream` reads them
+    const size_t mk = own.mark();
+    if (own.upload(&d_adj_cp, h_colptr) || own.upload(&d_adj_rv, h_rowval) ||
+        cudaDeviceSynchronize()) {      // pageable uploads have landed before `stream` reads them
+      own.release_since(mk); d_adj_cp = nullptr; return CLDL_E_CUDA;
+    }
   }
   if (int rc = solve_async(d_gb, d_g)) return rc;
   if (d_gvals && nnzA) {
@@ -1481,26 +1463,25 @@ int LDLObject::schur_setup(const SolvePlan& sp) {
   for (int c : p.cut)     // their update matrices and vectors must hold S rows only
     if (S.sn_rowptr[c + 1] > S.sn_rowptr[c] && S.sn_rows[S.sn_rowptr[c]] < schur_first) return CLDL_E_ARG;
   const size_t kk = (size_t)schur_k * (size_t)schur_k;
-  if (cudaMalloc((void**)&d_sc_out, kk * sizeof(double)) != cudaSuccess) {
+  if (own.alloc(&d_sc_out, kk) != cudaSuccess) {
     cudaGetLastError();
-    d_sc_out = nullptr;
     std::fprintf(stderr, "[clarabel_b200] a Schur set of %d needs %zu bytes for the complement\n", schur_k, kk * sizeof(double));
     return CLDL_E_ARG;
   }
-  CK(cudaMalloc((void**)&d_sc_vec, 2 * (size_t)schur_k * sizeof(double)));
-  CK(upload(&d_sc_spos, p.spos));
-  CK(upload(&d_sc_kss_ptr, p.kss_ptr));
-  CK(upload(&d_sc_kss_dst, p.kss_dst));
-  CK(upload(&d_sc_kss_src, p.kss_src));
-  CK(upload(&d_sc_rec_ptr, p.rec_ptr));
-  CK(upload(&d_sc_recs, p.recs));
+  CK(own.alloc(&d_sc_vec, 2 * (size_t)schur_k));
+  CK(own.upload(&d_sc_spos, p.spos));
+  CK(own.upload(&d_sc_kss_ptr, p.kss_ptr));
+  CK(own.upload(&d_sc_kss_dst, p.kss_dst));
+  CK(own.upload(&d_sc_kss_src, p.kss_src));
+  CK(own.upload(&d_sc_rec_ptr, p.rec_ptr));
+  CK(own.upload(&d_sc_recs, p.recs));
   sv_bwd = sv;
   sv_bwd.ntask = (int)p.bwd.size();
   sv_bwd.tasks = nullptr;
   sv_bwd.parent = nullptr;
   sv_bwd.trace = nullptr;
-  CK(upload(&sv_bwd.tasks, p.bwd.empty() ? std::vector<SVTask>(1) : p.bwd));
-  CK(upload(&sv_bwd.parent, p.bparent));
+  CK(own.upload(&sv_bwd.tasks, p.bwd.empty() ? std::vector<SVTask>(1) : p.bwd));
+  CK(own.upload(&sv_bwd.parent, p.bparent));
   return CLDL_OK;
 }
 
@@ -1745,12 +1726,14 @@ int LDLObject::set_nccl(const char* libpath, const unsigned char* id128, int nra
 int LDLObject::exchange(int what, double* d_x) {
   uint64_t cnt = 1;
   for (int r = 0; r < shard_nranks; r++) cnt = std::max(cnt, shard_count(what, r));
-  if ((size_t)cnt > xbuf_cap) {
-    if (d_xsend) cudaFree(d_xsend);
-    if (d_xrecv) cudaFree(d_xrecv);
-    xbuf_cap = (size_t)cnt + (size_t)cnt / 4 + 64;
-    CK(cudaMalloc((void**)&d_xsend, xbuf_cap * sizeof(double)));
-    CK(cudaMalloc((void**)&d_xrecv, xbuf_cap * (size_t)shard_nranks * sizeof(double)));
+  if ((size_t)cnt > xbuf_cap) {     // the old buffers go first: a failure leaves none and a capacity of 0
+    own.free(d_xsend); own.free(d_xrecv);
+    d_xsend = d_xrecv = nullptr;
+    xbuf_cap = 0;
+    const size_t cap = (size_t)cnt + (size_t)cnt / 4 + 64;
+    CK(own.alloc(&d_xsend, cap));
+    CK(own.alloc(&d_xrecv, cap * (size_t)shard_nranks));
+    xbuf_cap = cap;
   }
   int rc = shard_pack(what, d_xsend, d_x);
   if (rc) return rc;
@@ -1803,11 +1786,8 @@ int LDLObject::shard_seglist(int what, int rank, const long long** d_out, int* n
     }
     shard_nsegs[what][rank] = (int)(h.size() / 3);
     if (h.empty()) h.assign(3, 0);
-    long long* dp = nullptr;
-    CK(cudaMalloc((void**)&dp, h.size() * sizeof(long long)));
-    CK(cudaMemcpy(dp, h.data(), h.size() * sizeof(long long), cudaMemcpyHostToDevice));
-    CK(cudaDeviceSynchronize());
-    slot = dp;
+    const size_t mk = own.mark();
+    if (own.upload(&slot, h) || cudaDeviceSynchronize()) { own.release_since(mk); slot = nullptr; return CLDL_E_CUDA; }
   }
   *d_out = slot; *nseg = shard_nsegs[what][rank];
   return CLDL_OK;
@@ -1849,13 +1829,14 @@ int LDLObject::shard_unpack(int what, int rank, const double* d_buf, double* d_x
 int LDLObject::ensure_tmp(size_t len) {
   if (len <= tmp_cap) return 0;
   CK(cudaSetDevice(device));
-  if (d_tmp_idx) cudaFree(d_tmp_idx);
-  if (d_tmp_val) cudaFree(d_tmp_val);
-  if (d_tmp_sgn) cudaFree(d_tmp_sgn);
-  tmp_cap = len + len / 2 + 256;
-  CK(cudaMalloc((void**)&d_tmp_idx, tmp_cap * sizeof(int)));
-  CK(cudaMalloc((void**)&d_tmp_val, tmp_cap * sizeof(double)));
-  CK(cudaMalloc((void**)&d_tmp_sgn, tmp_cap));
+  own.free(d_tmp_idx); own.free(d_tmp_val); own.free(d_tmp_sgn);   // first: a failure leaves none and a capacity of 0
+  d_tmp_idx = nullptr; d_tmp_val = nullptr; d_tmp_sgn = nullptr;
+  tmp_cap = 0;
+  const size_t cap = len + len / 2 + 256;
+  CK(own.alloc(&d_tmp_idx, cap));
+  CK(own.alloc(&d_tmp_val, cap));
+  CK(own.alloc(&d_tmp_sgn, cap));
+  tmp_cap = cap;
   return 0;
 }
 
@@ -1924,7 +1905,6 @@ int cldl_create(cldl_t** out, uint64_t n, const uint64_t* colptr, const uint64_t
   int rc = h->obj.init((int)n, Ap.data(), Ai.data(), nzval, dsigns, o,
                        perm_or_null ? perm.data() : nullptr);
   if (rc != CLDL_OK) {
-    h->obj.release();
     delete h;
     return rc;
   }
@@ -1934,7 +1914,6 @@ int cldl_create(cldl_t** out, uint64_t n, const uint64_t* colptr, const uint64_t
 
 void cldl_destroy(cldl_t* h) {
   if (!h) return;
-  h->obj.release();
   delete h;
 }
 
@@ -2057,8 +2036,7 @@ int cldl_selected_inverse(cldl_t* h, double* nzval_out) {
   if (!h || !nzval_out) return CLDL_E_ARG;
   LDLObject& o = h->obj;
   if (!o.sharded() && !o.schur && o.factor_ok && !o.d_si_out) {
-    if (cudaSetDevice(o.device) != cudaSuccess ||
-        cudaMalloc((void**)&o.d_si_out, (size_t)(o.nnzA ? o.nnzA : 1) * sizeof(double)) != cudaSuccess)
+    if (cudaSetDevice(o.device) != cudaSuccess || o.own.alloc(&o.d_si_out, (size_t)o.nnzA) != cudaSuccess)
       return CLDL_E_CUDA;
   }
   int rc = o.selected_inverse_async(o.d_si_out);
@@ -2085,10 +2063,7 @@ int cldl_adjoint_solve(cldl_t* h, const double* g, const double* x, double* gb, 
   if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
   if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
   const size_t n = (size_t)o.n, nnz = (size_t)o.nnzA;
-  if (!o.d_adj_buf && cudaMalloc((void**)&o.d_adj_buf, (3 * n + (nnz ? nnz : 1)) * sizeof(double)) != cudaSuccess) {
-    o.d_adj_buf = nullptr;
-    return CLDL_E_CUDA;
-  }
+  if (!o.d_adj_buf && o.own.alloc(&o.d_adj_buf, 3 * n + (nnz ? nnz : 1)) != cudaSuccess) return CLDL_E_CUDA;
   double *dg = o.d_adj_buf, *dx = dg + n, *dgb = dx + n, *dv = dgb + n;
   if (cudaMemcpyAsync(dg, g, n * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess ||
       (gvals && cudaMemcpyAsync(dx, x, n * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess))
@@ -2143,7 +2118,6 @@ int cldl_create_schur(cldl_t** out, uint64_t n, const uint64_t* colptr, const ui
   h->obj.schur_set = std::move(sidx);
   int rc = h->obj.init((int)n, Ap.data(), Ai.data(), nzval, dsigns, o, perm_or_null ? perm.data() : nullptr);
   if (rc != CLDL_OK) {
-    h->obj.release();
     delete h;
     return rc;
   }

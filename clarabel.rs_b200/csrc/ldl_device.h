@@ -11,6 +11,7 @@
 #include "symbolic.h"
 #include "ldl_plan.h"
 #include "ldl_solve_plan.h"
+#include "vec.cuh"
 
 #define CB_MAX_PANEL 128
 #define CB_PB_LD 66        /* padded leading dimension of the pivot block in shared memory */
@@ -86,6 +87,8 @@ struct SIPlan {
 
 class LDLObject {
  public:
+  DevOwner own;                     // every stream, event and buffer below
+  ~LDLObject() { release(); }
   // triangular solves (ldl_solve.cuh): task queue, counters, level-0 leaf lists
   SVPlan sv;
   int *d_sv_init = nullptr, *d_sv_cnt = nullptr, *d_sv_leaf1 = nullptr, *d_sv_leafn = nullptr, *d_sv_leafw = nullptr;
@@ -208,7 +211,7 @@ class LDLObject {
   // a Schur complement handle sets schur_set (caller indices, in output order) before init
   int init(int n, const int64_t* Ap, const int32_t* Ai, const double* Ax, const int8_t* dsigns,
            const cldl_opts& o, const int* perm_in);
-  void release();
+  void release();        // what is not the owner's: the NCCL communicator (the emulated build: its dense factor)
   int refactor_level0();   // the start of every refactor: counters reset, tree level 0 factored
   int refactor_async();
   int sync_status();

@@ -99,25 +99,23 @@ __global__ void k_sparse_soc_fill(ConeDev c, double* __restrict__ vals, const in
 }
 
 // ------------------------------------------------------------- host helpers
-static void dfree(const void* p) { if (p) cudaFree((void*)p); }
-
 // scalar slots shared between device reductions and the host
 enum Slot { S_NORMB = 0, S_NORME, S_MAXDIAG, S_QX, S_BZ, S_SZ, S_XPX, S_ALPHA, S_MARG0, S_MARG1,
             S_D0, S_D1, S_D2, S_D3, S_D4, S_D5, S_D6, S_D7, S_N0, S_N1, S_N2, S_N3, S_N4, S_N5, S_N6, S_N7,
             S_NORMB2, S_NORME2, S_BARR, S_BP0, S_BP1, S_BP2, S_BP3, S_BP4, S_SZSH, S_DMU, S_COUNT = 40 };
 
 struct Scalars {
+  DevOwner own;
   double* d = nullptr;  // device [S_COUNT]
   double* h = nullptr;  // pinned host mirror
   cudaStream_t st = nullptr;
   int init(cudaStream_t s) {
     st = s;
-    SCK(cudaMalloc((void**)&d, S_COUNT * sizeof(double)));
+    SCK(own.alloc(&d, S_COUNT));
     SCK(cudaMemset(d, 0, S_COUNT * sizeof(double)));
-    SCK(cudaMallocHost((void**)&h, S_COUNT * sizeof(double)));
+    SCK(own.alloc_host(&h, S_COUNT));
     return 0;
   }
-  void release() { if (d) cudaFree(d); if (h) cudaFreeHost(h); }
   int fetch() {
     SCK(cudaMemcpyAsync(h, d, S_COUNT * sizeof(double), cudaMemcpyDeviceToHost, st));
     SCK(cudaStreamSynchronize(st));
@@ -176,6 +174,7 @@ struct Vec {
 // the device half of a KKT assembly (the host copies stay for tests / get_kkt)
 class KKTDevice : public KKTAssembly {
  public:
+  DevOwner own;       // the buffers below (the LDL object owns its own)
   int n = 0, m = 0, p = 0;
   cipm_settings set{};
   ConeSet* cones = nullptr;
@@ -199,7 +198,6 @@ class KKTDevice : public KKTAssembly {
   int set_PA_values(const HostCsc& P, const HostCsc& A);
   int init(const HostCsc& P, const HostCsc& A, ConeSet* cs, const cipm_settings& s, const cldl_opts& lo,
            const int* perm, cudaStream_t stream_unused, Scalars* scal);
-  void release();
   int update();                                      // -> 1 ok / 0 failed / <0 error
   void setrhs(const double* rx, const double* rz);
   void setrhs2(const double* rx, const double* rz);  // right-hand side of the second system of solve2
@@ -243,8 +241,8 @@ int KKTDevice::init(const HostCsc& P, const HostCsc& A, ConeSet* cs, const cipm_
     if (cudaSetDevice(devid) != cudaSuccess) return CLDL_E_CUDA;
     const CsrMap S = triu_to_sym_csr(N, Kp.data(), Ki.data());
     nnzS = S.rowptr[N];
-    SCK(upload(&d_srow, S.rowptr)); SCK(upload(&d_scol, S.col)); SCK(upload(&d_sidx, S.src));
-    SCK(cudaMalloc((void**)&d_sval, (size_t)(nnzS ? nnzS : 1) * 8));
+    SCK(own.upload(&d_srow, S.rowptr)); SCK(own.upload(&d_scol, S.col)); SCK(own.upload(&d_sidx, S.src));
+    SCK(own.alloc(&d_sval, (size_t)nnzS));
     return 0;
   };
   std::thread th_csr([&]() { rc_csr = build_sym_csr(); });
@@ -257,15 +255,15 @@ int KKTDevice::init(const HostCsc& P, const HostCsc& A, ConeSet* cs, const cipm_
   th_csr.join();
   if (rc_csr) return rc_csr;
   std::vector<signed char> ds8(dsigns.begin(), dsigns.end());
-  SCK(upload(&d_map_P, map_P)); SCK(upload(&d_map_A, map_A)); SCK(upload(&d_map_Hs, map_Hs));
-  SCK(upload(&d_map_u, map_u)); SCK(upload(&d_map_v, map_v)); SCK(upload(&d_map_D, map_D));
-  SCK(upload(&d_map_diag, map_diag)); SCK(upload(&d_dsigns, ds8));
-  SCK(upload(&d_map_gqr, map_gqr)); SCK(upload(&d_map_gp, map_gp)); SCK(upload(&d_map_gD, map_gD));
-  SCK(cudaMalloc((void**)&d_Hs, (size_t)(cones->nHs ? cones->nHs : 1) * 8));
-  SCK(cudaMalloc((void**)&d_x, (size_t)N * 8)); SCK(cudaMalloc((void**)&d_b, (size_t)N * 8));
-  SCK(cudaMalloc((void**)&d_w1, (size_t)N * 8)); SCK(cudaMalloc((void**)&d_w2, (size_t)N * 8));
-  SCK(cudaMalloc((void**)&d_x2, (size_t)N * 8)); SCK(cudaMalloc((void**)&d_b2, (size_t)N * 8));
-  SCK(cudaMalloc((void**)&d_w1b, (size_t)N * 8)); SCK(cudaMalloc((void**)&d_w2b, (size_t)N * 8));
+  SCK(own.upload(&d_map_P, map_P)); SCK(own.upload(&d_map_A, map_A)); SCK(own.upload(&d_map_Hs, map_Hs));
+  SCK(own.upload(&d_map_u, map_u)); SCK(own.upload(&d_map_v, map_v)); SCK(own.upload(&d_map_D, map_D));
+  SCK(own.upload(&d_map_diag, map_diag)); SCK(own.upload(&d_dsigns, ds8));
+  SCK(own.upload(&d_map_gqr, map_gqr)); SCK(own.upload(&d_map_gp, map_gp)); SCK(own.upload(&d_map_gD, map_gD));
+  SCK(own.alloc(&d_Hs, (size_t)cones->nHs));
+  SCK(own.alloc(&d_x, (size_t)N)); SCK(own.alloc(&d_b, (size_t)N));
+  SCK(own.alloc(&d_w1, (size_t)N)); SCK(own.alloc(&d_w2, (size_t)N));
+  SCK(own.alloc(&d_x2, (size_t)N)); SCK(own.alloc(&d_b2, (size_t)N));
+  SCK(own.alloc(&d_w1b, (size_t)N)); SCK(own.alloc(&d_w2b, (size_t)N));
   SCK(cudaMemset(d_x, 0, (size_t)N * 8)); SCK(cudaMemset(d_b, 0, (size_t)N * 8));
   return 0;
 }
@@ -276,14 +274,6 @@ int KKTDevice::set_PA_values(const HostCsc& P, const HostCsc& A) {
   SCK(cudaMemcpyAsync(ldl.dev.vals, Kx.data(), (size_t)nnzK * 8, cudaMemcpyHostToDevice, st));
   SCK(cudaStreamSynchronize(st));
   return 0;
-}
-
-void KKTDevice::release() {
-  dfree(d_map_P); dfree(d_map_A); dfree(d_map_Hs); dfree(d_map_u); dfree(d_map_v); dfree(d_map_D); dfree(d_map_gqr); dfree(d_map_gp); dfree(d_map_gD);
-  dfree(d_map_diag); dfree(d_dsigns); dfree(d_srow); dfree(d_scol); dfree(d_sidx); dfree(d_sval);
-  dfree(d_Hs); dfree(d_x); dfree(d_b); dfree(d_w1); dfree(d_w2);
-  dfree(d_x2); dfree(d_b2); dfree(d_w1b); dfree(d_w2b);
-  ldl.release();
 }
 
 void KKTDevice::update_vals(const int* d_map, const double* d_src, int len) {
@@ -524,6 +514,7 @@ enum { IST_UNSOLVED = 0, IST_SOLVED, IST_PINF, IST_DINF, IST_ALMOST_SOLVED, IST_
 
 class IPM {
  public:
+  DevOwner own;       // the buffers, events and temporary stream below (cones, kkt and sc own theirs)
   int n = 0, m = 0;
   int mfull = 0;                 // rows of the caller's problem (m = rows left after the inf-bound presolve)
   double setup_time = 0.0;       // seconds spent in cipm_create: the reference's time limit runs on setup + solve
@@ -573,7 +564,6 @@ class IPM {
            const int32_t* ctype, const uint64_t* cdim, const cipm_settings& s, const cldl_opts& lo,
            const uint64_t* perm, const double* cparam = nullptr, const uint64_t* gp_dim2 = nullptr,
            const double* gp_alpha = nullptr);
-  void release();
   int upload_problem();
   int solve();
   // pieces
@@ -619,16 +609,16 @@ class IPM {
 int IPM::upload_problem() {
   // A as CSR (A x) and A' as CSR (== A in CSC) ; P as full symmetric CSR
   hAcsr = csc_to_csr(A);
-  SCK(upload(&dAr, hAcsr.rowptr)); SCK(upload(&dAc, hAcsr.col)); SCK(upload(&dAv, gather(A.nzval, hAcsr.src)));
+  SCK(own.upload(&dAr, hAcsr.rowptr)); SCK(own.upload(&dAc, hAcsr.col)); SCK(own.upload(&dAv, gather(A.nzval, hAcsr.src)));
   Acsr.nrows = m; Acsr.rowptr = dAr; Acsr.col = dAc; Acsr.val = dAv;
   std::vector<int> cp32(A.colptr.begin(), A.colptr.end());
-  SCK(upload(&dAtr, cp32)); SCK(upload(&dAtc, A.rowval)); SCK(upload(&dAtv, A.nzval));
+  SCK(own.upload(&dAtr, cp32)); SCK(own.upload(&dAtc, A.rowval)); SCK(own.upload(&dAtv, A.nzval));
   Atcsr.nrows = n; Atcsr.rowptr = dAtr; Atcsr.col = dAtc; Atcsr.val = dAtv;
   hPsym = triu_to_sym_csr(n, P.colptr.data(), P.rowval.data());
-  SCK(upload(&dPr, hPsym.rowptr)); SCK(upload(&dPc, hPsym.col)); SCK(upload(&dPv, gather(P.nzval, hPsym.src)));
+  SCK(own.upload(&dPr, hPsym.rowptr)); SCK(own.upload(&dPc, hPsym.col)); SCK(own.upload(&dPv, gather(P.nzval, hPsym.src)));
   Psym.nrows = n; Psym.rowptr = dPr; Psym.col = dPc; Psym.val = dPv;
-  SCK(upload(&dq, q)); SCK(upload(&db, b)); SCK(upload(&dd, eq.d)); SCK(upload(&ddinv, eq.dinv));
-  SCK(upload(&de, eq.e)); SCK(upload(&deinv, eq.einv));
+  SCK(own.upload(&dq, q)); SCK(own.upload(&db, b)); SCK(own.upload(&dd, eq.d)); SCK(own.upload(&ddinv, eq.dinv));
+  SCK(own.upload(&de, eq.e)); SCK(own.upload(&deinv, eq.einv));
   return 0;
 }
 
@@ -700,7 +690,7 @@ int IPM::init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const doub
   normq = 0; for (double v : q) normq = std::max(normq, std::fabs(v));
   normb = 0; for (double v : b) normb = std::max(normb, std::fabs(v));
   // cone set needs a stream: borrow the LDL's once it exists -> create ours first
-  SCK(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  SCK(own.stream(&st, cudaStreamNonBlocking));
   cb_tmark(nullptr);
   if ((rc = cones.init(layout, st))) return rc;
   cb_tmark("ipm: cone set init");
@@ -721,16 +711,16 @@ int IPM::init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const doub
     struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } th_guard{th};
     rc = kkt.init(P, A, &cones, set, lo, perm ? kperm.data() : nullptr, st, &sc);
     th.join();
-    if (rc || rc_up) { cudaStreamDestroy(st); st = nullptr; return rc ? rc : rc_up; }      // the temporary stream does not leak on the error paths
-    if ((rc = kkt.set_PA_values(P, A))) { cudaStreamDestroy(st); st = nullptr; return rc; }
+    if (rc || rc_up) return rc ? rc : rc_up;
+    if ((rc = kkt.set_PA_values(P, A))) return rc;
   }
   cb_tmark("ipm: equilibrate + upload problem || kkt init");
   // single stream for everything: adopt the LDL object's stream
-  cudaStreamDestroy(st);
+  own.free(st);
   st = kkt.st;
   cones.stream = st; sc.st = st; V.st = st; V.ws = cones.ws;
   cb_tmark("ipm: kkt init total");
-  auto al = [&](double** pp, int len) { return cudaMalloc((void**)pp, (size_t)(len ? len : 1) * 8) == cudaSuccess && cudaMemset(*pp, 0, (size_t)(len ? len : 1) * 8) == cudaSuccess; };
+  auto al = [&](double** pp, int len) { return own.alloc(pp, (size_t)len) == cudaSuccess && cudaMemset(*pp, 0, (size_t)(len ? len : 1) * 8) == cudaSuccess; };
   bool ok = al(&x, n) && al(&s, m) && al(&z, m) && al(&lx, n) && al(&ls, m) && al(&lz, m) && al(&rhx, n) &&
             al(&rhs_, m) && al(&rhz, m) && al(&px, n) && al(&ps, m) && al(&pz, m) && al(&rx, n) && al(&rz, m) &&
             al(&rx_inf, n) && al(&rz_inf, m) && al(&Px, n) && al(&x1, n) && al(&z1, m) && al(&x2, n) && al(&z2, m) &&
@@ -752,26 +742,6 @@ int IPM::init(int n_, int m_, const uint64_t* Pp, const uint64_t* Pi, const doub
   if (cudaGetDeviceProperties(&prop, lo.device) == cudaSuccess) psetup.device = prop.name;
 #endif
   return 0;
-}
-
-void IPM::release() {
-  for (const void* p_ : {(const void*)dPr, (const void*)dPc, (const void*)dAr, (const void*)dAc, (const void*)dAtr,
-                         (const void*)dAtc, (const void*)dPv, (const void*)dAv, (const void*)dAtv, (const void*)dq,
-                         (const void*)db, (const void*)dd, (const void*)ddinv, (const void*)de, (const void*)deinv,
-                         (const void*)x, (const void*)s, (const void*)z, (const void*)lx, (const void*)ls,
-                         (const void*)lz, (const void*)rhx, (const void*)rhs_, (const void*)rhz, (const void*)px,
-                         (const void*)ps, (const void*)pz, (const void*)rx, (const void*)rz, (const void*)rx_inf,
-                         (const void*)rz_inf, (const void*)Px, (const void*)x1, (const void*)z1, (const void*)x2,
-                         (const void*)z2, (const void*)workx, (const void*)workz, (const void*)work_conic,
-                         (const void*)tmpn})
-    dfree(p_);
-  for (auto ev : iter_ev) cudaEventDestroy(ev);
-  dfree(dw.map_Psym); dfree(dw.map_Acsr); dfree(dw.Pcp); dfree(dw.Pri); dfree(dw.arena);
-  dfree(d_verdict);
-  if (h_verdict) cudaFreeHost(h_verdict);
-  cones.release();
-  sc.release();
-  kkt.release();
 }
 
 int IPM::residuals_update() {
@@ -1048,7 +1018,7 @@ int IPM::solve() {
   n_iter_ev = 0;
   for (;;) {
     if (n_iter_ev < 1024) {
-      if ((int)iter_ev.size() <= n_iter_ev) { cudaEvent_t ev; SCK(cudaEventCreate(&ev)); iter_ev.push_back(ev); }
+      if ((int)iter_ev.size() <= n_iter_ev) { cudaEvent_t ev; SCK(own.event(&ev)); iter_ev.push_back(ev); }
       SCK(cudaEventRecord(iter_ev[n_iter_ev++], st));
     }
     if ((rc = residuals_update())) return rc;
@@ -1154,15 +1124,13 @@ int IPM::solve() {
 // one scratch arena.  A handle that never differentiates allocates none of it.
 int IPM::deriv_prepare() {
   if (dw.arena) return 0;
-  // what an earlier call that failed half way uploaded is freed, not overwritten
-  for (int** p : {&dw.map_Psym, &dw.map_Acsr, &dw.Pcp, &dw.Pri}) { dfree(*p); *p = nullptr; }
   std::vector<int> pcp(P.colptr.begin(), P.colptr.end());
-  SCK(upload(&dw.map_Psym, hPsym.src)); SCK(upload(&dw.map_Acsr, hAcsr.src));
-  SCK(upload(&dw.Pcp, pcp)); SCK(upload(&dw.Pri, P.rowval));
+  SCK(own.upload(&dw.map_Psym, hPsym.src)); SCK(own.upload(&dw.map_Acsr, hAcsr.src));
+  SCK(own.upload(&dw.Pcp, pcp)); SCK(own.upload(&dw.Pri, P.rowval));
   const size_t nnzP = (size_t)P.colptr[n], nnzA = (size_t)A.colptr[n], nnzPs = hPsym.src.size();
   const size_t total = 8 * (size_t)n + 10 * (size_t)m + nnzP + nnzPs + 2 * nnzA;
   double* a = nullptr;
-  SCK(cudaMalloc((void**)&a, total * 8));
+  SCK(own.alloc(&a, total));
   dw.arena = a;
   for (double** p : {&dw.xo, &dw.vn0, &dw.vn1, &dw.vn2, &dw.rn, &dw.an, &dw.on0, &dw.on1}) { *p = a; a += n; }
   for (double** p : {&dw.zo, &dw.sn, &dw.zn, &dw.vm0, &dw.vm1, &dw.vm2, &dw.rm, &dw.bm, &dw.om0, &dw.om1}) { *p = a; a += m; }
@@ -1179,8 +1147,9 @@ int IPM::deriv_prepare() {
 int IPM::deriv_factor() {
   if (!deriv_valid || !keep.empty()) return CLDL_E_ARG;
   SCK(cudaSetDevice(kkt.ldl.device));
+  const size_t mk = own.mark();
   int rc = deriv_prepare();
-  if (rc) return rc;
+  if (rc) { own.release_since(mk); dw.arena = nullptr; return rc; }
   g_launches++;
   k_deriv_point<<<(std::max(n, m) + 255) / 256, 256, 0, st>>>(n, m, x, s, z, dd, de, 1.0 / tau, 1.0 / eq.c, dw.xo, dw.zo,
                                                               dw.sn, dw.zn);
@@ -1312,8 +1281,10 @@ int IPM::report_pass(bool verbose, bool* stop) {
   if (!L.sharded() || !L.has_transport()) { *stop = mine; return 0; }
   const int R = L.shard_nranks;
   if (!d_verdict) {
-    SCK(cudaMalloc((void**)&d_verdict, (size_t)(1 + R) * sizeof(double)));
-    SCK(cudaMallocHost((void**)&h_verdict, (size_t)(1 + R) * sizeof(double)));
+    const size_t mk = own.mark();
+    if (own.alloc(&d_verdict, (size_t)(1 + R)) || own.alloc_host(&h_verdict, (size_t)(1 + R))) {
+      own.release_since(mk); d_verdict = nullptr; return CLDL_E_CUDA;
+    }
   }
   h_verdict[0] = mine ? 1.0 : 0.0;
   SCK(cudaMemcpyAsync(d_verdict, h_verdict, sizeof(double), cudaMemcpyHostToDevice, st));
@@ -1393,7 +1364,7 @@ int cipm_create_gp(cipm_t** out, uint64_t n, uint64_t m, const uint64_t* P_colpt
   const double t_create0 = cb::wall();
   int rc = h->ipm.init((int)n, (int)m, P_colptr, P_rowval, P_nzval, q, A_colptr, A_rowval, A_nzval, b, ncones,
                        cone_types, cone_dims, s, lo, kkt_perm_or_null, cone_params, genpow_dim2, genpow_alpha);
-  if (rc) { h->ipm.release(); delete h; return rc; }
+  if (rc) { delete h; return rc; }
   h->ipm.setup_time = cb::wall() - t_create0;
   *out = h;
   return CLDL_OK;
@@ -1427,7 +1398,6 @@ int cipm_set_transport(cipm_t* h, cldl_allgather_fn fn, void* ctx) {
 
 void cipm_destroy(cipm_t* h) {
   if (!h) return;
-  h->ipm.release();
   delete h;
 }
 
@@ -1599,15 +1569,15 @@ int cipm_test_spmv(cipm_t* h, int which, double* y, const double* x, double a, d
   IPM& I = h->ipm;
   if (cudaSetDevice(I.kkt.ldl.device) != cudaSuccess) return CLDL_E_CUDA;
   const int ny = which == 1 ? I.m : I.n, nx = which == 1 ? I.n : (which == 2 ? I.m : I.n);
+  cb::DevOwner own;
   double *dy = nullptr, *dx = nullptr;
-  if (cudaMalloc((void**)&dy, (size_t)(ny ? ny : 1) * 8) != cudaSuccess || cudaMalloc((void**)&dx, (size_t)(nx ? nx : 1) * 8) != cudaSuccess) return CLDL_E_CUDA;
+  if (own.alloc(&dy, (size_t)ny) != cudaSuccess || own.alloc(&dx, (size_t)nx) != cudaSuccess) return CLDL_E_CUDA;
   int rc = (h2d(dy, y, ny) || h2d(dx, x, nx)) ? CLDL_E_CUDA : CLDL_OK;
   if (!rc) {
     I.spmv(which == 0 ? I.Psym : (which == 1 ? I.Acsr : I.Atcsr), dy, dx, a, b);
     cudaStreamSynchronize(I.st);
     rc = d2h(y, dy, ny) ? CLDL_E_CUDA : CLDL_OK;
   }
-  cudaFree(dy); cudaFree(dx);
   return rc;
 }
 // what: 0  ||x||_2, 1  ||x||_inf (NaN propagates), 2  ||x .* v||_2, 3  <x, v>
@@ -1615,9 +1585,9 @@ int cipm_test_vec(cipm_t* h, int what, const double* x, const double* v, uint64_
   if (!h || !out || what < 0 || what > 3) return CLDL_E_ARG;
   IPM& I = h->ipm;
   if (cudaSetDevice(I.kkt.ldl.device) != cudaSuccess) return CLDL_E_CUDA;
+  cb::DevOwner own;
   double *dx = nullptr, *dv = nullptr, *dout = nullptr;
-  const size_t nb = (size_t)(n ? n : 1) * 8;
-  if (cudaMalloc((void**)&dx, nb) != cudaSuccess || cudaMalloc((void**)&dv, nb) != cudaSuccess || cudaMalloc((void**)&dout, 8) != cudaSuccess) return CLDL_E_CUDA;
+  if (own.alloc(&dx, n) != cudaSuccess || own.alloc(&dv, n) != cudaSuccess || own.alloc(&dout, 1) != cudaSuccess) return CLDL_E_CUDA;
   int rc = (h2d(dx, x, n) || h2d(dv, v ? v : x, n)) ? CLDL_E_CUDA : CLDL_OK;
   if (!rc) {
     if (what == 0) I.V.norm(dx, (int)n, dout);
@@ -1627,7 +1597,6 @@ int cipm_test_vec(cipm_t* h, int what, const double* x, const double* v, uint64_
     cudaStreamSynchronize(I.st);
     rc = d2h(out, dout, 1) ? CLDL_E_CUDA : CLDL_OK;
   }
-  cudaFree(dx); cudaFree(dv); cudaFree(dout);
   return rc;
 }
 int cipm_update_data(cipm_t* h, const double* P_nzval, const double* q, const double* A_nzval, const double* b) {
@@ -1652,11 +1621,11 @@ int ckkt_update_P(cipm_t* h, const double* P_nzval_scaled) {
   if (cudaSetDevice(I.kkt.ldl.device) != cudaSuccess) return CLDL_E_CUDA;
   I.deriv_valid = false;     // K no longer holds the data of the last solve
   const size_t len = I.kkt.map_P.size();
+  cb::DevOwner own;
   double* tmp = nullptr;
-  if (cudaMalloc((void**)&tmp, (len ? len : 1) * 8) != cudaSuccess) return CLDL_E_CUDA;
+  if (own.alloc(&tmp, len) != cudaSuccess) return CLDL_E_CUDA;
   int rc = h2d(tmp, P_nzval_scaled, len);
   if (!rc) { I.kkt.update_vals(I.kkt.d_map_P, tmp, (int)len); cudaStreamSynchronize(I.st); }
-  cudaFree(tmp);
   return rc;
 }
 int ckkt_update_A(cipm_t* h, const double* A_nzval_scaled) {
@@ -1665,11 +1634,11 @@ int ckkt_update_A(cipm_t* h, const double* A_nzval_scaled) {
   if (cudaSetDevice(I.kkt.ldl.device) != cudaSuccess) return CLDL_E_CUDA;
   I.deriv_valid = false;     // K no longer holds the data of the last solve
   const size_t len = I.kkt.map_A.size();
+  cb::DevOwner own;
   double* tmp = nullptr;
-  if (cudaMalloc((void**)&tmp, (len ? len : 1) * 8) != cudaSuccess) return CLDL_E_CUDA;
+  if (own.alloc(&tmp, len) != cudaSuccess) return CLDL_E_CUDA;
   int rc = h2d(tmp, A_nzval_scaled, len);
   if (!rc) { I.kkt.update_vals(I.kkt.d_map_A, tmp, (int)len); cudaStreamSynchronize(I.st); }
-  cudaFree(tmp);
   return rc;
 }
 int ckkt_get_values(cipm_t* h, double* nzval_out) {

@@ -16,6 +16,7 @@
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <mutex>
 #include <vector>
 
 namespace cb {
@@ -218,15 +219,78 @@ inline int red_grid(int n) {
   return g < 1 ? 1 : (g > RED_BLOCKS ? RED_BLOCKS : g);
 }
 
-// a device copy of v in *dst, at least one element long so that an empty vector still gets a pointer the kernels may
-// be passed; *dst is set as soon as the allocation succeeds, so that a failed copy leaves nothing unowned
-template <class D, class T>
-inline cudaError_t upload(D** dst, const std::vector<T>& v) {
-  T* p = nullptr;
-  cudaError_t e = cudaMalloc((void**)&p, (v.size() ? v.size() : 1) * sizeof(T));
-  if (e != cudaSuccess) return e;
-  *dst = reinterpret_cast<D*>(p);
-  return v.empty() ? cudaSuccess : cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
-}
+// Every CUDA resource one host object creates, released together: device memory, then pinned host memory, then
+// events, then streams.  A pointer is set only once the resource is recorded, so a failure leaves nothing unowned.
+// Lazy set-up takes a mark(), and on any failure calls release_since(mark) and clears the pointer the next call
+// tests, so that a retry starts clean.  The mutex guards the record only, not the CUDA call: init's helper thread
+// allocates gigabytes beside the main thread's uploads.
+class DevOwner {
+ public:
+  DevOwner() = default;
+  DevOwner(const DevOwner&) = delete;
+  DevOwner& operator=(const DevOwner&) = delete;
+  ~DevOwner() { release(); }
+
+  // device memory of at least one element, so that an empty vector still gets a pointer the kernels may be passed
+  template <class T> cudaError_t alloc(T** p, size_t n) {
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, (n ? n : 1) * sizeof(T));
+    if (e == cudaSuccess) { add(MEM, q); *p = (T*)q; }
+    return e;
+  }
+  template <class D, class T> cudaError_t upload(D** dst, const std::vector<T>& v) {
+    T* p = nullptr;
+    const cudaError_t e = alloc(&p, v.size());
+    if (e != cudaSuccess) return e;
+    *dst = reinterpret_cast<D*>(p);
+    return v.empty() ? cudaSuccess : cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
+  }
+  template <class T> cudaError_t alloc_host(T** p, size_t n) {
+    void* q = nullptr;
+    const cudaError_t e = cudaMallocHost(&q, (n ? n : 1) * sizeof(T));
+    if (e == cudaSuccess) { add(HOST, q); *p = (T*)q; }
+    return e;
+  }
+  cudaError_t stream(cudaStream_t* s, unsigned flags) {
+    const cudaError_t e = cudaStreamCreateWithFlags(s, flags);
+    if (e == cudaSuccess) add(STREAM, (const void*)*s);
+    return e;
+  }
+  cudaError_t event(cudaEvent_t* ev, unsigned flags = 0) {     // 0: cudaEventDefault, a timing event
+    const cudaError_t e = cudaEventCreateWithFlags(ev, flags);
+    if (e == cudaSuccess) add(EVENT, (const void*)*ev);
+    return e;
+  }
+  // releases one recorded resource now (buffers that grow, a temporary stream)
+  void free(const void* p) {
+    std::lock_guard<std::mutex> lk(mu);
+    for (size_t i = 0; i < recs.size(); i++)
+      if (recs[i].p == p) { destroy(recs[i]); recs.erase(recs.begin() + (long)i); return; }
+  }
+  size_t mark() { std::lock_guard<std::mutex> lk(mu); return next; }
+  void release_since(size_t m) {    // everything created since mark() returned m
+    std::lock_guard<std::mutex> lk(mu);
+    for (int k = MEM; k <= STREAM; k++)
+      for (const Rec& r : recs) if (r.kind == k && r.seq >= m) destroy(r);
+    size_t j = 0;
+    for (const Rec& r : recs) if (r.seq < m) recs[j++] = r;
+    recs.resize(j);
+  }
+  void release() { release_since(0); }
+
+ private:
+  enum { MEM = 0, HOST, EVENT, STREAM };
+  struct Rec { int kind; const void* p; size_t seq; };
+  std::mutex mu;
+  std::vector<Rec> recs;
+  size_t next = 0;
+  void add(int kind, const void* p) { std::lock_guard<std::mutex> lk(mu); recs.push_back({kind, p, next++}); }
+  static void destroy(const Rec& r) {
+    if (r.kind == MEM) cudaFree((void*)r.p);
+    else if (r.kind == HOST) cudaFreeHost((void*)r.p);
+    else if (r.kind == EVENT) cudaEventDestroy((cudaEvent_t)r.p);
+    else cudaStreamDestroy((cudaStream_t)r.p);
+  }
+};
 
 }  // namespace cb

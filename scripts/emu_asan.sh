@@ -8,7 +8,7 @@ mkdir -p /tmp/cb_asan
 g++ -O1 -g -fsanitize=address,alignment -fno-sanitize-recover=alignment -fno-omit-frame-pointer -march=x86-64-v3 -ffp-contract=fast -std=c++17 -fPIC -shared -pthread \
   -Wno-unknown-pragmas -Itests/emu/include -Itests/emu/gen -Iinclude -Iclarabel.rs_b200/csrc -o /tmp/cb_asan/libclarabel_emu_asan.so \
   tests/emu/gen/cones.cpp tests/emu/gen/cones_psd.cpp tests/emu/gen/cones_nonsym.cpp tests/emu/gen/solver.cpp tests/emu/gen/ldl.cpp \
-  tests/emu/cuda_emu.cpp clarabel.rs_b200/csrc/ordering.cpp clarabel.rs_b200/csrc/symbolic.cpp clarabel.rs_b200/csrc/symbolic_api.cpp
+  tests/emu/cuda_emu.cpp clarabel.rs_b200/csrc/*.cpp
 cat > /tmp/cb_asan/run.py <<'PY'
 import sys, os, numpy as np
 os.environ["CLARABEL_EMU"] = "1"

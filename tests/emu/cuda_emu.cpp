@@ -8,6 +8,7 @@
 #include "cuda_emu.h"
 
 #include <sys/mman.h>
+#include <atomic>
 #include <cstring>
 #include <mutex>
 #include <utility>
@@ -221,7 +222,34 @@ static int poison_mode() {
   if (v < 0) { const char* e = std::getenv("EMU_POISON"); v = (e && !std::atoi(e)) ? 0 : 1; }
   return v;
 }
+// live resources by kind, and the countdown to the creation that is made to fail (0: none)
+static std::atomic<int64_t> g_live[4];
+static std::atomic<int> g_fail_in{0};
+static bool fail_now() {
+  int k = g_fail_in.load();
+  while (k > 0 && !g_fail_in.compare_exchange_weak(k, k - 1)) {}
+  return k == 1;
+}
+void* res_create(int kind, size_t n) {
+  if (fail_now()) return nullptr;
+  void* p = std::calloc(1, n ? n : 1);
+  if (p) g_live[kind]++;
+  return p;
+}
+void res_destroy(int kind, void* p) {
+  if (!p) return;
+  g_live[kind]--;
+  std::free(p);
+}
+
+static void* dev_alloc_raw(size_t n);
 void* dev_alloc(size_t n) {
+  if (fail_now()) return nullptr;
+  void* p = dev_alloc_raw(n);
+  if (p) g_live[RES_DEV]++;
+  return p;
+}
+static void* dev_alloc_raw(size_t n) {
   if (!guard_mode()) {
     void* p = std::malloc(n ? n : 1);
     if (p) std::memset(p, poison_mode() ? 0xCB : 0, n ? n : 1);
@@ -245,6 +273,8 @@ void* dev_alloc(size_t n) {
   return p;
 }
 void dev_free(void* p) {
+  if (!p) return;
+  g_live[RES_DEV]--;
   if (guard_mode() && g_arena && (char*)p >= g_arena && (char*)p < g_arena + g_cap) return;   // never reused
   std::free(p);
 }
@@ -325,3 +355,9 @@ void run_grid(dim3 grid, dim3 block, size_t smem, const std::function<void()>& b
 }
 
 }  // namespace emu
+
+extern "C" void emu_live_resources(int64_t out[4]) {
+  for (int k = 0; k < 4; k++) out[k] = emu::g_live[k].load();
+}
+// the k-th creation of a resource from now (device or pinned memory, stream, event) fails; 0 disarms
+extern "C" void emu_fail_alloc_at(int k) { emu::g_fail_in.store(k > 0 ? k : 0); }

@@ -156,29 +156,33 @@ inline cudaError_t cudaSetDevice(int) { return 0; }
 // EMU_GUARD=1: device memory comes from an arena the host may only touch inside copies, memsets and kernel launches
 // (cuda_emu.cpp); a host-side dereference of a device pointer -- invisible otherwise, device memory being host memory
 // here -- ends the process with SIGSEGV.
+// Every resource is counted by kind (emu_live_resources), and any creation can be made to fail (emu_fail_alloc_at).
 namespace emu {
+enum { RES_DEV = 0, RES_HOST, RES_STREAM, RES_EVENT };
 void* dev_alloc(size_t n);
 void dev_free(void* p);
+void* res_create(int kind, size_t n);     // pinned host memory, a stream or an event
+void res_destroy(int kind, void* p);
 void dev_open();
 void dev_close();
 struct DevScope { DevScope() { dev_open(); } ~DevScope() { dev_close(); } };
 }
 inline cudaError_t cudaMalloc(void** p, size_t n) { *p = emu::dev_alloc(n); return *p ? 0 : 2; }
 inline cudaError_t cudaFree(void* p) { emu::dev_free(p); return 0; }
-inline cudaError_t cudaMallocHost(void** p, size_t n) { *p = std::calloc(1, n ? n : 1); return *p ? 0 : 2; }
-inline cudaError_t cudaFreeHost(void* p) { std::free(p); return 0; }
+inline cudaError_t cudaMallocHost(void** p, size_t n) { *p = emu::res_create(emu::RES_HOST, n); return *p ? 0 : 2; }
+inline cudaError_t cudaFreeHost(void* p) { emu::res_destroy(emu::RES_HOST, p); return 0; }
 inline cudaError_t cudaMemcpy(void* d, const void* s, size_t n, int) { emu::DevScope o; if (n) std::memmove(d, s, n); return 0; }
 inline cudaError_t cudaMemcpyAsync(void* d, const void* s, size_t n, int, cudaStream_t = nullptr) { emu::DevScope o; if (n) std::memmove(d, s, n); return 0; }
 inline cudaError_t cudaMemset(void* d, int v, size_t n) { emu::DevScope o; if (n) std::memset(d, v, n); return 0; }
 inline cudaError_t cudaMemsetAsync(void* d, int v, size_t n, cudaStream_t = nullptr) { emu::DevScope o; if (n) std::memset(d, v, n); return 0; }
-inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = std::malloc(1); return 0; }
-inline cudaError_t cudaStreamDestroy(cudaStream_t s) { std::free(s); return 0; }
+inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t* s, unsigned) { *s = emu::res_create(emu::RES_STREAM, 1); return *s ? 0 : 2; }
+inline cudaError_t cudaStreamDestroy(cudaStream_t s) { emu::res_destroy(emu::RES_STREAM, s); return 0; }
 inline cudaError_t cudaStreamSynchronize(cudaStream_t) { return 0; }
 inline cudaError_t cudaDeviceSynchronize() { return 0; }
 inline cudaError_t cudaStreamWaitEvent(cudaStream_t, cudaEvent_t, unsigned) { return 0; }
-inline cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = std::malloc(1); return 0; }
-inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned) { *e = std::malloc(1); return 0; }
-inline cudaError_t cudaEventDestroy(cudaEvent_t e) { std::free(e); return 0; }
+inline cudaError_t cudaEventCreate(cudaEvent_t* e) { *e = emu::res_create(emu::RES_EVENT, 1); return *e ? 0 : 2; }
+inline cudaError_t cudaEventCreateWithFlags(cudaEvent_t* e, unsigned) { return cudaEventCreate(e); }
+inline cudaError_t cudaEventDestroy(cudaEvent_t e) { emu::res_destroy(emu::RES_EVENT, e); return 0; }
 inline cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t = nullptr) { return 0; }
 inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return 0; }
 inline cudaError_t cudaEventElapsedTime(float* ms, cudaEvent_t, cudaEvent_t) { *ms = 0.0f; return 0; }

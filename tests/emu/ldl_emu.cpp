@@ -44,10 +44,10 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
   if (rc == -3) return CLDL_E_NOT_TRIU;
   if (rc == -5) return CLDL_E_BAD_PERM;
   if (rc) return CLDL_E_ARG;
-  cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking);
-  cudaEventCreate(&ev0); cudaEventCreate(&ev1);
+  if (own.stream(&stream, cudaStreamNonBlocking) || own.event(&ev0) || own.event(&ev1))
+    return CLDL_E_CUDA;
   nnzA = Ap[n];
-  cudaMalloc((void**)&dev.vals, (size_t)(nnzA ? nnzA : 1) * sizeof(double));
+  if (own.alloc(&dev.vals, (size_t)nnzA)) return CLDL_E_CUDA;
   std::memcpy(dev.vals, Ax, (size_t)nnzA * sizeof(double));
   dev.reg_enable = o.regularize_enable; dev.reg_eps = o.regularize_eps; dev.reg_delta = o.regularize_delta;
   Dense* d = new Dense();
@@ -65,10 +65,6 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
 void LDLObject::release() {
   delete dense_of(this);
   d_bx = nullptr;
-  cudaFree(dev.vals); dev.vals = nullptr;
-  if (stream) cudaStreamDestroy(stream);
-  for (cudaEvent_t* e : {&ev0, &ev1}) if (*e) cudaEventDestroy(*e);
-  stream = nullptr; ev0 = ev1 = nullptr;
 }
 
 static int g_nonfinite = 0, g_zeropiv = 0;

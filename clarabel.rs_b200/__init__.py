@@ -135,6 +135,49 @@ class cldl_info_t(C.Structure):
     ]
 
 
+class cldl_refine_opts(C.Structure):
+    _fields_ = [
+        ("max_iter", C.c_int32),
+        ("tol", C.c_double),
+        ("stop_ratio", C.c_double),
+        ("error_analysis", C.c_int32),
+    ]
+
+
+class cldl_refine_info(C.Structure):
+    _fields_ = [
+        ("steps", C.c_uint32),
+        ("solves", C.c_uint32),
+        ("converged", C.c_int32),
+        ("norm_K_inf", C.c_double),
+        ("norm_x_inf", C.c_double),
+        ("resid_inf", C.c_double),
+        ("scaled_resid", C.c_double),
+        ("omega1", C.c_double),
+        ("omega2", C.c_double),
+        ("cond1", C.c_double),
+        ("cond2", C.c_double),
+        ("ferr", C.c_double),
+    ]
+
+
+@dataclass
+class RefineInfo:
+    """Mirror of cldl_refine_info: the analysis of the x a refined solve returned."""
+    steps: int
+    solves: int
+    converged: bool
+    norm_K_inf: float
+    norm_x_inf: float
+    resid_inf: float
+    scaled_resid: float
+    omega1: float
+    omega2: float
+    cond1: float
+    cond2: float
+    ferr: float
+
+
 # every symbol declared in include/clarabel_b200.h (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [
     "cldl_default_opts", "cldl_create", "cldl_destroy", "cldl_update_values",
@@ -146,6 +189,7 @@ EXPORTED_SYMBOLS = [
     "cldl_create_schur", "cldl_schur_complement", "cldl_schur_complement_dev", "cldl_schur_reduce",
     "cldl_schur_reduce_dev", "cldl_schur_expand", "cldl_schur_expand_dev",
     "cldl_logdet", "cldl_adjoint_solve", "cldl_adjoint_solve_dev",
+    "cldl_default_refine_opts", "cldl_solve_refined", "cldl_solve_refined_dev", "cldl_refine_abi_sizes",
 ]
 
 
@@ -411,6 +455,54 @@ class CudaLDLSolver:
         _check(f(self._h, _p(g, C.c_double), _p(x, C.c_double), _p(gb, C.c_double), _p(gv, C.c_double)),
                "adjoint_solve")
         return gb, sps.csc_matrix((gv, rv.astype(np.int64), cp.astype(np.int64)), shape=(self.n, self.n))
+
+    def _refine_opts(self, max_iter, tol, stop_ratio, error_analysis):
+        o = cldl_refine_opts()
+        o.max_iter, o.tol, o.stop_ratio = int(max_iter), float(tol), float(stop_ratio)
+        o.error_analysis = 1 if error_analysis else 0
+        return o
+
+    @staticmethod
+    def _refine_info(i):
+        return RefineInfo(int(i.steps), int(i.solves), bool(i.converged), i.norm_K_inf, i.norm_x_inf, i.resid_inf,
+                          i.scaled_resid, i.omega1, i.omega2, i.cond1, i.cond2, i.ferr)
+
+    def solve_refined(self, b, *, max_iter=10, tol=float(np.finfo(np.float64).eps), stop_ratio=2.0,
+                      error_analysis=False):
+        """Iteratively refined solve of K x = b: (x, RefineInfo).  K is the matrix of the handle's CURRENT values, with
+        every update_values / scale_values / offset_values / set_values_dev since the last refactor; the corrections
+        use the factor of the last ``refactor()``, so after a value change the factor is only a preconditioner.  x0 is
+        bitwise ``solve(b)``; steps stop at omega1 + omega2 <= tol, after max_iter steps, when a step does not divide
+        omega1 + omega2 by stop_ratio, or at a non-finite omega, and the iterate with the smallest omega1 + omega2 is
+        returned.  omega1 / omega2 are the componentwise backward errors of Arioli, Demmel and Duff; with
+        ``error_analysis`` also cond1, cond2 and ferr = omega1 cond1 + omega2 cond2 from Higham's 1-norm estimator
+        (extra solves; of the factored matrix's inverse).  Convergence is ``info.converged``, not an exception.
+        Synchronises the handle's stream.  BackendError (NotFactored) before a refactor that returned True,
+        (BadArgument) on a Schur or sharded handle and for max_iter < 0, tol < 0 or stop_ratio < 1 (see
+        cldl_solve_refined)."""
+        f = self._L.cldl_solve_refined
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(cldl_refine_opts),
+                      C.POINTER(cldl_refine_info)]
+        f.restype = C.c_int
+        b = _f64(b)
+        assert b.size == self.n
+        x = np.empty_like(b)
+        o, i = self._refine_opts(max_iter, tol, stop_ratio, error_analysis), cldl_refine_info()
+        _check(f(self._h, _p(x, C.c_double), _p(b, C.c_double), C.byref(o), C.byref(i)), "solve_refined")
+        return x, self._refine_info(i)
+
+    def solve_refined_dev(self, d_x_ptr, d_b_ptr, *, max_iter=10, tol=float(np.finfo(np.float64).eps),
+                          stop_ratio=2.0, error_analysis=False):
+        """``solve_refined`` on device buffers (n doubles each, not overlapping): writes x to d_x_ptr and returns the
+        RefineInfo.  Unlike the other _dev calls it SYNCHRONISES the handle's stream (the stopping test reads a few
+        scalars per step on the host); no vector is copied to the host.  The same K and refusals as
+        ``solve_refined``."""
+        f = self._L.cldl_solve_refined_dev
+        f.argtypes = [C.c_void_p] * 3 + [C.POINTER(cldl_refine_opts), C.POINTER(cldl_refine_info)]
+        f.restype = C.c_int
+        o, i = self._refine_opts(max_iter, tol, stop_ratio, error_analysis), cldl_refine_info()
+        _check(f(self._h, C.c_void_p(d_x_ptr), C.c_void_p(d_b_ptr), C.byref(o), C.byref(i)), "solve_refined_dev")
+        return self._refine_info(i)
 
     # --- Schur complement handles (constructed with schur=...) ---
     def _schur_call(self, name, *args):

@@ -21,6 +21,7 @@
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 
+#include <cfloat>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -30,6 +31,7 @@
 
 #include "../../include/clarabel_b200.h"
 #include "ldl_device.h"
+#include "problem_setup.h"
 #include "symbolic.h"
 #include "vec.cuh"
 
@@ -1070,6 +1072,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
 
 #include "ldl_selinv.cuh"
 #include "ldl_schur.cuh"
+#include "ldl_refine.cuh"
 
 __global__ void k_update_values(double* __restrict__ vals, const int* __restrict__ idx,
                                 const double* __restrict__ v, long long len) {
@@ -1452,6 +1455,199 @@ int LDLObject::adjoint_async(const double* d_g, const double* d_x, double* d_gb,
     k_grad_P<<<(unsigned)((n + 7) / 8), 256, 0, stream>>>(n, d_adj_cp, d_adj_rv, d_x, d_gb, d_gvals);   // a warp per column
     CK(cudaGetLastError());
   }
+  return CLDL_OK;
+}
+
+// the mirrored pattern of K (triu_to_sym_csr of the caller's pattern) uploaded, work vectors and scalars allocated: on
+// the first refined solve
+int LDLObject::refine_setup() {
+  const std::vector<int64_t> cp64(h_colptr.begin(), h_colptr.end());
+  const CsrMap M = triu_to_sym_csr(n, cp64.data(), h_rowval.data());
+  CK(own.upload(&d_rf_rowptr, M.rowptr));
+  CK(own.upload(&d_rf_col, M.col));
+  CK(own.upload(&d_rf_src, M.src));
+  CK(own.alloc(&d_rf_work, (size_t)RF_NVEC * (size_t)n));
+  CK(own.alloc(&d_rf_ws, 8 * (size_t)RED_BLOCKS + RF_NS));
+  CK(own.alloc(&d_rf_cnt, 1));
+  CK(cudaMemset(d_rf_cnt, 0, sizeof(unsigned)));     // the reductions' last block leaves it at 0 again
+  CK(own.alloc_host(&h_rf, RF_NS));
+  CK(cudaDeviceSynchronize());      // pageable uploads have landed before `stream` reads them
+  return CLDL_OK;
+}
+
+// omega1, omega2, ||r||_inf, ||x||_inf (and, first, ||K||_inf) at the iterate d_xv into the scalars, then read to
+// h_rf: the work vectors r, kx, rmax hold the residual, |K||x| and the rows' max |K_ij| of that iterate
+int LDLObject::refine_analyse(const double* d_xv, const double* d_b, bool first) {
+  double *r = d_rf_work + (size_t)n, *rsum = d_rf_work + 2 * (size_t)n, *kx = d_rf_work + 3 * (size_t)n,
+         *rmax = d_rf_work + 4 * (size_t)n, *sc = d_rf_ws + 8 * RED_BLOCKS;
+  const ReduceWS ws{d_rf_ws, d_rf_cnt};
+  CK(cudaMemsetAsync(sc + RF_XN, 0, (first ? 2 : 1) * sizeof(double), stream));
+  g_launches += first ? 4 : 3;
+  k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(n, [=] __device__(int i) { return d_xv[i]; }, sc + RF_XN);
+  k_refine_residual<<<(unsigned)((n + RF_NT / 32 - 1) / (RF_NT / 32)), RF_NT, 0, stream>>>(
+      n, d_rf_rowptr, d_rf_col, d_rf_src, dev.vals, d_xv, d_b, r, kx, rmax, first ? rsum : nullptr);
+  if (first) k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(n, [=] __device__(int i) { return rsum[i]; }, sc + RF_KN);
+  k_refine_omega<<<red_grid(n), RED_THREADS, 0, stream>>>(n, r, kx, rmax, d_b, sc + RF_XN, 1000.0 * n * DBL_EPSILON, ws,
+                                                          sc + RF_W1);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(h_rf, sc, (RF_HAS2 + 1) * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));
+  return CLDL_OK;
+}
+
+// Higham's 1-norm estimator (LAPACK dlacn2) for B = diag(g) K^-1 with g = den1 o 1_I1 (which = 1) or den2 o 1_I2
+// (which = 2) at the iterate last analysed: ||B||_1 = || |K^-1| g ||_inf as K is symmetric.  B v = g o K^-1 v and
+// B^T v = K^-1 (g o v), one solve each; a host state machine over device vectors, one scalar read per product.
+int LDLObject::condest(int which, const double* b, double* est, uint32_t* solves) {
+  double *v = d_rf_work, *g = d_rf_work + (size_t)n, *w = d_rf_work + 2 * (size_t)n, *xi = d_rf_work + 5 * (size_t)n;
+  const double *kx = d_rf_work + 3 * (size_t)n, *rmax = d_rf_work + 4 * (size_t)n;
+  double* sc = d_rf_ws + 8 * RED_BLOCKS;
+  const double* xn = sc + RF_XN;
+  const double c = 1000.0 * n * DBL_EPSILON;
+  const ReduceWS ws{d_rf_ws, d_rf_cnt};
+  const int nn = n, grid = (n + 255) / 256;
+  g_launches += 1;
+  k_map<<<grid, 256, 0, stream>>>(nn, [=] __device__(int i) {
+    const RfRow q = rf_row(i, kx, rmax, b, *xn, c);
+    g[i] = which == 1 ? (q.in1 ? q.den1 : 0.0) : (q.in1 ? 0.0 : q.den2);
+  });
+  // v <- B v: w = K^-1 v, v = g o w; then ||v||_1 and the number of signs that differ from xi (which becomes sign(v),
+  // and v with it, when `signs`)
+  auto apply_B = [&](bool signs) -> int {
+    if (int rc = solve_async(w, v)) return rc;
+    (*solves)++;
+    g_launches += signs ? 4 : 2;
+    k_map<<<grid, 256, 0, stream>>>(nn, [=] __device__(int i) { v[i] = g[i] * w[i]; });
+    k_sum<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return fabs(v[i]); }, ws, sc + RF_EST);
+    if (signs) {
+      k_sum<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) {
+        return (v[i] >= 0.0 ? 1.0 : -1.0) != xi[i] ? 1.0 : 0.0; }, ws, sc + RF_CNT);
+      k_map<<<grid, 256, 0, stream>>>(nn, [=] __device__(int i) { xi[i] = v[i] >= 0.0 ? 1.0 : -1.0; v[i] = xi[i]; });
+    }
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(h_rf + RF_EST, sc + RF_EST, 2 * sizeof(double), cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+    return CLDL_OK;
+  };
+  // v <- B^T v: w = g o v, v = K^-1 w; then the first j of max |v_j|, and v[jlast]
+  auto apply_Bt = [&](int jlast) -> int {
+    g_launches += 1;
+    k_map<<<grid, 256, 0, stream>>>(nn, [=] __device__(int i) { w[i] = g[i] * v[i]; });
+    if (int rc = solve_async(v, w)) return rc;
+    (*solves)++;
+    g_launches += 1;
+    k_refine_argmax<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, v, ws, sc);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(sc + RF_VJL, v + jlast, sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    CK(cudaMemcpyAsync(h_rf + RF_J, sc + RF_J, 3 * sizeof(double), cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+    return CLDL_OK;
+  };
+  auto unit = [&](int j) {
+    g_launches += 1;
+    k_map<<<grid, 256, 0, stream>>>(nn, [=] __device__(int i) { v[i] = i == j ? 1.0 : 0.0; });
+  };
+  *est = 0.0;
+  if (n == 1) {
+    unit(0);
+    if (int rc = apply_B(false)) return rc;
+    *est = h_rf[RF_EST];
+    return CLDL_OK;
+  }
+  g_launches += 1;
+  k_map<<<grid, 256, 0, stream>>>(nn, [=] __device__(int i) { v[i] = 1.0 / nn; });
+  if (int rc = apply_B(true)) return rc;               // dlacn2 jump 1
+  double e = h_rf[RF_EST];
+  if (!(e == e)) { *est = e; return CLDL_OK; }
+  if (int rc = apply_Bt(0)) return rc;                 // jump 2
+  int j = (int)h_rf[RF_J];
+  for (int iter = 2;;) {
+    if (!(j >= 0 && j < n)) { *est = NAN; return CLDL_OK; }
+    unit(j);
+    if (int rc = apply_B(true)) return rc;             // jump 3
+    const double eold = e;
+    e = h_rf[RF_EST];
+    if (h_rf[RF_CNT] == 0.0 || !(e > eold)) break;     // repeated sign vector, or no increase
+    const int jlast = j;
+    if (int rc = apply_Bt(jlast)) return rc;           // jump 4
+    j = (int)h_rf[RF_J];
+    if (!(h_rf[RF_VJL] != h_rf[RF_VJ] && iter < 5)) break;
+    iter++;
+  }
+  // the alternating-sign test vector (jump 5)
+  g_launches += 1;
+  k_map<<<grid, 256, 0, stream>>>(nn, [=] __device__(int i) { v[i] = (i & 1 ? -1.0 : 1.0) * (1.0 + (double)i / (nn - 1)); });
+  if (int rc = apply_B(false)) return rc;
+  const double t = 2.0 * h_rf[RF_EST] / (3.0 * n);
+  *est = t > e ? t : e;
+  return CLDL_OK;
+}
+
+// Iterative refinement against the current values (the header's cldl_solve_refined): x0 = the plain solve into d_x,
+// each step dx = K^-1 r and x <- x + dx in the work vector, the best iterate copied to d_x.  The stopping test reads
+// the iterate's omega1 + omega2 on the host.
+int LDLObject::solve_refined(double* d_x, const double* d_b, const cldl_refine_opts& o, cldl_refine_info* info) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!(o.max_iter >= 0 && o.tol >= 0.0 && o.stop_ratio >= 1.0)) return CLDL_E_ARG;
+  if (2 * nnzA - n > 0x7fffffff) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  CK(cudaSetDevice(device));
+  if (!d_rf_work) {
+    const size_t mk = own.mark();
+    if (int rc = refine_setup()) { own.release_since(mk); d_rf_work = nullptr; return rc; }
+  }
+  double *xc = d_rf_work, *r = d_rf_work + (size_t)n, *dx = d_rf_work + 2 * (size_t)n;
+  const size_t bytes = (size_t)n * sizeof(double);
+  cldl_refine_info in{};
+  auto record = [&]() {          // the analysis just read into h_rf, as the info of its iterate
+    in.norm_x_inf = h_rf[RF_XN];
+    in.resid_inf = h_rf[RF_RINF];
+    in.omega1 = h_rf[RF_W1];
+    in.omega2 = h_rf[RF_W2];
+  };
+  if (int rc = solve_async(d_x, d_b)) return rc;
+  in.solves = 1;
+  if (int rc = refine_analyse(d_x, d_b, true)) return rc;
+  in.norm_K_inf = h_rf[RF_KN];
+  record();
+  double w = h_rf[RF_W1] + h_rf[RF_W2], best = w;
+  bool best_last = true;         // the best iterate is the one analysed last (its r, kx, rmax are in the work vectors)
+  if (o.max_iter > 0 && std::isfinite(w) && w > o.tol) CK(cudaMemcpyAsync(xc, d_x, bytes, cudaMemcpyDeviceToDevice, stream));
+  for (int k = 0; k < o.max_iter && std::isfinite(w) && w > o.tol; k++) {
+    if (int rc = solve_async(dx, r)) return rc;
+    in.solves++;
+    in.steps++;
+    g_launches++;
+    k_map<<<(n + 255) / 256, 256, 0, stream>>>(n, [=] __device__(int i) { xc[i] += dx[i]; });
+    if (int rc = refine_analyse(xc, d_b, false)) return rc;
+    const double wn = h_rf[RF_W1] + h_rf[RF_W2];
+    best_last = wn < best;
+    if (best_last) {
+      best = wn;
+      record();
+      CK(cudaMemcpyAsync(d_x, xc, bytes, cudaMemcpyDeviceToDevice, stream));
+    }
+    if (!(wn * o.stop_ratio <= w)) break;    // not divided by stop_ratio, or not finite
+    w = wn;
+  }
+  in.converged = best <= o.tol ? 1 : 0;
+  const double den = in.norm_K_inf * in.norm_x_inf;
+  in.scaled_resid = in.resid_inf == 0.0 ? 0.0 : in.resid_inf / den;
+  if (o.error_analysis) {
+    if (!best_last)                // den1, den2 and the sets of the returned x
+      if (int rc = refine_analyse(d_x, d_b, false)) return rc;
+    const bool has[2] = {h_rf[RF_HAS1] != 0.0, h_rf[RF_HAS2] != 0.0};
+    double est[2] = {0.0, 0.0};
+    for (int c = 0; c < 2; c++)
+      if (has[c] && in.norm_x_inf > 0.0)
+        if (int rc = condest(c + 1, d_b, est + c, &in.solves)) return rc;
+    if (in.norm_x_inf > 0.0) {
+      in.cond1 = est[0] / in.norm_x_inf;
+      in.cond2 = est[1] / in.norm_x_inf;
+    }
+    in.ferr = in.omega1 * in.cond1 + in.omega2 * in.cond2;
+  }
+  if (info) *info = in;
   return CLDL_OK;
 }
 
@@ -2079,6 +2275,40 @@ int cldl_adjoint_solve(cldl_t* h, const double* g, const double* x, double* gb, 
 int cldl_adjoint_solve_dev(cldl_t* h, const double* d_g, const double* d_x, double* d_gb, double* d_gvals) {
   if (!h || !d_g || !d_gb || (d_gvals && !d_x)) return CLDL_E_ARG;
   return h->obj.adjoint_async(d_g, d_x, d_gb, d_gvals);
+}
+
+void cldl_default_refine_opts(cldl_refine_opts* o) {
+  std::memset(o, 0, sizeof(*o));
+  o->max_iter = 10;
+  o->tol = DBL_EPSILON;
+  o->stop_ratio = 2.0;
+  o->error_analysis = 0;
+}
+void cldl_refine_abi_sizes(uint64_t* out2) {
+  out2[0] = sizeof(cldl_refine_opts);
+  out2[1] = sizeof(cldl_refine_info);
+}
+int cldl_solve_refined_dev(cldl_t* h, double* d_x, const double* d_b, const cldl_refine_opts* opts,
+                           cldl_refine_info* info) {
+  if (!h || !d_x || !d_b) return CLDL_E_ARG;
+  cldl_refine_opts o;
+  if (opts) o = *opts; else cldl_default_refine_opts(&o);
+  return h->obj.solve_refined(d_x, d_b, o, info);
+}
+int cldl_solve_refined(cldl_t* h, double* x, const double* b, const cldl_refine_opts* opts, cldl_refine_info* info) {
+  if (!h || !x || !b) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (o.sharded() || o.schur) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t bytes = (size_t)o.n * sizeof(double);
+  if (cudaMemcpyAsync(o.d_bx, b, bytes, cudaMemcpyHostToDevice, o.stream) != cudaSuccess) return CLDL_E_CUDA;
+  int rc = cldl_solve_refined_dev(h, o.d_bx + o.n, o.d_bx, opts, info);
+  if (rc) return rc;
+  if (cudaMemcpyAsync(x, o.d_bx + o.n, bytes, cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
 }
 
 int cldl_create_schur(cldl_t** out, uint64_t n, const uint64_t* colptr, const uint64_t* rowval,

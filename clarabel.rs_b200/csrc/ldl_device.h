@@ -147,6 +147,16 @@ class LDLObject {
   unsigned* d_ld_cnt = nullptr;          // the reduction's block counter
   int logdet(double* logabsdet, int32_t* sign);
   int adjoint_async(const double* d_g, const double* d_x, double* d_gb, double* d_gvals);
+  // iterative refinement and error analysis (cldl_solve_refined, ldl_refine.cuh): allocated by the first call
+  int *d_rf_rowptr = nullptr, *d_rf_col = nullptr, *d_rf_src = nullptr;   // K's mirrored pattern, CSR, src into vals
+  double* d_rf_work = nullptr;           // [RF_NVEC n] work vectors
+  double* d_rf_ws = nullptr;             // [8 RED_BLOCKS] reduction partials, then [RF_NS] scalars
+  unsigned* d_rf_cnt = nullptr;          // the reductions' block counter
+  double* h_rf = nullptr;                // [RF_NS] pinned copy of the scalars
+  int refine_setup();
+  int refine_analyse(const double* d_xv, const double* d_b, bool first);
+  int condest(int which, const double* d_b, double* est, uint32_t* solves);
+  int solve_refined(double* d_x, const double* d_b, const cldl_refine_opts& o, cldl_refine_info* info);
   // Schur complement handle (cldl_create_schur; SchurPlan in ldl_plan.h): B's fronts are factored, S's never
   std::vector<int> schur_set;            // non-empty: a Schur complement handle
   bool schur = false;

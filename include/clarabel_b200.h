@@ -196,6 +196,67 @@ int cldl_logdet(cldl_t *h, double *logabsdet, int32_t *sign);
 int cldl_adjoint_solve(cldl_t *h, const double *g, const double *x, double *gb, double *gvals);
 int cldl_adjoint_solve_dev(cldl_t *h, const double *d_g, const double *d_x, double *d_gb, double *d_gvals);
 
+/* Iterative refinement and error analysis (MUMPS ICNTL(10) / ICNTL(11), PARDISO iparm(8)).
+ * K is the symmetric matrix of the handle's CURRENT values, cldl_values_dev: the caller's upper triangle mirrored,
+ * including every cldl_update_values / scale / offset / set_values_dev since the last refactor.  The correction solves
+ * use the factor of the last refactor; when the two differ the factor is only a preconditioner, and refinement
+ * converges only when the change is small.  For an iterate x, with r = b - K x:
+ *     den1_i = (|K||x|)_i + |b_i|
+ *     den2_i = (|K||x|)_i + ||K_i||_inf ||x||_inf          (||K_i||_inf = max_j |K_ij|)
+ *     tau_i  = 1000 n eps (||K_i||_inf ||x||_inf + |b_i|)
+ *     I1 = {i : den1_i > tau_i}, I2 the rest
+ *     omega1 = max over I1 of |r_i| / den1_i
+ *     omega2 = max over I2 of |r_i| / den2_i, a row with den2_i = 0 and r_i = 0 counting 0
+ * and an empty set gives 0: the componentwise backward errors of Arioli, Demmel and Duff (1989), as MUMPS reports them
+ * in RINFOG(7..8).
+ *   - Loop: x0 is the plain solve, bitwise cldl_solve(b).  Each step solves for dx with the factor and sets
+ *     x <- x + dx.  It stops when omega1 + omega2 <= tol, when max_iter steps are done, when a step does not divide
+ *     omega1 + omega2 by at least stop_ratio, or when omega1 + omega2 is not finite.  The iterate with the smallest
+ *     omega1 + omega2 seen is returned (the earlier one on a tie), with its analysis in info.
+ *   - Error analysis (error_analysis = 1), at the returned x:
+ *         cond1 = || |K^-1| (den1 o 1_I1) ||_inf / ||x||_inf,   cond2 = || |K^-1| (den2 o 1_I2) ||_inf / ||x||_inf,
+ *         ferr = omega1 cond1 + omega2 cond2,
+ *     each from Higham's 1-norm estimator (Hager's method with Higham's safeguards, LAPACK dlacn2) applied to
+ *     B = diag(g) K^-1, B^T y = K^-1 (g o y): at most 5 iterations plus the alternating-sign test vector, at most 11
+ *     solves per estimate; an empty I1 or I2 costs no solves.  K^-1 here is the inverse of the factored matrix: with
+ *     dynamic regularisation (cldl_info.regularize_count > 0) or values changed since the refactor, the estimates are
+ *     of that matrix's inverse.  Without error analysis cond1, cond2 and ferr are 0; they are 0 also when x = 0.
+ *   - Returns CLDL_OK or a negative code; convergence is info.converged (omega1 + omega2 <= tol for the returned x),
+ *     not the return value.  CLDL_E_NOT_FACTORED without a refactor that returned 1.  CLDL_E_ARG on a Schur handle, a
+ *     sharded handle, for max_iter < 0, tol < 0 or stop_ratio < 1 (or NaN), and when the mirrored pattern (2 nnzA - n
+ *     entries) does not fit int32 indices.
+ *   - No floating-point atomics: two calls give the same bits.  The factor, D, 1/D and every later plain solve are
+ *     left bit for bit unchanged.
+ *   - Synchronisation: the stopping test runs on the host, so BOTH forms synchronise the handle's stream: one read of a
+ *     few scalars per refinement step, and one after every solve of the estimator.  cldl_solve_refined_dev takes
+ *     device buffers (d_x and d_b must not overlap) and never copies a vector to the host.
+ *   - The first call builds and uploads the mirrored pattern (int32 rowptr, column indices and a source map into the
+ *     values: (n + 1 + 2 (2 nnzA - n)) * 4 bytes) and allocates 6 n doubles of work vectors, 8 * 296 + 16 doubles of
+ *     reduction workspace and 16 doubles of pinned host memory.  cldl_destroy frees them.
+ * opts == NULL means the defaults of cldl_default_refine_opts; info may be NULL. */
+typedef struct {
+  int32_t max_iter;        /* refinement steps at most; 0 = the plain solve, analysed only      (default 10) */
+  double tol;              /* stop once omega1 + omega2 <= tol                                  (default DBL_EPSILON) */
+  double stop_ratio;       /* stop when a step does not divide omega1 + omega2 by at least this (default 2) */
+  int32_t error_analysis;  /* 1: also estimate cond1, cond2 and ferr (extra solves)             (default 0) */
+} cldl_refine_opts;
+
+typedef struct {
+  uint32_t steps;          /* refinement steps taken */
+  uint32_t solves;         /* LDL solves made by the call, estimator included */
+  int32_t converged;       /* 1 when the returned x has omega1 + omega2 <= tol */
+  double norm_K_inf, norm_x_inf, resid_inf;   /* ||K||_inf (current values), ||x||_inf, ||b - K x||_inf */
+  double scaled_resid;     /* resid_inf / (norm_K_inf * norm_x_inf); 0 when resid_inf = 0 */
+  double omega1, omega2;   /* componentwise backward errors of the returned x */
+  double cond1, cond2, ferr;   /* error_analysis only, else 0 */
+} cldl_refine_info;
+
+void cldl_default_refine_opts(cldl_refine_opts *o);
+int cldl_solve_refined(cldl_t *h, double *x, const double *b, const cldl_refine_opts *opts, cldl_refine_info *info);
+int cldl_solve_refined_dev(cldl_t *h, double *d_x, const double *d_b, const cldl_refine_opts *opts,
+                           cldl_refine_info *info);
+void cldl_refine_abi_sizes(uint64_t *out2);   /* sizeof cldl_refine_opts, cldl_refine_info */
+
 /* ---- device-pointer twins (asynchronous on the handle's stream) ---- */
 int cldl_update_values_dev(cldl_t *h, const int32_t *d_index, const double *d_values, uint64_t len);
 int cldl_set_values_dev(cldl_t *h, const double *d_nzval);   /* whole array, caller order */

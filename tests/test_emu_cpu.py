@@ -17,7 +17,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 MODULES = ["tests/test_cones_gpu.py", "tests/test_psd_gpu.py", "tests/test_ipm_gpu.py", "tests/test_zz_nonsym_gpu.py",
            "tests/test_zz_golden.py", "tests/test_zz_psd_large_gpu.py", "tests/test_zz_equilibration_gpu.py",
            "tests/test_zz_data_updating_gpu.py", "tests/test_zz_algebra_gpu.py", "tests/test_cone_shapes_gpu.py",
-           "tests/test_nonsym_shapes_gpu.py"]
+           "tests/test_nonsym_shapes_gpu.py", "tests/test_kkt_shapes_gpu.py"]
 # lists of tests/cone_shapes.py whose KKT matrix exceeds the dense stand-in's cap (PSD 64 and up, the 1e5 SOC, the
 # nonnegative pass boundaries); the full build runs PSD(64, 65)
 CONE_SHAPES_BIG = ["psd-n96-97", "psd-n128", "soc-long", "nonneg-75775", "nonneg-75776", "nonneg-75777", "nonneg-300000"]
@@ -38,6 +38,16 @@ _NS_BIG = [f"tests/test_nonsym_shapes_gpu.py::test_update_scaling_Hs_and_secant[
           [f"tests/test_nonsym_shapes_gpu.py::test_barrier[ns-big-{r}]" for r in ("opening", "late", "late-off", "edge")] + \
           [f"tests/test_nonsym_shapes_gpu.py::test_step_length[ns-big-{r}]" for r in ("opening", "late")]
 TOO_BIG += _NS_BIG
+# the lists of tests/kkt_shapes.py whose KKT matrix exceeds the dense stand-in's cap
+import kkt_shapes  # noqa: E402
+_KKT = "tests/test_kkt_shapes_gpu.py::"
+_KKT_BIG = [f"{_KKT}{t}[{c.name}-{r}]" for c in kkt_shapes.CASES if not c.emu
+            for r in kkt_shapes.REGIMES for t in ("test_values_after_update", "test_eps_is_the_references")] + \
+           [f"{_KKT}test_refined_solve[{c.name}-{r}-{s}]" for c in kkt_shapes.CASES if not c.emu
+            for r in kkt_shapes.REGIMES for s in ("defaults", "constant-1e-4")] + \
+           [f"{_KKT}test_regularisation_is_undone[{c.name}]" for c in kkt_shapes.CASES if not c.emu] + \
+           [f"{_KKT}test_paired_solves_with_extension_rows[{c.name}]" for c in kkt_shapes.CASES if not c.emu]
+TOO_BIG += _KKT_BIG
 
 
 # ---- the whole product, multifrontal kernels included (tests/emu/libclarabel_emu_full.so) ----
@@ -53,7 +63,7 @@ FULL_SKIP = [
     # amplified past the test's 1e-7; both thread orders agree bitwise with each other and the regularisation counts
     # equal the oracle's
     "tests/test_ldl_gpu.py::test_dynamic_regularisation_counts",
-] + _SHAPE_BIG + _NS_BIG
+] + _SHAPE_BIG + _NS_BIG + _KKT_BIG
 
 
 

@@ -190,6 +190,7 @@ EXPORTED_SYMBOLS = [
     "cldl_schur_reduce_dev", "cldl_schur_expand", "cldl_schur_expand_dev",
     "cldl_logdet", "cldl_adjoint_solve", "cldl_adjoint_solve_dev",
     "cldl_default_refine_opts", "cldl_solve_refined", "cldl_solve_refined_dev", "cldl_refine_abi_sizes",
+    "cldl_solve_sparse", "cldl_solve_sparse_dev", "cldl_inverse_entries", "cldl_sparse_stats",
 ]
 
 
@@ -425,6 +426,75 @@ class CudaLDLSolver:
         out = np.empty(rv.size, np.float64)
         _check(f(self._h, _p(out, C.c_double)), "selected_inverse")
         return sps.csc_matrix((out, rv.astype(np.int64), cp.astype(np.int64)), shape=(self.n, self.n))
+
+    def _sparse_args(self, b, want):
+        if isinstance(b, tuple):
+            bi, bv = _u64(np.asarray(b[0], dtype=np.int64).ravel()), _f64(np.asarray(b[1]).ravel())
+            assert bi.size == bv.size
+        else:
+            bi, bv = None, _f64(np.asarray(b).ravel())
+            assert bv.size == self.n
+        wi = None if want is None else _u64(np.asarray(want, dtype=np.int64).ravel())
+        return bi, bv, wi
+
+    def solve_sparse(self, b, want=None):
+        """x = (K + E)^-1 b with a sparse b and / or only some entries of x wanted, by solves pruned to the assembly
+        tree's paths from b's and the wanted indices to the root (see cldl_solve_sparse).  ``b`` is an (index, values)
+        pair (no duplicate indices) or a dense array of n values; ``want`` is None (all n entries) or an index array
+        (duplicates allowed).  Returns x[want] (or the whole x).  The entries equal (==) those of ``solve()`` on the
+        densified b.  BackendError (NotFactored) before a refactor that returned True, (BadArgument) on a Schur or
+        sharded handle, for an index out of range or a duplicate index in b."""
+        f = self._L.cldl_solve_sparse
+        f.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_double), C.c_uint64,
+                      C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        bi, bv, wi = self._sparse_args(b, want)
+        nx = self.n if wi is None else wi.size
+        x = np.empty(nx, np.float64)
+        _check(f(self._h, self.n if bi is None else bi.size, None if bi is None else _p(bi, C.c_uint64),
+                 _p(bv, C.c_double), nx, None if wi is None else _p(wi, C.c_uint64), _p(x, C.c_double)),
+               "solve_sparse")
+        return x
+
+    def solve_sparse_dev(self, b_index, d_b_ptr, nb, want, d_x_ptr):
+        """device-pointer form of ``solve_sparse`` (cldl_solve_sparse_dev): b's values at d_b_ptr (nb doubles, or n
+        when ``b_index`` is None), the result at d_x_ptr (len(want) doubles, or n when ``want`` is None); the index
+        arrays are host arrays.  Only enqueued on the handle's stream."""
+        f = self._L.cldl_solve_sparse_dev
+        f.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.c_void_p, C.c_uint64,
+                      C.POINTER(C.c_uint64), C.c_void_p]
+        f.restype = C.c_int
+        bi = None if b_index is None else _u64(np.asarray(b_index, dtype=np.int64).ravel())
+        wi = None if want is None else _u64(np.asarray(want, dtype=np.int64).ravel())
+        _check(f(self._h, int(nb), None if bi is None else _p(bi, C.c_uint64), C.c_void_p(d_b_ptr),
+                 self.n if wi is None else wi.size, None if wi is None else _p(wi, C.c_uint64), C.c_void_p(d_x_ptr)),
+               "solve_sparse_dev")
+
+    def inverse_entries(self, rows, cols):
+        """((K + E)^-1)[rows[k], cols[k]] for any positions, not only K's pattern (see cldl_inverse_entries): the
+        positions grouped by column, two columns per pair of pruned sweeps.  Each entry equals (==)
+        ``solve(e_j)[i]``.  Errors as for ``solve_sparse``."""
+        f = self._L.cldl_inverse_entries
+        f.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        r = _u64(np.asarray(rows, dtype=np.int64).ravel())
+        c = _u64(np.asarray(cols, dtype=np.int64).ravel())
+        assert r.size == c.size
+        out = np.empty(r.size, np.float64)
+        _check(f(self._h, r.size, _p(r, C.c_uint64), _p(c, C.c_uint64), _p(out, C.c_double)), "inverse_entries")
+        return out
+
+    def sparse_stats(self):
+        """counts of the last ``solve_sparse`` / ``inverse_entries`` call (cldl_sparse_stats): a dict with the host
+        milliseconds of its plan building, the fronts and panel entries its forward and backward sweeps reached, and
+        its host steps"""
+        f = self._L.cldl_sparse_stats
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        v = np.zeros(6, np.float64)
+        _check(f(self._h, _p(v, C.c_double)), "sparse_stats")
+        return {"plan_ms": v[0], "fronts_fwd": int(v[1]), "fronts_bwd": int(v[2]), "entries_fwd": int(v[3]),
+                "entries_bwd": int(v[4]), "host_work": int(v[5])}
 
     def slogdet(self):
         """(sign, logabsdet) of K + E, the matrix the last ``refactor()`` factored (E its dynamic regularisation), from

@@ -22,6 +22,7 @@
 #include <dlfcn.h>
 
 #include <cfloat>
+#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstring>
@@ -1073,6 +1074,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
 #include "ldl_selinv.cuh"
 #include "ldl_schur.cuh"
 #include "ldl_refine.cuh"
+#include "ldl_sparse.cuh"
 
 __global__ void k_update_values(double* __restrict__ vals, const int* __restrict__ idx,
                                 const double* __restrict__ v, long long len) {
@@ -1314,6 +1316,9 @@ int LDLObject::init(int n_, const int64_t* Ap, const int32_t* Ai, const double* 
     for (int g = 0; g < shard_nranks; g++) CK(own.upload(&d_shard_xidx[g], shard_xidx[g]));
   }
   if (schur && (rc = schur_setup(sp))) return rc;
+  sv_host = std::move(sp);          // pruned solves derive their plans from it; the gather lists live on the device only
+  sv_host.gat_ptr = std::vector<int>();
+  sv_host.gat_src = std::vector<int>();
   if (big_alloc.joinable()) big_alloc.join();
   if (big_alloc_rc) { std::fprintf(stderr, "[clarabel_b200] device allocation of the factor storage failed\n"); return CLDL_E_CUDA; }
   cb_tmark("ldl: big allocations joined");
@@ -1691,7 +1696,7 @@ int LDLObject::schur_reduce_async(double* d_wS, const double* d_b) {
   g_launches += 2;
   k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, d_b, d_xp);
   if (int rc = sv_reset()) return rc;
-  sv_leaves(true, 1, r);
+  sv_leaves(true, 1, r, sv_leaf_lists());
   SVPlan qv = sv;
   qv.ntask = sv_ntask_owned;
   sv_sweep(true, 1, qv, r);
@@ -1713,7 +1718,7 @@ int LDLObject::schur_expand_async(double* d_x, const double* d_xS) {
   g_launches++;
   k_schur_expand_in<<<(schur_k + 255) / 256, 256, 0, stream>>>(schur_first, schur_k, d_sc_spos, dev.perm, d_xS, d_xp, d_x);
   if (sv_bwd.ntask) sv_sweep(false, 1, sv_bwd, r);
-  sv_leaves(false, 1, r);
+  sv_leaves(false, 1, r, sv_leaf_lists());
   CK(cudaGetLastError());
   schur_fwd = false;     // the backward sweep overwrote the forward state
   return CLDL_OK;
@@ -1767,8 +1772,8 @@ void LDLObject::sv_sweep(bool fwd, int nrhs, const SVPlan& q, const SVRhs& r) {
 // the level-0 fronts: before the forward sweep, after the backward sweep.  The three kernels touch disjoint fronts and
 // none depends on another, so the two narrow-leaf kernels run on side streams next to the wide-leaf kernel
 // (C4: 24 + 48 + 186 us one after the other -> ~190 us together)
-void LDLObject::sv_leaves(bool fwd, int nrhs, const SVRhs& r) {
-  const bool side = ((sv_nleaf1 ? 1 : 0) + (sv_nleafn ? 1 : 0) + (sv_nleafw ? 1 : 0)) > 1;
+void LDLObject::sv_leaves(bool fwd, int nrhs, const SVRhs& r, const SVLeaves& lv) {
+  const bool side = ((lv.n1 ? 1 : 0) + (lv.nn ? 1 : 0) + (lv.nw ? 1 : 0)) > 1;
   cudaStream_t s1 = side ? stream_a : stream, sn = side ? stream_b : stream;
   if (side) {
     cudaEventRecord(ev_leaf[0], stream);
@@ -1776,18 +1781,18 @@ void LDLObject::sv_leaves(bool fwd, int nrhs, const SVRhs& r) {
     cudaStreamWaitEvent(sn, ev_leaf[0], 0);
   }
   if (fwd) {
-    if (sv_nleaf1) { g_launches++; if (nrhs == 1) k_fwd_leaf1<1><<<(sv_nleaf1 + 255) / 256, 256, 0, s1>>>(dev, d_sv_leaf1, sv_nleaf1, r); else k_fwd_leaf1<2><<<(sv_nleaf1 + 255) / 256, 256, 0, s1>>>(dev, d_sv_leaf1, sv_nleaf1, r); }
-    if (sv_nleafn) { g_launches++; if (nrhs == 1) k_leaf_small<1, true><<<(sv_nleafn + 7) / 8, 256, 0, sn>>>(dev, d_sv_leafn, sv_nleafn, r); else k_leaf_small<2, true><<<(sv_nleafn + 7) / 8, 256, 0, sn>>>(dev, d_sv_leafn, sv_nleafn, r); }
-    if (sv_nleafw) { g_launches++; if (nrhs == 1) k_fwd_leafw<1><<<sv_nleafw, SV_LEAF_NT, 0, stream>>>(dev, d_sv_leafw, sv_nleafw, r); else k_fwd_leafw<2><<<sv_nleafw, SV_LEAF_NT, 0, stream>>>(dev, d_sv_leafw, sv_nleafw, r); }
+    if (lv.n1) { g_launches++; if (nrhs == 1) k_fwd_leaf1<1><<<(lv.n1 + 255) / 256, 256, 0, s1>>>(dev, lv.l1, lv.n1, r); else k_fwd_leaf1<2><<<(lv.n1 + 255) / 256, 256, 0, s1>>>(dev, lv.l1, lv.n1, r); }
+    if (lv.nn) { g_launches++; if (nrhs == 1) k_leaf_small<1, true><<<(lv.nn + 7) / 8, 256, 0, sn>>>(dev, lv.ln, lv.nn, r); else k_leaf_small<2, true><<<(lv.nn + 7) / 8, 256, 0, sn>>>(dev, lv.ln, lv.nn, r); }
+    if (lv.nw) { g_launches++; if (nrhs == 1) k_fwd_leafw<1><<<lv.nw, SV_LEAF_NT, 0, stream>>>(dev, lv.lw, lv.nw, r); else k_fwd_leafw<2><<<lv.nw, SV_LEAF_NT, 0, stream>>>(dev, lv.lw, lv.nw, r); }
   } else {
-    if (sv_nleafw) {
+    if (lv.nw) {
       g_launches++;
       const size_t sm = (size_t)nrhs * (sv_leafw_nrmax + CB_PB_MAXNS) * sizeof(double);
-      if (nrhs == 1) k_bwd_leafw<1><<<sv_nleafw, SV_LEAF_NT, sm, stream>>>(dev, d_sv_leafw, sv_nleafw, r, sv_leafw_nrmax);
-      else k_bwd_leafw<2><<<sv_nleafw, SV_LEAF_NT, sm, stream>>>(dev, d_sv_leafw, sv_nleafw, r, sv_leafw_nrmax);
+      if (nrhs == 1) k_bwd_leafw<1><<<lv.nw, SV_LEAF_NT, sm, stream>>>(dev, lv.lw, lv.nw, r, sv_leafw_nrmax);
+      else k_bwd_leafw<2><<<lv.nw, SV_LEAF_NT, sm, stream>>>(dev, lv.lw, lv.nw, r, sv_leafw_nrmax);
     }
-    if (sv_nleafn) { g_launches++; if (nrhs == 1) k_leaf_small<1, false><<<(sv_nleafn + 7) / 8, 256, 0, sn>>>(dev, d_sv_leafn, sv_nleafn, r); else k_leaf_small<2, false><<<(sv_nleafn + 7) / 8, 256, 0, sn>>>(dev, d_sv_leafn, sv_nleafn, r); }
-    if (sv_nleaf1) { g_launches++; if (nrhs == 1) k_bwd_leaf1<1><<<(sv_nleaf1 + 255) / 256, 256, 0, s1>>>(dev, d_sv_leaf1, sv_nleaf1, r); else k_bwd_leaf1<2><<<(sv_nleaf1 + 255) / 256, 256, 0, s1>>>(dev, d_sv_leaf1, sv_nleaf1, r); }
+    if (lv.nn) { g_launches++; if (nrhs == 1) k_leaf_small<1, false><<<(lv.nn + 7) / 8, 256, 0, sn>>>(dev, lv.ln, lv.nn, r); else k_leaf_small<2, false><<<(lv.nn + 7) / 8, 256, 0, sn>>>(dev, lv.ln, lv.nn, r); }
+    if (lv.n1) { g_launches++; if (nrhs == 1) k_bwd_leaf1<1><<<(lv.n1 + 255) / 256, 256, 0, s1>>>(dev, lv.l1, lv.n1, r); else k_bwd_leaf1<2><<<(lv.n1 + 255) / 256, 256, 0, s1>>>(dev, lv.l1, lv.n1, r); }
   }
   if (side) {
     cudaEventRecord(ev_leaf[1], s1);
@@ -1822,11 +1827,321 @@ int LDLObject::solve_async(double* d_x, const double* d_b, double* d_x1, const d
   if (nrhs == 2) k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, d_b1, d_xp2);
   int rc = sv_reset();
   if (rc) return rc;
-  sv_leaves(true, nrhs, r);
+  sv_leaves(true, nrhs, r, sv_leaf_lists());
   sv_sweep(true, nrhs, sv, r);
   sv_sweep(false, nrhs, sv, r);
-  sv_leaves(false, nrhs, r);
+  sv_leaves(false, nrhs, r, sv_leaf_lists());
   CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Pruned solves (cldl_solve_sparse, cldl_inverse_entries): the sweeps of solve_async over the full plan restricted to
+// the upward closure of b's indices (forward) and of the wanted indices (backward), see PrunedPlan in ldl_plan.h.  A
+// side given densely (b or x at all n indices) runs the full plan.  Per call the host builds the plans and one payload
+// (plans, index lists, host values), which goes to the device in one copy out of a pinned buffer; the two pinned
+// buffers are used in turn, each guarded by an event, so the host builds the next payload while the device sweeps.
+
+// the first call: counters like the full plan's, marks, the pruned front2task, bpart and the host-side prune index
+int LDLObject::sparse_setup() {
+  CK(own.alloc(&d_sp_cnt, sv_ninit + sv_nzero));
+  CK(own.alloc(&d_sp_f2t, (size_t)S.nsup));
+  CK(own.alloc(&d_sp_mark, (size_t)S.nsup));
+  CK(own.alloc(&d_sp_bpart, (size_t)2 * sv.bpart_stride));
+  for (auto& e : sp_ev) CK(own.event(&e, cudaEventDisableTiming));
+  sp_prune = build_solve_prune(S, sv_host);
+  sp_seen.assign(n, 0);
+  sp_seen_epoch = 0;
+  return CLDL_OK;
+}
+
+namespace {
+template <class T>
+size_t sp_put(std::vector<char>& buf, const T* p, size_t cnt) {    // 16-byte aligned section of the payload
+  const size_t off = (buf.size() + 15) & ~(size_t)15;
+  buf.resize(off + cnt * sizeof(T));
+  if (cnt) std::memcpy(buf.data() + off, p, cnt * sizeof(T));
+  return off;
+}
+template <class T>
+size_t sp_put(std::vector<char>& buf, const std::vector<T>& v) { return sp_put(buf, v.data(), v.size()); }
+struct SPOff { size_t tasks, fronts, pend, pairs, reached, l1, ln, lw; };
+SPOff sp_put_plan(std::vector<char>& b, const PrunedPlan& P) {
+  SPOff o;
+  o.tasks = sp_put(b, P.tasks); o.fronts = sp_put(b, P.fronts); o.pend = sp_put(b, P.pend); o.pairs = sp_put(b, P.f2t);
+  o.reached = sp_put(b, P.reached); o.l1 = sp_put(b, P.leaf1); o.ln = sp_put(b, P.leafn); o.lw = sp_put(b, P.leafw);
+  return o;
+}
+}  // namespace
+
+SparseSide LDLObject::sparse_full_side() const {
+  SparseSide sd;
+  sd.q = sv;
+  sd.lv = sv_leaf_lists();
+  return sd;
+}
+
+// the payload in sp_payload to the device stage (capacities grow here: the only place a pruned call synchronises
+// the stream), and d_sp_out of at least need_out doubles
+int LDLObject::sparse_stage(size_t need_out) {
+  const size_t bytes = sp_payload.size();
+  if (bytes > sp_stage_cap || need_out > sp_out_cap) {
+    CK(cudaStreamSynchronize(stream));          // enqueued sweeps may still read the device stage
+    if (bytes > sp_stage_cap) {
+      own.free(d_sp_stage); own.free(h_sp_stage[0]); own.free(h_sp_stage[1]);   // first: a failure leaves a capacity of 0
+      d_sp_stage = nullptr; h_sp_stage[0] = h_sp_stage[1] = nullptr;
+      sp_stage_cap = 0;
+      const size_t cap = bytes + bytes / 2 + 4096;
+      CK(own.alloc(&d_sp_stage, cap));
+      CK(own.alloc_host(&h_sp_stage[0], cap));
+      CK(own.alloc_host(&h_sp_stage[1], cap));
+      sp_stage_cap = cap;
+    }
+    if (need_out > sp_out_cap) {
+      own.free(d_sp_out);
+      d_sp_out = nullptr;
+      sp_out_cap = 0;
+      const size_t cap = need_out + need_out / 2 + 256;
+      CK(own.alloc(&d_sp_out, cap));
+      sp_out_cap = cap;
+    }
+  }
+  char* h = h_sp_stage[sp_turn];
+  CK(cudaEventSynchronize(sp_ev[sp_turn]));    // the copy out of this buffer, two calls ago, has finished
+  if (bytes) std::memcpy(h, sp_payload.data(), bytes);
+  CK(cudaMemcpyAsync(d_sp_stage, h, bytes, cudaMemcpyHostToDevice, stream));
+  CK(cudaEventRecord(sp_ev[sp_turn], stream));
+  sp_turn ^= 1;
+  return CLDL_OK;
+}
+
+// counters reset, the pruned forward set's marks, task pairs and fringe, then the solve's launch sequence over F and B
+int LDLObject::sparse_sweeps(int nrhs, const SparseSide& F0, const SparseSide& B0, const SVRhs& r) {
+  SparseSide F = F0, B = B0;
+  const int nt = sv.ntask, nsup = S.nsup;
+  int* cnt = d_sp_cnt;
+  for (SVPlan* q : {&F.q, &B.q}) {
+    q->trace = nullptr;
+    q->bpart = d_sp_bpart;
+    q->fleft = cnt + nt; q->bleft = q->fleft + nsup;
+    q->tdone = cnt + sv_ninit; q->ydone = q->tdone + nt; q->done = q->ydone + nsup; q->qhead = q->done + nsup;
+  }
+  if (!F.pruned) F.q.pend = cnt;
+  B.q.pend = cnt;
+  CK(cudaMemcpyAsync(cnt, d_sv_init, sv_ninit * sizeof(int), cudaMemcpyDeviceToDevice, stream));
+  CK(cudaMemsetAsync(cnt + sv_ninit, 0, sv_nzero * sizeof(int), stream));
+  if (F.pruned) {
+    F.q.front2task = d_sp_f2t;
+    CK(cudaMemsetAsync(d_sp_mark, 0, (size_t)nsup, stream));
+    const int m = std::max(F.nreached, F.npairs);
+    if (m) {
+      g_launches += 2;
+      k_sparse_setup<<<(m + 255) / 256, 256, 0, stream>>>(F.nreached, F.reached, d_sp_mark, F.npairs, F.pairs, d_sp_f2t);
+      k_sparse_fringe<<<(F.nreached + 7) / 8, 256, 0, stream>>>(dev, F.reached, F.nreached, d_sp_mark, r.u[0],
+                                                                nrhs == 2 ? r.u[1] : nullptr);
+    }
+  }
+  sv_leaves(true, nrhs, r, F.lv);
+  if (F.q.ntask) sv_sweep(true, nrhs, F.q, r);
+  if (B.q.ntask) sv_sweep(false, nrhs, B.q, r);
+  sv_leaves(false, nrhs, r, B.lv);
+  CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+namespace {
+// a pruned side whose arrays sit in the device stage at the offsets o
+SparseSide sp_side(const SVPlan& sv, const PrunedPlan& P, const SPOff& o, char* base) {
+  SparseSide sd;
+  sd.q = sv;
+  sd.pruned = true;
+  sd.q.ntask = (int)P.tasks.size();
+  sd.q.tasks = reinterpret_cast<const int4*>(base + o.tasks);
+  sd.q.fronts = reinterpret_cast<const int*>(base + o.fronts);
+  sd.q.pend = reinterpret_cast<int*>(base + o.pend);
+  sd.pairs = reinterpret_cast<const int*>(base + o.pairs);
+  sd.npairs = (int)P.f2t.size() / 2;
+  sd.reached = reinterpret_cast<const int*>(base + o.reached);
+  sd.nreached = (int)P.reached.size();
+  sd.lv = SVLeaves{reinterpret_cast<const int*>(base + o.l1), reinterpret_cast<const int*>(base + o.ln),
+                   reinterpret_cast<const int*>(base + o.lw), (int)P.leaf1.size(), (int)P.leafn.size(), (int)P.leafw.size()};
+  return sd;
+}
+double sp_ms_since(const std::chrono::steady_clock::time_point& t0) {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
+}  // namespace
+
+int LDLObject::solve_sparse_async(uint64_t nb, const uint64_t* b_index, const double* b_values, bool b_dev,
+                                  uint64_t nx, const uint64_t* x_index, double* x_values, bool x_dev) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if ((!b_index && nb != (uint64_t)n) || (nb && !b_values) || (!x_index && nx != (uint64_t)n) || (nx && !x_values))
+    return CLDL_E_ARG;
+  CK(cudaSetDevice(device));
+  if (!sp_ready) {
+    const size_t mk = own.mark();
+    if (int rc = sparse_setup()) {
+      own.release_since(mk);
+      d_sp_cnt = d_sp_f2t = nullptr; d_sp_mark = nullptr; d_sp_bpart = nullptr; sp_ev[0] = sp_ev[1] = nullptr;
+      return rc;
+    }
+    sp_ready = true;
+  }
+  const auto t0 = std::chrono::steady_clock::now();
+  const int* iperm = S.iperm.data();
+  std::vector<int> bpos(b_index ? nb : 0), xpos(x_index ? nx : 0);
+  if (b_index) {
+    if (++sp_seen_epoch == 0) { std::fill(sp_seen.begin(), sp_seen.end(), 0u); sp_seen_epoch = 1; }
+    for (uint64_t i = 0; i < nb; i++) {
+      if (b_index[i] >= (uint64_t)n) return CLDL_E_ARG;
+      const int p = iperm[b_index[i]];
+      if (sp_seen[p] == sp_seen_epoch) return CLDL_E_ARG;
+      sp_seen[p] = sp_seen_epoch;
+      bpos[i] = p;
+    }
+  }
+  for (uint64_t i = 0; x_index && i < nx; i++) {
+    if (x_index[i] >= (uint64_t)n) return CLDL_E_ARG;
+    xpos[i] = iperm[x_index[i]];
+  }
+  if (nx == 0) return CLDL_OK;
+  if (nb == 0) {        // b = 0
+    if (x_dev) CK(cudaMemsetAsync(x_values, 0, nx * sizeof(double), stream));
+    else std::memset(x_values, 0, nx * sizeof(double));
+    return CLDL_OK;
+  }
+  const bool fpr = b_index != nullptr, bpr = x_index != nullptr;
+  sp_payload.clear();
+  SPOff fo{}, bo{};
+  sp_work = 0;
+  sp_reached[0] = sp_reached[1] = sp_entries[0] = sp_entries[1] = 0;
+  if (fpr) {
+    build_pruned_plan(S, sv_host, sp_prune, bpos.data(), bpos.size(), sp_plan[0]);
+    fo = sp_put_plan(sp_payload, sp_plan[0]);
+    sp_work += sp_plan[0].work; sp_reached[0] = (long long)sp_plan[0].reached.size(); sp_entries[0] = sp_plan[0].entries;
+  }
+  if (bpr) {
+    build_pruned_plan(S, sv_host, sp_prune, xpos.data(), xpos.size(), sp_plan[1]);
+    bo = sp_put_plan(sp_payload, sp_plan[1]);
+    sp_work += sp_plan[1].work; sp_reached[1] = (long long)sp_plan[1].reached.size(); sp_entries[1] = sp_plan[1].entries;
+  }
+  const size_t o_bpos = sp_put(sp_payload, bpos);
+  const size_t o_bval = (fpr && !b_dev) ? sp_put(sp_payload, b_values, nb) : 0;
+  const size_t o_xpos = sp_put(sp_payload, xpos);
+  sp_plan_ms = sp_ms_since(t0);
+  if (int rc = sparse_stage(x_dev ? 0 : nx)) return rc;
+  char* base = d_sp_stage;
+  const SparseSide F = fpr ? sp_side(sv, sp_plan[0], fo, base) : sparse_full_side();
+  const SparseSide B = bpr ? sp_side(sv, sp_plan[1], bo, base) : sparse_full_side();
+  SVRhs r;
+  double* out = (!bpr && x_dev) ? x_values : d_bx + n;     // every entry of x when the backward side is full
+  r.xp[0] = r.xp[1] = d_xp; r.u[0] = r.u[1] = dev.u; r.out[0] = r.out[1] = out;
+  if (fpr) {
+    CK(cudaMemsetAsync(d_xp, 0, (size_t)n * sizeof(double), stream));
+    g_launches++;
+    k_sparse_scatter<<<(unsigned)((nb + 255) / 256), 256, 0, stream>>>((int)nb, reinterpret_cast<const int*>(base + o_bpos),
+                                                                      b_dev ? b_values : reinterpret_cast<const double*>(base + o_bval), d_xp);
+  } else {
+    const double* db = b_values;
+    if (!b_dev) { CK(cudaMemcpyAsync(d_bx, b_values, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, stream)); db = d_bx; }
+    g_launches++;
+    k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, db, d_xp);
+  }
+  if (int rc = sparse_sweeps(1, F, B, r)) return rc;
+  if (bpr) {
+    g_launches++;
+    k_sparse_gather<<<(unsigned)((nx + 255) / 256), 256, 0, stream>>>((int)nx, (int)nx, reinterpret_cast<const int*>(base + o_xpos),
+                                                                     nullptr, d_xp, d_xp, x_dev ? x_values : d_sp_out);
+  }
+  CK(cudaGetLastError());
+  if (!x_dev) {
+    CK(cudaMemcpyAsync(x_values, bpr ? d_sp_out : out, nx * sizeof(double), cudaMemcpyDeviceToHost, stream));
+    CK(cudaStreamSynchronize(stream));
+  }
+  return CLDL_OK;
+}
+
+// entries of (K + E)^-1: the requested (i, j) grouped by column j, the columns solved two per sweep (NR = 2) over the
+// union of the pair's closures, each column's rows gathered into out (host, nnz doubles)
+int LDLObject::inverse_entries(uint64_t nnz, const uint64_t* rows, const uint64_t* cols, double* out) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if (nnz && (!rows || !cols || !out)) return CLDL_E_ARG;
+  for (uint64_t k = 0; k < nnz; k++)
+    if (rows[k] >= (uint64_t)n || cols[k] >= (uint64_t)n) return CLDL_E_ARG;
+  if (nnz == 0) return CLDL_OK;
+  if (nnz > (uint64_t)INT32_MAX) return CLDL_E_ARG;
+  CK(cudaSetDevice(device));
+  if (!sp_ready) {
+    const size_t mk = own.mark();
+    if (int rc = sparse_setup()) {
+      own.release_since(mk);
+      d_sp_cnt = d_sp_f2t = nullptr; d_sp_mark = nullptr; d_sp_bpart = nullptr; sp_ev[0] = sp_ev[1] = nullptr;
+      return rc;
+    }
+    sp_ready = true;
+  }
+  const auto t0 = std::chrono::steady_clock::now();
+  std::vector<int> order(nnz);
+  for (uint64_t k = 0; k < nnz; k++) order[k] = (int)k;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return cols[a] < cols[b]; });
+  std::vector<size_t> cstart;                 // ranges of order[] with one column
+  for (size_t k = 0; k < nnz; k++) if (k == 0 || cols[order[k]] != cols[order[k - 1]]) cstart.push_back(k);
+  cstart.push_back(nnz);
+  const int ncol = (int)cstart.size() - 1;
+  const int* iperm = S.iperm.data();
+  double plan_ms = sp_ms_since(t0);
+  long long work = 0, reached[2] = {0, 0}, entries[2] = {0, 0};
+  std::vector<int> fcols, bcols, gpos, gdst;
+  for (int c = 0; c < ncol; c += 2) {
+    const auto t1 = std::chrono::steady_clock::now();
+    const int nrhs = c + 1 < ncol ? 2 : 1;
+    fcols.clear(); bcols.clear(); gpos.clear(); gdst.clear();
+    int cnt0 = 0;
+    for (int h = 0; h < nrhs; h++) {
+      fcols.push_back(iperm[cols[order[cstart[c + h]]]]);
+      for (size_t k = cstart[c + h]; k < cstart[c + h + 1]; k++) {
+        const int p = iperm[rows[order[k]]];
+        bcols.push_back(p);
+        gpos.push_back(p);
+        gdst.push_back(order[k]);
+      }
+      if (h == 0) cnt0 = (int)gpos.size();
+    }
+    build_pruned_plan(S, sv_host, sp_prune, fcols.data(), fcols.size(), sp_plan[0]);
+    build_pruned_plan(S, sv_host, sp_prune, bcols.data(), bcols.size(), sp_plan[1]);
+    sp_payload.clear();
+    const SPOff fo = sp_put_plan(sp_payload, sp_plan[0]), bo = sp_put_plan(sp_payload, sp_plan[1]);
+    const size_t o_f = sp_put(sp_payload, fcols), o_gp = sp_put(sp_payload, gpos), o_gd = sp_put(sp_payload, gdst);
+    work += sp_plan[0].work + sp_plan[1].work;
+    for (int d = 0; d < 2; d++) { reached[d] += (long long)sp_plan[d].reached.size(); entries[d] += sp_plan[d].entries; }
+    plan_ms += sp_ms_since(t1);
+    if (int rc = sparse_stage(nnz)) return rc;
+    char* base = d_sp_stage;
+    const SparseSide F = sp_side(sv, sp_plan[0], fo, base), B = sp_side(sv, sp_plan[1], bo, base);
+    SVRhs r;
+    r.xp[0] = d_xp; r.u[0] = dev.u; r.out[0] = d_bx;
+    r.xp[1] = nrhs == 2 ? d_xp2 : d_xp; r.u[1] = nrhs == 2 ? d_u2 : dev.u; r.out[1] = nrhs == 2 ? d_bx + n : d_bx;
+    const int* fp = reinterpret_cast<const int*>(base + o_f);
+    g_launches += nrhs;
+    for (int h = 0; h < nrhs; h++) {
+      CK(cudaMemsetAsync(r.xp[h], 0, (size_t)n * sizeof(double), stream));
+      k_sparse_scatter<<<1, 32, 0, stream>>>(1, fp + h, nullptr, r.xp[h]);
+    }
+    if (int rc = sparse_sweeps(nrhs, F, B, r)) return rc;
+    g_launches++;
+    const int cnt = (int)gpos.size();
+    k_sparse_gather<<<(unsigned)((cnt + 255) / 256), 256, 0, stream>>>(cnt, cnt0, reinterpret_cast<const int*>(base + o_gp),
+                                                                      reinterpret_cast<const int*>(base + o_gd), r.xp[0],
+                                                                      r.xp[1], d_sp_out);
+    CK(cudaGetLastError());
+  }
+  sp_plan_ms = plan_ms;
+  sp_work = work;
+  for (int d = 0; d < 2; d++) { sp_reached[d] = reached[d]; sp_entries[d] = entries[d]; }
+  CK(cudaMemcpyAsync(out, d_sp_out, nnz * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));
   return CLDL_OK;
 }
 
@@ -1889,7 +2204,7 @@ int LDLObject::solve_phase_async(double* d_x, const double* d_b, int phase) {
     k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, d_b, d_xp);
     int rc = sv_reset();
     if (rc) return rc;
-    sv_leaves(true, 1, r);
+    sv_leaves(true, 1, r, sv_leaf_lists());
     qv.ntask = sv_ntask_owned;
     sv_sweep(true, 1, qv, r);
   } else {
@@ -1897,7 +2212,7 @@ int LDLObject::solve_phase_async(double* d_x, const double* d_b, int phase) {
     CK(cudaMemcpyAsync(qv.qhead, &h_phase_start[1], sizeof(int), cudaMemcpyHostToDevice, stream));
     sv_sweep(true, 1, qv, r);
     sv_sweep(false, 1, qv, r);
-    sv_leaves(false, 1, r);
+    sv_leaves(false, 1, r, sv_leaf_lists());
   }
   CK(cudaGetLastError());
   return CLDL_OK;
@@ -2250,6 +2565,29 @@ int cldl_selected_inverse_dev(cldl_t* h, double* d_nzval_out) {
 int cldl_logdet(cldl_t* h, double* logabsdet, int32_t* sign) {
   if (!h || !logabsdet || !sign) return CLDL_E_ARG;
   return h->obj.logdet(logabsdet, sign);
+}
+
+int cldl_solve_sparse(cldl_t* h, uint64_t nb, const uint64_t* b_index, const double* b_values,
+                      uint64_t nx, const uint64_t* x_index, double* x_values) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.solve_sparse_async(nb, b_index, b_values, false, nx, x_index, x_values, false);
+}
+int cldl_solve_sparse_dev(cldl_t* h, uint64_t nb, const uint64_t* b_index, const double* d_b_values,
+                          uint64_t nx, const uint64_t* x_index, double* d_x_values) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.solve_sparse_async(nb, b_index, d_b_values, true, nx, x_index, d_x_values, true);
+}
+int cldl_inverse_entries(cldl_t* h, uint64_t nnz, const uint64_t* rows, const uint64_t* cols, double* out) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.inverse_entries(nnz, rows, cols, out);
+}
+int cldl_sparse_stats(const cldl_t* h, double* out6) {
+  if (!h || !out6) return CLDL_E_ARG;
+  const LDLObject& o = h->obj;
+  const double v[6] = {o.sp_plan_ms, (double)o.sp_reached[0], (double)o.sp_reached[1], (double)o.sp_entries[0],
+                       (double)o.sp_entries[1], (double)o.sp_work};
+  for (int i = 0; i < 6; i++) out6[i] = v[i];
+  return CLDL_OK;
 }
 
 int cldl_adjoint_solve(cldl_t* h, const double* g, const double* x, double* gb, double* gvals) {

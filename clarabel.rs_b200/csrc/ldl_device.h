@@ -85,6 +85,22 @@ struct SIPlan {
 };
 
 
+// the level-0 fronts the plain leaf kernels solve: single-column, other narrow, wide
+struct SVLeaves {
+  const int *l1 = nullptr, *ln = nullptr, *lw = nullptr;
+  int n1 = 0, nn = 0, nw = 0;
+};
+
+// one direction of a pruned solve on the device: the queue, its leaves and (forward) the closure with its task pairs
+struct SparseSide {
+  SVPlan q;
+  SVLeaves lv;
+  bool pruned = false;
+  const int* reached = nullptr;
+  const int* pairs = nullptr;
+  int nreached = 0, npairs = 0;
+};
+
 class LDLObject {
  public:
   DevOwner own;                     // every stream, event and buffer below
@@ -95,11 +111,40 @@ class LDLObject {
   size_t sv_ninit = 0, sv_nzero = 0, sv_smem[2] = {0, 0};
   int sv_cap = 0, sv_nwide = 0, sv_nleaf1 = 0, sv_nleafn = 0, sv_nleafw = 0, sv_leafw_nrmax = 0, sv_leafw_grid = 1, sv_ntask_owned = 0;
   std::vector<SVTask> h_sv_tasks;
+  SolvePlan sv_host;                // the full solve plan on the host, gather lists dropped (pruned plans derive from it)
   int sv_configure();
   int sv_occupancy();
   int sv_reset();
   void sv_sweep(bool fwd, int nrhs, const SVPlan& q, const SVRhs& r);
-  void sv_leaves(bool fwd, int nrhs, const SVRhs& r);
+  SVLeaves sv_leaf_lists() const { return SVLeaves{d_sv_leaf1, d_sv_leafn, d_sv_leafw, sv_nleaf1, sv_nleafn, sv_nleafw}; }
+  void sv_leaves(bool fwd, int nrhs, const SVRhs& r, const SVLeaves& lv);
+  // pruned solves (cldl_solve_sparse, cldl_inverse_entries; ldl_sparse.cuh): set up by the first call
+  SolvePrune sp_prune;
+  PrunedPlan sp_plan[2];            // forward, backward
+  bool sp_ready = false;
+  int* d_sp_cnt = nullptr;          // counters, laid out like d_sv_cnt
+  int* d_sp_f2t = nullptr;          // [nsup] front2task of the pruned forward plan
+  unsigned char* d_sp_mark = nullptr;   // [nsup] fronts of the pruned forward set
+  double* d_sp_bpart = nullptr;     // like sv.bpart
+  char* d_sp_stage = nullptr;       // the per-call payload (plans, index lists, values) on the device
+  char* h_sp_stage[2] = {nullptr, nullptr};   // the same, pinned, used in turn; sp_ev[k] follows the copy out of [k]
+  cudaEvent_t sp_ev[2] = {nullptr, nullptr};
+  size_t sp_stage_cap = 0;
+  int sp_turn = 0;
+  double* d_sp_out = nullptr;       // host-pointer calls: the wanted entries
+  size_t sp_out_cap = 0;
+  std::vector<unsigned> sp_seen;    // [n] duplicate check of b's indices (stamps)
+  unsigned sp_seen_epoch = 0;
+  std::vector<char> sp_payload;
+  double sp_plan_ms = 0.0;          // host time of the last call's plan building
+  long long sp_work = 0, sp_reached[2] = {0, 0}, sp_entries[2] = {0, 0};   // the last call's counts (diagnostics)
+  int sparse_setup();
+  int sparse_stage(size_t need_out);
+  int sparse_sweeps(int nrhs, const SparseSide& F, const SparseSide& B, const SVRhs& r);
+  SparseSide sparse_full_side() const;
+  int solve_sparse_async(uint64_t nb, const uint64_t* b_index, const double* b_values, bool b_dev, uint64_t nx,
+                         const uint64_t* x_index, double* x_values, bool x_dev);
+  int inverse_entries(uint64_t nnz, const uint64_t* rows, const uint64_t* cols, double* out);
   DFFactor dff;
   int *d_dff_init = nullptr, *d_dff_cnt = nullptr;
   std::vector<DFTask> h_dff_tasks;

@@ -479,6 +479,115 @@ SolvePlan build_solve_plan(const Symbolic& S, const std::vector<int>& owner, int
   return P;
 }
 
+SolvePrune build_solve_prune(const Symbolic& S, const SolvePlan& full) {
+  SolvePrune X;
+  const int nsup = S.nsup;
+  X.col2sn.assign(S.n, 0);
+  for (int s = 0; s < nsup; s++)
+    for (int j = S.sn_first[s]; j < S.sn_first[s + 1]; j++) X.col2sn[j] = s;
+  X.cls.assign(nsup, -1);
+  for (int s : full.leaf1) X.cls[s] = 0;
+  for (int s : full.leafn) X.cls[s] = 1;
+  for (int s : full.leafw) X.cls[s] = 2;
+  for (int s = 0; s < nsup; s++)
+    if (full.front2task[s] >= 0) X.cls[s] = full.tasks[full.front2task[s]].kind == 0 ? 3 : 4;
+  X.f2t = full.front2task;
+  X.stamp.assign(nsup, 0);
+  X.ntf2t.assign(nsup, -1);
+  return X;
+}
+
+void build_pruned_plan(const Symbolic& S, const SolvePlan& full, SolvePrune& X, const int* cols, size_t k,
+                       PrunedPlan& P) {
+  P.reached.clear(); P.tasks.clear(); P.pend.clear(); P.fronts.clear(); P.f2t.clear();
+  P.leaf1.clear(); P.leafn.clear(); P.leafw.clear();
+  P.entries = 0; P.work = 0;
+  if (++X.epoch == 0) { std::fill(X.stamp.begin(), X.stamp.end(), 0u); X.epoch = 1; }   // once in 2^32 calls
+  const unsigned ep = X.epoch;
+  // upward closure: a walk stops at the first front already reached
+  for (size_t i = 0; i < k; i++) {
+    P.work++;
+    for (int s = X.col2sn[cols[i]]; s >= 0 && X.stamp[s] != ep; s = S.sn_parent[s]) {
+      X.stamp[s] = ep;
+      P.reached.push_back(s);
+      P.work++;
+    }
+  }
+  // queue order of the full plan: levels ascending, fronts ascending inside a level
+  std::sort(P.reached.begin(), P.reached.end(), [&](int a, int b) {
+    P.work++;
+    return S.sn_level[a] != S.sn_level[b] ? S.sn_level[a] < S.sn_level[b] : a < b;
+  });
+  const int per = SV_NT / 32;
+  const size_t r = P.reached.size();
+  // task indices, level by level: batches of the level's narrow fronts, then the wide fronts' task ranges
+  for (size_t i0 = 0; i0 < r;) {
+    size_t i1 = i0;
+    while (i1 < r && S.sn_level[P.reached[i1]] == S.sn_level[P.reached[i0]]) i1++;
+    int in_batch = 0;
+    for (size_t i = i0; i < i1; i++) {
+      const int s = P.reached[i];
+      P.entries += (long long)(S.sn_first[s + 1] - S.sn_first[s]) *
+                   (S.sn_first[s + 1] - S.sn_first[s] + S.sn_rowptr[s + 1] - S.sn_rowptr[s]);
+      P.work++;
+      switch (X.cls[s]) {
+        case 0: P.leaf1.push_back(s); break;
+        case 1: P.leafn.push_back(s); break;
+        case 2: P.leafw.push_back(s); break;
+        case 3:
+          if (in_batch == 0) {
+            SVTask t{};
+            t.kind = 0; t.s = (int)P.fronts.size(); t.cnt = 0; t.dep1 = -1; t.dep2 = -1; t.bowner = -1; t.ptask = -1; t.cuoff = -1;
+            P.tasks.push_back(t);
+          }
+          P.tasks.back().cnt++;
+          X.ntf2t[s] = (int)P.tasks.size() - 1;
+          P.fronts.push_back(s);
+          in_batch = in_batch + 1 == per ? 0 : in_batch + 1;
+          break;
+        default: break;
+      }
+    }
+    for (size_t i = i0; i < i1; i++) {
+      const int s = P.reached[i];
+      if (X.cls[s] != 4) continue;
+      const int h = X.f2t[s], nrt = full.tasks[h].nrt;
+      X.ntf2t[s] = (int)P.tasks.size();
+      P.tasks.insert(P.tasks.end(), full.tasks.begin() + h, full.tasks.begin() + h + 1 + nrt);
+      P.work += 1 + nrt;
+    }
+    i0 = i1;
+  }
+  // remapped index fields, counters and the (front, task) pairs
+  P.pend.assign(P.tasks.size(), 0);
+  for (size_t i = 0; i < r; i++) {
+    const int s = P.reached[i];
+    if (X.cls[s] < 3) continue;
+    const int p = S.sn_parent[s], nt = X.ntf2t[s];
+    P.f2t.push_back(s);
+    P.f2t.push_back(nt);
+    P.work++;
+    if (X.cls[s] == 3) { if (p >= 0) P.pend[X.ntf2t[p]]++; continue; }
+    const int h = X.f2t[s], nrt = full.tasks[h].nrt;
+    if (p >= 0 && full.tasks[h].notify) P.pend[X.ntf2t[p]]++;
+    for (int b = 0; b <= nrt; b++) {
+      SVTask& t = P.tasks[nt + b];
+      const SVTask& o = full.tasks[h + b];
+      t.ptask = p >= 0 ? X.ntf2t[p] : -1;
+      if (o.dep1 >= o.dep0) {                   // follows its chain child: remapped when reached, else dropped
+        const int c = full.tasks[o.dep0].s;
+        if (X.stamp[c] == ep) {
+          const int d = X.ntf2t[c] - X.f2t[c];
+          t.dep0 = o.dep0 + d; t.dep1 = o.dep1 + d; t.dep2 = o.dep2 >= 0 ? o.dep2 + d : o.dep2;
+        } else {
+          t.dep0 = 0; t.dep1 = -1; t.dep2 = -1;
+        }
+      }
+      P.work++;
+    }
+  }
+}
+
 // Selected inversion (k_selinv): the queue runs the levels from the root down, as the backward sweep does.  The
 // gather maps follow every front's rows up the tree: `cur` holds their positions in the current ancestor's front; the
 // rows that are pivots of that ancestor form the next segment (rows are ascending, so segments are contiguous and

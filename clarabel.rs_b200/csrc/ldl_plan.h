@@ -117,6 +117,38 @@ struct SolvePlan {
 // cap: doubles of the shared-memory slab of a sweep CTA
 SolvePlan build_solve_plan(const Symbolic& S, const std::vector<int>& owner, int rank, int cap);
 
+// Pruned solves (cldl_solve_sparse, cldl_inverse_entries).  The nonzeros of L^-1 b lie in the fronts of b's indices
+// and their ancestors, and the backward sweep needs only the fronts of the wanted entries and their ancestors: the
+// upward closure of an index set in sn_parent.  A pruned plan is the full solve plan restricted to such a closure:
+// a wide front keeps its full-plan tasks (same head / row split, same bslot), narrow fronts are regrouped into batches
+// of the reached fronts, the leaf lists are filtered, task indices are remapped in the level order of the full queue,
+// and waits on fronts outside the closure are dropped (pend counts reached non-chain children only; a chain child
+// outside the closure is not followed).  Fronts outside the closure contribute exact zeros.
+struct SolvePrune {                      // built once per handle from the full plan
+  std::vector<int> col2sn;               // [n] permuted column -> front
+  std::vector<signed char> cls;          // [nsup] 0 leaf1, 1 leafn, 2 leafw, 3 narrow batch, 4 wide tasks, -1 none
+  std::vector<int> f2t;                  // [nsup] the full plan's front2task
+  std::vector<unsigned> stamp;           // [nsup] closure marks: stamp[s] == epoch while the current closure holds s
+  unsigned epoch = 0;
+  std::vector<int> ntf2t;                // [nsup] scratch: the pruned plan's task of a reached front
+};
+SolvePrune build_solve_prune(const Symbolic& S, const SolvePlan& full);
+
+struct PrunedPlan {
+  std::vector<int> reached;              // the closure, in queue order (level, then front)
+  std::vector<SVTask> tasks;
+  std::vector<int> pend;                 // [tasks] forward: reached non-chain children with tasks
+  std::vector<int> fronts;               // narrow batches' fronts
+  std::vector<int> f2t;                  // (front, task) pairs of the reached fronts that have tasks
+  std::vector<int> leaf1, leafn, leafw;
+  long long entries = 0;                 // panel entries (ns + nr) ns of the reached fronts
+  long long work = 0;                    // host steps: closure visits, sort comparisons, records written
+};
+// the upward closure of the fronts of permuted columns cols[0, k) (cols may repeat), then its plan.  O(r log r) in the
+// r reached fronts plus O(k); nothing proportional to n or nsup.
+void build_pruned_plan(const Symbolic& S, const SolvePlan& full, SolvePrune& X, const int* cols, size_t k,
+                       PrunedPlan& P);
+
 // One task of k_selinv (48 bytes = 3 x int4), queued root to leaves.  kind 0: a whole front with at most SI_RB rows
 // (its rows, then its pivot block); 1: rows [r0, r1) of Z_RS of a front with more rows; 2: the pivot block Z_SS of
 // such a front, after all of its row tasks.  Kinds 0 and 1 wait for the parent front's Z, kind 2 for its row tasks.

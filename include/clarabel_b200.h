@@ -176,6 +176,43 @@ int cldl_schur_expand_dev(cldl_t *h, double *d_x, const double *d_xS);
  *   - Synchronises the handle's stream.  The first call allocates a few kilobytes of reduction workspace. */
 int cldl_logdet(cldl_t *h, double *logabsdet, int32_t *sign);
 
+/* Sparse right-hand sides and selected solution entries: x = (K + E)^-1 b with b given by nb (index, value) pairs
+ * (b_index NULL: b_values is dense, n doubles, and nb must be n) and x wanted at nx caller indices (x_index NULL: all
+ * n, x_values n doubles, and nx must be n).  E is the refactor's dynamic regularisation, as for cldl_logdet.  The
+ * solve is pruned to the assembly tree: the forward sweep visits only the fronts of b's indices and their ancestors
+ * (the nonzeros of L^-1 b), the backward sweep only the fronts of the wanted indices and their ancestors.  Each front
+ * it visits does the arithmetic cldl_solve does there, so the entries returned compare equal (==) to the same entries
+ * of cldl_solve on the densified b.  Index lists stay on the host: the plan of a call is built there, in time
+ * O(r log r) in the r fronts it reaches plus the lengths of the index lists.
+ *   - Valid after a refactor that returned 1; otherwise CLDL_E_NOT_FACTORED.
+ *   - CLDL_E_ARG on a Schur or sharded handle, for an index >= n, for a duplicate index in b_index, and for a NULL
+ *     array that is needed.  Duplicates in x_index are allowed.  nb = 0 gives zeros.
+ *   - The first call allocates counters and marks like the full solve's (about 4 (2 ntask + 6 nsup) bytes plus the
+ *     backward partial sums) and keeps the host prune index (about 4 n + 13 nsup bytes); each call may grow a device
+ *     buffer and two pinned buffers for its plan and index lists.  cldl_destroy frees them.
+ *   - The factor, D, 1/D and every later cldl_solve are left bit for bit unchanged; cldl_solve keeps its launch
+ *     sequence.  No floating-point atomics: repeated calls give the same bits.
+ * cldl_solve_sparse reads and writes host buffers and synchronises.  The _dev form takes b_values / x_values in
+ * device memory (the index lists on the host) and is only enqueued on the handle's stream; it waits on the host only
+ * for the copy out of the pinned buffer it reuses (two calls back) and when a buffer grows. */
+int cldl_solve_sparse(cldl_t *h, uint64_t nb, const uint64_t *b_index, const double *b_values,
+                      uint64_t nx, const uint64_t *x_index, double *x_values);
+int cldl_solve_sparse_dev(cldl_t *h, uint64_t nb, const uint64_t *b_index, const double *d_b_values,
+                          uint64_t nx, const uint64_t *x_index, double *d_x_values);   /* indices on the host */
+
+/* Entries of the inverse anywhere: out[k] = ((K + E)^-1)[rows[k], cols[k]] for nnz positions, not only K's pattern
+ * (host arrays).  The positions are grouped by column; two columns at a time are solved in one pair of sweeps
+ * (the two-right-hand-side sweeps) pruned to the union of their forward closures and of their wanted rows' closures,
+ * and each column's rows are gathered.  out[k] compares equal to cldl_solve(e_cols[k])[rows[k]].  Validity, refusals
+ * (an index >= n), regularisation and what stays unchanged as for cldl_solve_sparse.  Synchronises the handle's
+ * stream. */
+int cldl_inverse_entries(cldl_t *h, uint64_t nnz, const uint64_t *rows, const uint64_t *cols, double *out);
+
+/* Diagnostics of the last cldl_solve_sparse(_dev) / cldl_inverse_entries call: host milliseconds spent building its
+ * plans, fronts reached forward and backward, panel entries ((ns + nr) ns per front) of those fronts forward and
+ * backward, and the host steps the plan building took (summed over the column pairs of cldl_inverse_entries). */
+int cldl_sparse_stats(const cldl_t *h, double *out6);
+
 /* Adjoint solve: the adjoint of x = K^-1 b.  For an output gradient g (n doubles):
  *     gb = (K + E)^-1 g
  * and, when gvals is not NULL, the gradient of <g, x> with respect to the stored values of the upper triangle passed

@@ -191,6 +191,7 @@ EXPORTED_SYMBOLS = [
     "cldl_logdet", "cldl_adjoint_solve", "cldl_adjoint_solve_dev",
     "cldl_default_refine_opts", "cldl_solve_refined", "cldl_solve_refined_dev", "cldl_refine_abi_sizes",
     "cldl_solve_sparse", "cldl_solve_sparse_dev", "cldl_inverse_entries", "cldl_sparse_stats",
+    "cldl_set_null_pivot_tol", "cldl_null_pivots", "cldl_inertia", "cldl_null_space", "cldl_null_space_dev",
 ]
 
 
@@ -308,10 +309,11 @@ class CudaLDLSolver:
     def __init__(self, n, colptr, rowval, nzval, dsigns, *, perm=None,
                  regularize_eps=1e-13, regularize_delta=2e-7, regularize_enable=True,
                  amd_dense_scale=1.5, ordering=ORDER_BEST, device=0, max_panel=0, nd_leaf=0,
-                 shard_nranks=0, shard_rank=0, schur=None):
+                 shard_nranks=0, shard_rank=0, schur=None, null_pivot_tol=0.0):
         """``schur``: a Schur set (caller indices, in the order the complement's rows and columns take) makes a Schur
         complement handle: ``refactor()`` factors the other indices only, and ``schur_complement()``,
-        ``schur_reduce()`` and ``schur_expand()`` replace ``solve()`` (see cldl_create_schur)."""
+        ``schur_reduce()`` and ``schur_expand()`` replace ``solve()`` (see cldl_create_schur).
+        ``null_pivot_tol`` > 0 calls ``set_null_pivot_tol()`` after the handle is created."""
         L = lib()
         self._L = L
         self.n = int(n)
@@ -348,6 +350,8 @@ class CudaLDLSolver:
             self.nschur = int(si.size)
         self._h = h
         self._pattern = (cp, rv)
+        if null_pivot_tol:
+            self.set_null_pivot_tol(null_pivot_tol)
 
     def close(self):
         if getattr(self, "_h", None):
@@ -499,14 +503,72 @@ class CudaLDLSolver:
     def slogdet(self):
         """(sign, logabsdet) of K + E, the matrix the last ``refactor()`` factored (E its dynamic regularisation), from
         the factor's pivots: logabsdet = sum log|d_k|, sign = (-1)^(negative pivots).  On a Schur handle, of
-        K_BB + E_B.  BackendError (NotFactored) before a refactor that returned True, (BadArgument) on a sharded
-        handle (see cldl_logdet)."""
+        K_BB + E_B.  (0, -inf) when the refactor found null pivots (see set_null_pivot_tol).  BackendError
+        (NotFactored) before a refactor that returned True, (BadArgument) on a sharded handle (see cldl_logdet)."""
         f = self._L.cldl_logdet
         f.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_int32)]
         f.restype = C.c_int
         ld, sg = C.c_double(), C.c_int32()
         _check(f(self._h, C.byref(ld), C.byref(sg)), "logdet")
         return int(sg.value), float(ld.value)
+
+    def set_null_pivot_tol(self, tol):
+        """From the next ``refactor()`` on, a pivot with |d| <= tol (absolute) is a null pivot: stored as D = 1/D = 0,
+        its column of L zero, counted by ``inertia()`` and listed by ``null_pivots()``; solves then use the generalised
+        inverse P^T L^-T D^+ L^-1 P and ``slogdet()`` is (0, -inf).  0 turns it off.  Meant for semidefinite matrices
+        (see cldl_set_null_pivot_tol).  BackendError (BadArgument) for tol < 0 or NaN and on Schur and sharded
+        handles."""
+        f = self._L.cldl_set_null_pivot_tol
+        f.argtypes = [C.c_void_p, C.c_double]
+        f.restype = C.c_int
+        _check(f(self._h, float(tol)), "set_null_pivot_tol")
+
+    def null_pivots(self):
+        """caller indices of the last refactor's null pivots, in elimination order (int64 array).  BackendError
+        (NotFactored) before a refactor that returned True."""
+        f = self._L.cldl_null_pivots
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
+        f.restype = C.c_int
+        cnt = C.c_uint64()
+        _check(f(self._h, C.byref(cnt), None), "null_pivots")
+        out = np.empty(cnt.value, np.uint64)
+        _check(f(self._h, C.byref(cnt), _p(out, C.c_uint64)), "null_pivots")
+        return out.astype(np.int64)
+
+    def inertia(self):
+        """(n+, n-, n0) of the last refactor: positive, negative and null pivots (cldl_inertia)"""
+        f = self._L.cldl_inertia
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        f.restype = C.c_int
+        v = np.zeros(3, np.uint64)
+        _check(f(self._h, _p(v, C.c_uint64)), "inertia")
+        return int(v[0]), int(v[1]), int(v[2])
+
+    def null_space(self, orthonormalize=False):
+        """(V, resid): V (n x r) spans the null space of the factored matrix, r the number of null pivots.  Column k is
+        P^T L^-T e_{p_k}, exactly 1 at the k-th null pivot's caller index; resid[k] = ||K v_k||_inf / (||K||_inf
+        ||v_k||_inf) with K the handle's current values.  ``orthonormalize``: V replaced by the Q of its QR (on the
+        host; resid stays that of the unorthonormalised columns).  Synchronises (see cldl_null_space)."""
+        f = self._L.cldl_null_space
+        f.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        r = self.null_pivots().size
+        V = np.empty((self.n, r), np.float64, order="F")
+        resid = np.empty(r, np.float64)
+        _check(f(self._h, r, _p(V, C.c_double), _p(resid, C.c_double)), "null_space")
+        if orthonormalize and r:
+            V = np.linalg.qr(V)[0]
+        return V, resid
+
+    def null_space_dev(self, r, d_V_ptr):
+        """``null_space`` into device memory (n x r doubles, column-major, at d_V_ptr); returns resid.
+        Synchronises."""
+        f = self._L.cldl_null_space_dev
+        f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        resid = np.empty(int(r), np.float64)
+        _check(f(self._h, int(r), C.c_void_p(d_V_ptr), _p(resid, C.c_double)), "null_space_dev")
+        return resid
 
     def adjoint_solve(self, g, x):
         """The adjoint of x = K^-1 b for an output gradient g: (gb, gvals) with gb = (K + E)^-1 g (n values) and gvals

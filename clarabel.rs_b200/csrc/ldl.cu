@@ -146,22 +146,27 @@ __global__ void __launch_bounds__(NT) k_factor_level(LDLDev d, int task_base, in
   for (long long e = d.asm_ptr[s] + tid; e < d.asm_ptr[s + 1]; e += NT)
     W[d.asm_dst[e]] = d.vals[d.asm_src[e]];
 
-  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0;
+  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0, c_null = 0;
   for (int j = 0; j < ns; j++) {
     __syncthreads();    // column j is final: assembled, and updated by every earlier pivot
     const double* __restrict__ cj = W + (long long)j * ld;
     double dj = cj[j];
     bool reg = false;
-    if (d.reg_enable) {
+    // a null pivot (cldl_set_null_pivot_tol) is taken as infinite: D = 1/D = 0, before the sign test (the same at the
+    // other three pivot sites: k_factor_leaf1, dff_small, dff_diag)
+    const bool nul = d.null_tol > 0.0 && fabs(dj) <= d.null_tol;
+    if (nul) dj = 0.0;
+    else if (d.reg_enable) {
       const double sg = (double)d.dsigns[f + j];
       if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; reg = true; }
     }
-    const double inv = 1.0 / dj;
+    const double inv = nul ? 0.0 : 1.0 / dj;
     if (tid == 0) {
       c_reg += reg ? 1 : 0;
       c_pos += dj > 0.0 ? 1 : 0;
-      if (dj == 0.0) c_zero = 1;
+      if (dj == 0.0 && !nul) c_zero = 1;
       if (!isfinite(inv)) c_nonf = 1;
+      if (nul) { c_null++; d.nullmark[f + j] = 1; }
       d.D[f + j] = dj;
       d.Dinv[f + j] = inv;
       sD[j] = dj;
@@ -183,6 +188,7 @@ __global__ void __launch_bounds__(NT) k_factor_level(LDLDev d, int task_base, in
   if (tid == 0) {
     if (c_reg) atomicAdd(&d.status[ST_REGCOUNT], c_reg);
     if (c_pos) atomicAdd(&d.status[ST_POSINERTIA], c_pos);
+    if (c_null) atomicAdd(&d.status[ST_NULLCOUNT], c_null);
     if (c_zero) atomicExch(&d.status[ST_ZEROPIV], 1);
     if (c_nonf) atomicExch(&d.status[ST_NONFINITE], 1);
   }
@@ -231,10 +237,10 @@ __global__ void __launch_bounds__(NT) k_factor_level(LDLDev d, int task_base, in
 static_assert(LEAF1_MAXLD > CB_BIG_NR, "a level-0 column must fit the per-warp buffer");
 __global__ void __launch_bounds__(LEAF1_NT) k_factor_leaf1(LDLDev d, int task_base, int count) {
   __shared__ double s_col[LEAF1_NT / 32][LEAF1_MAXLD];
-  __shared__ int s_pos, s_reg;
+  __shared__ int s_pos, s_reg, s_null;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int i = blockIdx.x * (LEAF1_NT / 32) + warp;
-  if (threadIdx.x == 0) { s_pos = 0; s_reg = 0; }
+  if (threadIdx.x == 0) { s_pos = 0; s_reg = 0; s_null = 0; }
   __syncthreads();
   if (i < count) {
     double* col = s_col[warp];
@@ -251,16 +257,19 @@ __global__ void __launch_bounds__(LEAF1_NT) k_factor_leaf1(LDLDev d, int task_ba
     __syncwarp();
     double dj = col[0];
     bool reg = false;
-    if (d.reg_enable) {
+    const bool nul = d.null_tol > 0.0 && fabs(dj) <= d.null_tol;
+    if (nul) dj = 0.0;
+    else if (d.reg_enable) {
       const double sg = (double)d.dsigns[f];
       if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; reg = true; }
     }
-    const double inv = 1.0 / dj;
+    const double inv = nul ? 0.0 : 1.0 / dj;
     if (lane == 0) {
-      if (dj == 0.0) atomicExch(&d.status[ST_ZEROPIV], 1);
+      if (dj == 0.0 && !nul) atomicExch(&d.status[ST_ZEROPIV], 1);
       if (!isfinite(inv)) atomicExch(&d.status[ST_NONFINITE], 1);
       if (dj > 0.0) atomicAdd(&s_pos, 1);
       if (reg) atomicAdd(&s_reg, 1);
+      if (nul) { atomicAdd(&s_null, 1); d.nullmark[f] = 1; }
       d.D[f] = dj;
       d.Dinv[f] = inv;
     }
@@ -285,6 +294,7 @@ __global__ void __launch_bounds__(LEAF1_NT) k_factor_leaf1(LDLDev d, int task_ba
   if (threadIdx.x == 0) {
     if (s_pos) atomicAdd(&d.status[ST_POSINERTIA], s_pos);
     if (s_reg) atomicAdd(&d.status[ST_REGCOUNT], s_reg);
+    if (s_null) atomicAdd(&d.status[ST_NULLCOUNT], s_null);
   }
 }
 
@@ -410,17 +420,19 @@ __device__ void dff_small(const LDLDev& d, int s, double* sm, int* s_flag) {
     }
     __syncthreads();
   }
-  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0;
+  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0, c_null = 0;
   for (int j = 0; j < ns; j++) {
     if (tid == 0) {
       double dj = W[(long long)j * ld + j];
-      if (d.reg_enable) {
+      const bool nul = d.null_tol > 0.0 && fabs(dj) <= d.null_tol;
+      if (nul) { dj = 0.0; c_null++; d.nullmark[f + j] = 1; }
+      else if (d.reg_enable) {
         const double sg = (double)d.dsigns[f + j];
         if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; c_reg++; }
       }
-      if (dj == 0.0) c_zero = 1;
+      if (dj == 0.0 && !nul) c_zero = 1;
       if (dj > 0.0) c_pos++;
-      const double inv = 1.0 / dj;
+      const double inv = nul ? 0.0 : 1.0 / dj;
       if (!isfinite(inv)) c_nonf = 1;
       d.D[f + j] = dj;
       d.Dinv[f + j] = inv;
@@ -444,6 +456,7 @@ __device__ void dff_small(const LDLDev& d, int s, double* sm, int* s_flag) {
   if (tid == 0) {
     if (c_reg) atomicAdd(&d.status[ST_REGCOUNT], c_reg);
     if (c_pos) atomicAdd(&d.status[ST_POSINERTIA], c_pos);
+    if (c_null) atomicAdd(&d.status[ST_NULLCOUNT], c_null);
     if (c_zero) atomicExch(&d.status[ST_ZEROPIV], 1);
     if (c_nonf) atomicExch(&d.status[ST_NONFINITE], 1);
   }
@@ -673,7 +686,7 @@ __device__ void dff_diag(const LDLDev& d, const DFFactor& q, const DFTask& tk, d
   for (int k = 0; k < 4; k++)
 #pragma unroll
     for (int i = 0; i < 4; i++) a[i][k] = active ? sA[(4 * bj + k) * CB_PB_LD + 4 * bi + i] : 0.0;
-  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0;
+  int c_reg = 0, c_pos = 0, c_zero = 0, c_nonf = 0, c_null = 0;
   const int nJ = (ns + 3) >> 2;
   for (int J = 0; J < nJ; J++) {
 #pragma unroll
@@ -684,13 +697,15 @@ __device__ void dff_diag(const LDLDev& d, const DFFactor& q, const DFTask& tk, d
       if (bj == J && active) {
         if (bi == J) {
           double dj = a[jj][jj];
-          if (d.reg_enable) {
+          const bool nul = d.null_tol > 0.0 && fabs(dj) <= d.null_tol;
+          if (nul) { dj = 0.0; c_null++; d.nullmark[f + j] = 1; }
+          else if (d.reg_enable) {
             const double sg = sSign[j];
             if (dj * sg < d.reg_eps) { dj = d.reg_delta * sg; c_reg++; }
           }
-          if (dj == 0.0) c_zero = 1;
+          if (dj == 0.0 && !nul) c_zero = 1;
           if (dj > 0.0) c_pos++;
-          const double inv = __drcp_rn(dj);
+          const double inv = nul ? 0.0 : __drcp_rn(dj);
           if (!isfinite(inv)) c_nonf = 1;
           a[jj][jj] = dj;
           buf[64] = dj;
@@ -730,6 +745,7 @@ __device__ void dff_diag(const LDLDev& d, const DFFactor& q, const DFTask& tk, d
   }
   if (c_reg) atomicAdd(&d.status[ST_REGCOUNT], c_reg);
   if (c_pos) atomicAdd(&d.status[ST_POSINERTIA], c_pos);
+  if (c_null) atomicAdd(&d.status[ST_NULLCOUNT], c_null);
   if (c_zero) atomicExch(&d.status[ST_ZEROPIV], 1);
   if (c_nonf) atomicExch(&d.status[ST_NONFINITE], 1);
 #pragma unroll
@@ -1336,6 +1352,7 @@ void LDLObject::release() {
 // plain launches of `plan`
 int LDLObject::refactor_level0() {
   CK(cudaMemsetAsync(dev.status, 0, ST_COUNT * sizeof(int), stream));
+  if (dev.null_tol > 0.0) CK(cudaMemsetAsync(dev.nullmark, 0, (size_t)n, stream));
   CK(cudaMemcpyAsync(d_dff_cnt, d_dff_init, dff_nsup4 * sizeof(int), cudaMemcpyDeviceToDevice, stream));
   CK(cudaMemsetAsync(dff.qhead, 0, sizeof(int), stream));
   g_launches += plan.size();
@@ -1414,10 +1431,11 @@ int LDLObject::selected_inverse_async(double* d_out) {
 }
 
 // log|det(K + E)| as one deterministic sum of log|d_k| over the factored pivots (B's alone on a Schur handle); the sign
-// from the negative-pivot count the refactor collected
+// from the negative-pivot count the refactor collected.  A factor with null pivots is singular: sign 0, -inf.
 int LDLObject::logdet(double* logabsdet, int32_t* sign) {
   if (sharded()) return CLDL_E_ARG;
   if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if (null_count) { *logabsdet = -INFINITY; *sign = 0; return CLDL_OK; }
   CK(cudaSetDevice(device));
   if (!d_ld_ws) {
     const size_t mk = own.mark();
@@ -1656,6 +1674,116 @@ int LDLObject::solve_refined(double* d_x, const double* d_b, const cldl_refine_o
   return CLDL_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------
+// Null pivots (cldl_set_null_pivot_tol, cldl_null_pivots, cldl_null_space).  A pivot with |d| <= null_tol is taken as
+// infinite: D = 1/D = 0, so the factorisation scales its column below the pivot by 0 and the Schur updates add nothing
+// from it.  The factored model is K with that pivot's row and column of the Schur complement dropped; its generalised
+// inverse P^T L^-T D^+ L^-1 P is what the solves compute, with D^+ = 1/D (0 at the null pivots), and its null space is
+// spanned by P^T L^-T e_p over the null pivots p: K P^T L^-T e_p = P^T L D e_p = 0.
+
+int LDLObject::set_null_tol(double tol) {
+  if (sharded() || schur || !(tol >= 0.0)) return CLDL_E_ARG;
+  if (tol > 0.0 && !dev.nullmark) {
+    CK(cudaSetDevice(device));
+    CK(own.alloc(&dev.nullmark, (size_t)n));
+  }
+  dev.null_tol = tol;
+  return CLDL_OK;
+}
+
+int LDLObject::null_positions(std::vector<int>& pos) {
+  pos.clear();
+  if (!null_count) return CLDL_OK;
+  std::vector<unsigned char> mark((size_t)n);
+  CK(cudaSetDevice(device));
+  CK(cudaMemcpyAsync(mark.data(), dev.nullmark, (size_t)n, cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));
+  for (int k = 0; k < n; k++) if (mark[k]) pos.push_back(k);
+  return pos.size() == null_count ? CLDL_OK : CLDL_E_CUDA;
+}
+
+// Column k of V: the backward sweeps of the solve, unchanged, with y = e_{p_k} and 1/D read from an array of ones, so
+// that they compute x = L^-T y (instead of L^-T D^-1 y), permuted out into the caller's order.  Two columns per pair
+// of sweeps.  resid[k] = ||K v_k||_inf / (||K||_inf ||v_k||_inf) with K the current values, from k_refine_residual at
+// b = 0.
+int LDLObject::null_space(uint64_t r, double* V, bool v_dev, double* resid) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if (r != null_count || (r && !V)) return CLDL_E_ARG;
+  if (resid && 2 * nnzA - n > 0x7fffffff) return CLDL_E_ARG;
+  if (r == 0) return CLDL_OK;
+  CK(cudaSetDevice(device));
+  std::vector<int> pos;
+  if (int rc = null_positions(pos)) return rc;
+  const int nn = n;
+  if (!d_ns_ones) {
+    const size_t mk = own.mark();
+    if (own.alloc(&d_ns_ones, (size_t)n) != cudaSuccess) { own.release_since(mk); d_ns_ones = nullptr; return CLDL_E_CUDA; }
+    double* ones = d_ns_ones;
+    g_launches++;
+    k_map<<<(n + 255) / 256, 256, 0, stream>>>(nn, [=] __device__(int i) { ones[i] = 1.0; });
+  }
+  if (resid && !d_rf_work) {
+    const size_t mk = own.mark();
+    if (int rc = refine_setup()) { own.release_since(mk); d_rf_work = nullptr; return rc; }
+  }
+  if (resid && 2 * r + 1 > ns_stat_cap) {
+    own.free(d_ns_stat);
+    d_ns_stat = nullptr;
+    ns_stat_cap = 0;
+    CK(own.alloc(&d_ns_stat, 2 * (size_t)r + 1));
+    ns_stat_cap = 2 * (size_t)r + 1;
+  }
+  double *st = d_ns_stat, *zero = nullptr, *res = nullptr, *rsum = nullptr, *kx = nullptr, *rmax = nullptr;
+  if (resid) {
+    zero = d_rf_work; res = zero + (size_t)n; rsum = zero + 2 * (size_t)n; kx = zero + 3 * (size_t)n; rmax = zero + 4 * (size_t)n;
+    CK(cudaMemsetAsync(st, 0, (2 * r + 1) * sizeof(double), stream));
+    CK(cudaMemsetAsync(zero, 0, (size_t)n * sizeof(double), stream));
+  }
+  const size_t bytes = (size_t)n * sizeof(double);
+  for (uint64_t k = 0; k < r; k += 2) {
+    const int nrhs = k + 1 < r ? 2 : 1;
+    SVRhs rr;
+    rr.xp[0] = d_xp; rr.u[0] = dev.u; rr.out[0] = v_dev ? V + k * (size_t)n : d_bx;
+    rr.xp[1] = nrhs == 2 ? d_xp2 : d_xp; rr.u[1] = nrhs == 2 ? d_u2 : dev.u;
+    rr.out[1] = nrhs == 2 ? (v_dev ? V + (k + 1) * (size_t)n : d_bx + n) : rr.out[0];
+    for (int h = 0; h < nrhs; h++) {
+      double* xp = rr.xp[h];
+      const int p = pos[k + h];
+      CK(cudaMemsetAsync(xp, 0, bytes, stream));
+      g_launches++;
+      k_map<<<1, 32, 0, stream>>>(1, [=] __device__(int) { xp[p] = 1.0; });
+    }
+    if (int rc = sv_reset()) return rc;
+    double* const dinv = dev.Dinv;
+    dev.Dinv = d_ns_ones;                 // the launches below take their own copy of dev
+    sv_sweep(false, nrhs, sv, rr);
+    sv_leaves(false, nrhs, rr, sv_leaf_lists());
+    dev.Dinv = dinv;
+    for (int h = 0; resid && h < nrhs; h++) {
+      const double* v = rr.out[h];
+      double* sk = st + 2 * (k + h);
+      const bool first = k == 0 && h == 0;
+      g_launches += first ? 4 : 3;
+      k_refine_residual<<<(unsigned)((n + RF_NT / 32 - 1) / (RF_NT / 32)), RF_NT, 0, stream>>>(
+          n, d_rf_rowptr, d_rf_col, d_rf_src, dev.vals, v, zero, res, kx, rmax, first ? rsum : nullptr);
+      k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return v[i]; }, sk);
+      k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return res[i]; }, sk + 1);
+      if (first) k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return rsum[i]; }, st + 2 * r);
+    }
+    CK(cudaGetLastError());
+    if (!v_dev) CK(cudaMemcpyAsync(V + k * (size_t)n, d_bx, (size_t)nrhs * bytes, cudaMemcpyDeviceToHost, stream));
+  }
+  std::vector<double> h((size_t)(2 * r + 1), 0.0);
+  if (resid) CK(cudaMemcpyAsync(h.data(), st, h.size() * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));
+  for (uint64_t k = 0; resid && k < r; k++) {
+    const double num = h[2 * k + 1];
+    resid[k] = num == 0.0 ? 0.0 : num / (h[2 * r] * h[2 * k]);
+  }
+  return CLDL_OK;
+}
+
 // the Schur plan (ldl_plan.cpp) uploaded and the complement allocated, at the end of init
 int LDLObject::schur_setup(const SolvePlan& sp) {
   const SchurPlan p = build_schur_plan(S, schur_set, sp);
@@ -1729,6 +1857,7 @@ int LDLObject::sync_status() {
   CK(cudaStreamSynchronize(stream));
   regularize_count = (uint64_t)h_status[ST_REGCOUNT];
   positive_inertia = (uint64_t)h_status[ST_POSINERTIA];
+  null_count = (uint64_t)h_status[ST_NULLCOUNT];
   if (dff.trace) {  // diagnostic: CB_DF_TRACE=<file> dumps the last refactor's task timeline
     std::vector<unsigned long long> tr((size_t)dff.ntask * 10);
     CK(cudaMemcpy(tr.data(), dff.trace, tr.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
@@ -2565,6 +2694,41 @@ int cldl_selected_inverse_dev(cldl_t* h, double* d_nzval_out) {
 int cldl_logdet(cldl_t* h, double* logabsdet, int32_t* sign) {
   if (!h || !logabsdet || !sign) return CLDL_E_ARG;
   return h->obj.logdet(logabsdet, sign);
+}
+
+int cldl_set_null_pivot_tol(cldl_t* h, double tol) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.set_null_tol(tol);
+}
+int cldl_null_pivots(cldl_t* h, uint64_t* count, uint64_t* index_out) {
+  if (!h || !count) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  std::vector<int> pos;
+  if (int rc = o.null_positions(pos)) return rc;
+  *count = (uint64_t)pos.size();
+  if (index_out)
+    for (size_t k = 0; k < pos.size(); k++) index_out[k] = (uint64_t)o.S.perm[pos[k]];
+  return CLDL_OK;
+}
+int cldl_inertia(const cldl_t* h, uint64_t out3[3]) {
+  if (!h || !out3) return CLDL_E_ARG;
+  const LDLObject& o = h->obj;
+  if (o.sharded()) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  const uint64_t nf = (uint64_t)(o.schur ? o.schur_first : o.n);
+  out3[0] = o.positive_inertia;
+  out3[1] = nf - o.positive_inertia - o.null_count;
+  out3[2] = o.null_count;
+  return CLDL_OK;
+}
+int cldl_null_space(cldl_t* h, uint64_t r, double* V, double* resid) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.null_space(r, V, false, resid);
+}
+int cldl_null_space_dev(cldl_t* h, uint64_t r, double* d_V, double* resid) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.null_space(r, d_V, true, resid);
 }
 
 int cldl_solve_sparse(cldl_t* h, uint64_t nb, const uint64_t* b_index, const double* b_values,

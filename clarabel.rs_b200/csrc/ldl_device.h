@@ -20,7 +20,7 @@ namespace cb {
 
 struct ncclComm;   // NCCL's communicator, opaque (ldl.cu loads NCCL with dlopen)
 
-enum { ST_REGCOUNT = 0, ST_ZEROPIV = 1, ST_POSINERTIA = 2, ST_NONFINITE = 3, ST_COUNT = 8 };
+enum { ST_REGCOUNT = 0, ST_ZEROPIV = 1, ST_POSINERTIA = 2, ST_NONFINITE = 3, ST_NULLCOUNT = 4, ST_COUNT = 8 };
 
 // Plain-pointer bundle passed by value to kernels.
 struct LDLDev {
@@ -53,6 +53,10 @@ struct LDLDev {
   int* status = nullptr;
   double reg_eps = 1e-13, reg_delta = 2e-7;
   int reg_enable = 1;
+  // null pivots (cldl_set_null_pivot_tol): a pivot with |d| <= null_tol is stored as D = 1/D = 0 and marked; 0 = off.
+  // Last in the struct, so that the kernels that never read them keep their parameter offsets.
+  double null_tol = 0.0;
+  unsigned char* nullmark = nullptr;    // [n] permuted order, 1 at the null pivots; cleared by every refactor with null_tol > 0
 };
 
 // dataflow factorisation plan (see k_factor_df in ldl.cu)
@@ -176,6 +180,15 @@ class LDLObject {
   bool factored = false;
   bool factor_ok = false;                // the last refactor's status was collected and it returned 1
   uint64_t regularize_count = 0, positive_inertia = 0;
+  // null pivots (cldl_set_null_pivot_tol, cldl_null_pivots, cldl_null_space): dev.null_tol / dev.nullmark, the last
+  // refactor's count, and the null-space sweeps' 1/D (ones) and scalars, allocated by their first call
+  uint64_t null_count = 0;
+  double* d_ns_ones = nullptr;           // [n]
+  double* d_ns_stat = nullptr;           // [2 r + 1]: ||v_k||_inf, ||K v_k||_inf per column, then ||K||_inf
+  size_t ns_stat_cap = 0;
+  int set_null_tol(double tol);
+  int null_positions(std::vector<int>& pos);   // the null pivots' permuted positions, ascending (synchronises)
+  int null_space(uint64_t r, double* V, bool v_dev, double* resid);
   // selected inversion: plan, Z panels and counters, allocated by the first call
   SIPlan si;
   long long* d_si_pos = nullptr;         // [nnzA] caller entry -> offset in si.Z

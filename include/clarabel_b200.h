@@ -208,6 +208,43 @@ int cldl_solve_sparse_dev(cldl_t *h, uint64_t nb, const uint64_t *b_index, const
  * stream. */
 int cldl_inverse_entries(cldl_t *h, uint64_t nnz, const uint64_t *rows, const uint64_t *cols, double *out);
 
+/* Null pivots: rank detection, inertia with zeros, solves of singular systems and a null-space basis (MUMPS ICNTL(24) /
+ * CNTL(3), INFOG(28), ICNTL(25)).
+ *   - cldl_set_null_pivot_tol: from the next refactor on, a pivot with |d| <= tol (absolute) is a null pivot.  It is
+ *     taken as infinite: D = 1/D = 0 is stored, its column of L below the pivot is 0 and it updates no later pivot.
+ *     It is tested before the sign test and the regularisation, counts neither in regularize_count nor in
+ *     positive_inertia, and is not a zero pivot (no CLDL_E_ZERO_PIVOT): the refactor returns 1 when every other
+ *     reciprocal pivot is finite.  tol = 0 turns the test off (the default; the factor is then bit for bit the one of a
+ *     handle that never called this).  CLDL_E_ARG for tol < 0 or NaN, and on Schur and sharded handles.  The first
+ *     tol > 0 allocates n bytes of marks.
+ *   - cldl_null_pivots: the number of null pivots of the last refactor and, when index_out is not NULL, their caller
+ *     indices in elimination order.  Synchronises.
+ *   - cldl_inertia: (n+, n-, n0) of the last refactor: pivots > 0, < 0 and null (n0 = 0 with the test off).  On a Schur
+ *     handle, of B's pivots.  CLDL_E_ARG on a sharded handle.
+ *   - cldl_null_space: V (n x r, column-major, caller's order) with r the null count (else CLDL_E_ARG).  Column k is
+ *     P^T L^-T e_{p_k} for the k-th null pivot p_k: it is exactly 1 at that pivot's caller index, and
+ *     K v = P^T L D e_{p_k} = 0 for the factored matrix.  It is computed by the solve's backward sweeps with 1/D replaced
+ *     by ones, two columns per pair of sweeps.  resid (r doubles, may be NULL) gets ||K v_k||_inf / (||K||_inf
+ *     ||v_k||_inf) with K the handle's current values: this tells whether the pivots found span a null space of K.
+ *     The first call with resid sets up what cldl_solve_refined sets up, and CLDL_E_ARG is returned when that set-up
+ *     is refused.  Both forms synchronise; cldl_null_space_dev writes V to device memory, resid stays on the host.
+ * All three need a refactor that returned 1, else CLDL_E_NOT_FACTORED.
+ * With n0 > 0 every solve-type call (cldl_solve(_dev), cldl_solve_sparse(_dev), cldl_inverse_entries,
+ * cldl_selected_inverse(_dev), cldl_adjoint_solve(_dev), cldl_solve_refined(_dev)) uses the generalised inverse
+ *     K^- = P^T L^-T D^+ L^-1 P,   D^+ = 1/D with 0 at the null pivots,
+ * which solves K x = b for a compatible b.  cldl_logdet returns sign 0 and logabsdet = -inf.
+ * Scope: the test reads the pivot alone (static pivoting, no interchanges).  It finds the rank when each null pivot's
+ * column of the Schur complement is as small as the pivot, which always holds for a semidefinite K
+ * (|s_ik|^2 <= s_ii s_kk): the feature is meant for semidefinite matrices (graph Laplacians, floating finite-element
+ * subdomains, duplicated variables).  On an indefinite (quasidefinite) matrix a zero pivot with a large column, such as
+ * a constraint row eliminated first, is what regularisation is for; declaring it null drops that column, and resid
+ * shows it. */
+int cldl_set_null_pivot_tol(cldl_t *h, double tol);
+int cldl_null_pivots(cldl_t *h, uint64_t *count, uint64_t *index_out /* NULL: count only */);
+int cldl_inertia(const cldl_t *h, uint64_t out3[3]);
+int cldl_null_space(cldl_t *h, uint64_t r, double *V, double *resid);
+int cldl_null_space_dev(cldl_t *h, uint64_t r, double *d_V, double *resid);
+
 /* Diagnostics of the last cldl_solve_sparse(_dev) / cldl_inverse_entries call: host milliseconds spent building its
  * plans, fronts reached forward and backward, panel entries ((ns + nr) ns per front) of those fronts forward and
  * backward, and the host steps the plan building took (summed over the column pairs of cldl_inverse_entries). */

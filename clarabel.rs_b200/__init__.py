@@ -192,6 +192,7 @@ EXPORTED_SYMBOLS = [
     "cldl_default_refine_opts", "cldl_solve_refined", "cldl_solve_refined_dev", "cldl_refine_abi_sizes",
     "cldl_solve_sparse", "cldl_solve_sparse_dev", "cldl_inverse_entries", "cldl_sparse_stats",
     "cldl_set_null_pivot_tol", "cldl_null_pivots", "cldl_inertia", "cldl_null_space", "cldl_null_space_dev",
+    "cldl_updown", "cldl_updown_dev", "cldl_updown_stats",
 ]
 
 
@@ -499,6 +500,65 @@ class CudaLDLSolver:
         _check(f(self._h, _p(v, C.c_double)), "sparse_stats")
         return {"plan_ms": v[0], "fronts_fwd": int(v[1]), "fronts_bwd": int(v[2]), "entries_fwd": int(v[3]),
                 "entries_bwd": int(v[4]), "host_work": int(v[5])}
+
+    def _updown_args(self, W, sigma):
+        import scipy.sparse as sps
+        if sps.issparse(W):
+            W = sps.csc_matrix(W)
+            assert W.shape[0] == self.n
+            cp, ri, wv = _u64(W.indptr), _u64(W.indices), _f64(W.data)
+        else:
+            w = np.asarray(W, dtype=np.float64).ravel()
+            assert w.size == self.n
+            ri = _u64(np.flatnonzero(w))
+            cp, wv = _u64([0, ri.size]), _f64(w[ri.astype(np.int64)])
+        k = cp.size - 1
+        sg = _f64(np.broadcast_to(np.asarray(sigma, dtype=np.float64), (k,)) if np.ndim(sigma) == 0 else sigma)
+        assert sg.size == k
+        return k, cp, ri, wv, sg
+
+    def updown(self, W, sigma=1.0) -> bool:
+        """K <- K + W diag(sigma) W^T on the stored values and on the factor, by updating the factor along the
+        assembly-tree paths of W's columns instead of refactoring (see cldl_updown).  ``W``: a scipy sparse n x k
+        matrix or a 1-D array of n values (its nonzeros are the column); ``sigma``: a scalar or k values (> 0 update,
+        < 0 downdate).  Each column's rows must form a clique of the constructor's pattern.  Returns True, or False
+        when an updated pivot fails the refactor's tests: the values are then updated and ``refactor()`` is needed
+        before any solve.  BackendError (NotFactored) before a refactor that returned True, (ZeroPivot) for an exact
+        zero pivot with regularisation off, (BadArgument) on a Schur or sharded handle, after a refactor that found null
+        pivots, for an index out of range, a duplicate row, a non-finite sigma or a pair outside the pattern."""
+        f = self._L.cldl_updown
+        f.argtypes = [C.c_void_p, C.c_uint64] + [C.POINTER(C.c_uint64)] * 2 + [C.POINTER(C.c_double)] * 2
+        f.restype = C.c_int
+        k, cp, ri, wv, sg = self._updown_args(W, sigma)
+        return bool(_check(f(self._h, k, _p(cp, C.c_uint64), _p(ri, C.c_uint64), _p(wv, C.c_double),
+                             _p(sg, C.c_double)), "updown"))
+
+    def updown_dev(self, w_colptr, w_rowidx, d_w_ptr, sigma):
+        """device-pointer form of ``updown`` (cldl_updown_dev): W's pattern (CSC colptr, row indices) and sigma on the
+        host, its values at d_w_ptr (len(w_rowidx) doubles).  Only enqueued on the handle's stream; the verdict comes
+        from ``sync_status()``."""
+        f = self._L.cldl_updown_dev
+        f.argtypes = [C.c_void_p, C.c_uint64] + [C.POINTER(C.c_uint64)] * 2 + [C.c_void_p, C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        cp = _u64(np.asarray(w_colptr, dtype=np.int64).ravel())
+        ri = _u64(np.asarray(w_rowidx, dtype=np.int64).ravel())
+        k = cp.size - 1
+        sg = _f64(np.broadcast_to(np.asarray(sigma, dtype=np.float64), (k,)) if np.ndim(sigma) == 0 else sigma)
+        assert sg.size == k
+        _check(f(self._h, k, _p(cp, C.c_uint64), _p(ri, C.c_uint64), C.c_void_p(d_w_ptr), _p(sg, C.c_double)),
+               "updown_dev")
+
+    def updown_stats(self):
+        """counts of the last ``updown`` / ``updown_dev`` call (cldl_updown_stats): a dict with the host milliseconds of
+        its checks and plans, its passes of 8 columns, the fronts, tasks and panel entries they reached, and its host
+        steps"""
+        f = self._L.cldl_updown_stats
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        v = np.zeros(6, np.float64)
+        _check(f(self._h, _p(v, C.c_double)), "updown_stats")
+        return {"plan_ms": v[0], "passes": int(v[1]), "fronts": int(v[2]), "tasks": int(v[3]), "entries": int(v[4]),
+                "host_work": int(v[5])}
 
     def slogdet(self):
         """(sign, logabsdet) of K + E, the matrix the last ``refactor()`` factored (E its dynamic regularisation), from

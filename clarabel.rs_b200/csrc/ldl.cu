@@ -1091,6 +1091,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
 #include "ldl_schur.cuh"
 #include "ldl_refine.cuh"
 #include "ldl_sparse.cuh"
+#include "ldl_updown.cuh"
 
 __global__ void k_update_values(double* __restrict__ vals, const int* __restrict__ idx,
                                 const double* __restrict__ v, long long len) {
@@ -1371,6 +1372,7 @@ int LDLObject::refactor_async() {
   CK(cudaSetDevice(device));
   factor_ok = false;
   schur_fwd = false;
+  ud_last = false;
   if (int rc = refactor_level0()) return rc;
   g_launches++;
   if (schur) {    // B's tasks only (they come first in the queue), then the complement from the cut roots
@@ -1855,6 +1857,7 @@ int LDLObject::schur_expand_async(double* d_x, const double* d_xS) {
 int LDLObject::sync_status() {
   CK(cudaSetDevice(device));
   CK(cudaStreamSynchronize(stream));
+  if (ud_last) return updown_verdict();
   regularize_count = (uint64_t)h_status[ST_REGCOUNT];
   positive_inertia = (uint64_t)h_status[ST_POSINERTIA];
   null_count = (uint64_t)h_status[ST_NULLCOUNT];
@@ -2272,6 +2275,194 @@ int LDLObject::inverse_entries(uint64_t nnz, const uint64_t* rows, const uint64_
   CK(cudaMemcpyAsync(out, d_sp_out, nnz * sizeof(double), cudaMemcpyDeviceToHost, stream));
   CK(cudaStreamSynchronize(stream));
   return CLDL_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Rank-k updates (cldl_updown, ldl_updown.cuh): K <- K + W diag(sigma) W^T on the stored values and on the factor.
+// Per call the host checks W against the caller's pattern, builds the values' contribution lists and one UpdownPlan
+// per pass of UD_PASS columns, and sends everything in one payload through the pruned solves' stage.  Launches: the
+// values, then per pass the work vectors (zeroed on the closure's pivots, W scattered in) and k_updown.
+
+// the first call: the pruned solves' set-up (stage, col2sn), the work vectors, the (p, beta) slots and the flags
+int LDLObject::updown_setup() {
+  if (!sp_ready) {
+    if (int rc = sparse_setup()) return rc;
+    sp_ready = true;
+  }
+  ud_slots = std::max(1, updown_slot_bound(S));
+  CK(own.alloc(&d_ud_w, (size_t)UD_PASS * (size_t)n));
+  CK(own.alloc(&d_ud_pb, (size_t)ud_slots * CB_PB_MAXNS * UD_PASS * 2));
+  CK(own.alloc(&d_ud_stat, UD_NSTAT));
+  CK(own.alloc_host(&h_ud_stat, UD_NSTAT));
+  int occ = 0, nsm = 0;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_updown, UD_NT, 0));
+  CK(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, device));
+  if (occ < 1) return CLDL_E_CUDA;
+  ud_grid = nsm * occ;
+  return CLDL_OK;
+}
+
+int LDLObject::updown_async(uint64_t k, const uint64_t* cp, const uint64_t* ri, const double* wv, bool w_dev,
+                            const double* sigma) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if (null_count) return CLDL_E_ARG;
+  if (k && (!cp || !sigma || cp[0] != 0)) return CLDL_E_ARG;
+  const uint64_t nnzw = k ? cp[k] : 0;
+  if (k > (uint64_t)INT32_MAX || nnzw > (uint64_t)INT32_MAX || (nnzw && (!ri || !wv))) return CLDL_E_ARG;
+  const auto t0 = std::chrono::steady_clock::now();
+  long long work = 0;
+  if (ud_cp.empty()) {      // the caller's pattern, each column's rows ascending (ties: the first stored entry)
+    ud_cp.assign(h_colptr.begin(), h_colptr.end());
+    ud_row.assign(h_rowval.begin(), h_rowval.end());
+    ud_src.resize(h_rowval.size());
+    std::vector<std::pair<int, int>> e;
+    for (int j = 0; j < n; j++) {
+      e.clear();
+      for (int p = ud_cp[j]; p < ud_cp[j + 1]; p++) e.emplace_back(h_rowval[p], p);
+      std::sort(e.begin(), e.end());
+      for (size_t t = 0; t < e.size(); t++) { ud_row[ud_cp[j] + t] = e[t].first; ud_src[ud_cp[j] + t] = e[t].second; }
+    }
+    ud_seen.assign(n, 0);
+    ud_seen_epoch = 0;
+  }
+  // the refusals, before anything changes; the values' contributions (position, column, w_i's and w_j's entry of W)
+  struct Contrib { int pos, r, a, b; };
+  std::vector<Contrib> con;
+  std::vector<int> act;                  // the columns that change something, ascending
+  for (uint64_t r = 0; r < k; r++) {
+    if (!std::isfinite(sigma[r]) || cp[r + 1] < cp[r] || cp[r + 1] > nnzw) return CLDL_E_ARG;
+    if (++ud_seen_epoch == 0) { std::fill(ud_seen.begin(), ud_seen.end(), 0u); ud_seen_epoch = 1; }
+    for (uint64_t t = cp[r]; t < cp[r + 1]; t++) {
+      if (ri[t] >= (uint64_t)n || ud_seen[ri[t]] == ud_seen_epoch) return CLDL_E_ARG;
+      ud_seen[ri[t]] = ud_seen_epoch;
+    }
+    const bool live = sigma[r] != 0.0 && cp[r + 1] > cp[r];
+    for (uint64_t t1 = cp[r]; t1 < cp[r + 1]; t1++)
+      for (uint64_t t2 = t1; t2 < cp[r + 1]; t2++) {
+        const bool lo1 = ri[t1] <= ri[t2];
+        const int i = (int)(lo1 ? ri[t1] : ri[t2]), j = (int)(lo1 ? ri[t2] : ri[t1]);
+        const int* b0 = ud_row.data() + ud_cp[j];
+        const int* b1 = ud_row.data() + ud_cp[j + 1];
+        const int* it = std::lower_bound(b0, b1, i);
+        work++;
+        if (it == b1 || *it != i) return CLDL_E_ARG;
+        if (live) con.push_back(Contrib{ud_src[it - ud_row.data()], (int)act.size(), (int)(lo1 ? t1 : t2), (int)(lo1 ? t2 : t1)});
+      }
+    if (live) act.push_back((int)r);
+  }
+  CK(cudaSetDevice(device));
+  if (!ud_ready) {
+    const size_t mk = own.mark();
+    const bool had_sp = sp_ready;
+    if (int rc = updown_setup()) {
+      own.release_since(mk);
+      if (!had_sp) {
+        sp_ready = false;
+        d_sp_cnt = d_sp_f2t = nullptr; d_sp_mark = nullptr; d_sp_bpart = nullptr; sp_ev[0] = sp_ev[1] = nullptr;
+      }
+      d_ud_w = d_ud_pb = nullptr; d_ud_stat = h_ud_stat = nullptr;
+      return rc;
+    }
+    ud_ready = true;
+  }
+  ud_passes = ud_fronts = ud_tasks = ud_entries = 0;
+  factor_ok = false;                     // until the verdict (sync_status)
+  ud_last = true;
+  ud_pos_base = positive_inertia;
+  if (act.empty()) {
+    for (int i = 0; i < UD_NSTAT; i++) h_ud_stat[i] = 0;
+    ud_work = work;
+    ud_plan_ms = sp_ms_since(t0);
+    return CLDL_OK;
+  }
+  // the values: contributions grouped per position, ascending column inside a group
+  std::stable_sort(con.begin(), con.end(), [](const Contrib& x, const Contrib& y) { return x.pos < y.pos; });
+  work += (long long)con.size();
+  std::vector<int> vpos, vptr, vc;
+  vc.reserve(3 * con.size());
+  for (size_t e = 0; e < con.size(); e++) {
+    if (e == 0 || con[e].pos != con[e - 1].pos) { vpos.push_back(con[e].pos); vptr.push_back((int)e); }
+    vc.push_back(con[e].r); vc.push_back(con[e].a); vc.push_back(con[e].b);
+  }
+  vptr.push_back((int)con.size());
+  std::vector<double> sig(act.size());
+  for (size_t a = 0; a < act.size(); a++) sig[a] = sigma[act[a]];
+  sp_payload.clear();
+  const size_t o_sig = sp_put(sp_payload, sig), o_vpos = sp_put(sp_payload, vpos), o_vptr = sp_put(sp_payload, vptr);
+  const size_t o_vc = sp_put(sp_payload, vc);
+  const size_t o_wv = w_dev ? 0 : sp_put(sp_payload, wv, nnzw);
+  // the passes
+  struct PassOff { size_t tasks, cnt, alpha, reached, mask, scat; int ntask, nreached, nscat; };
+  std::vector<PassOff> po;
+  const int* iperm = S.iperm.data();
+  for (size_t a0 = 0; a0 < act.size(); a0 += UD_PASS) {
+    const int kk = (int)std::min<size_t>(UD_PASS, act.size() - a0);
+    int first[UD_PASS];
+    double alpha[UD_PASS] = {0, 0, 0, 0, 0, 0, 0, 0};
+    std::vector<int> scat;
+    for (int r = 0; r < kk; r++) {
+      const int c = act[a0 + r];
+      first[r] = n;
+      alpha[r] = sigma[c];
+      for (uint64_t t = cp[c]; t < cp[c + 1]; t++) {
+        const int p = iperm[ri[t]];
+        first[r] = std::min(first[r], p);
+        scat.push_back(r); scat.push_back(p); scat.push_back((int)t);
+      }
+    }
+    build_updown_plan(S, sp_prune, first, kk, ud_plan);
+    if (ud_plan.nslots > ud_slots) return CLDL_E_CUDA;    // cannot happen: updown_slot_bound
+    ud_plan.cnt_init.push_back(0);                         // the queue head
+    PassOff o;
+    o.tasks = sp_put(sp_payload, ud_plan.tasks); o.cnt = sp_put(sp_payload, ud_plan.cnt_init);
+    o.alpha = sp_put(sp_payload, alpha, UD_PASS); o.reached = sp_put(sp_payload, ud_plan.reached);
+    o.mask = sp_put(sp_payload, ud_plan.mask); o.scat = sp_put(sp_payload, scat);
+    o.ntask = (int)ud_plan.tasks.size(); o.nreached = (int)ud_plan.reached.size(); o.nscat = (int)scat.size() / 3;
+    po.push_back(o);
+    ud_passes++;
+    ud_fronts += o.nreached; ud_tasks += o.ntask; ud_entries += ud_plan.entries;
+    work += ud_plan.work + o.nscat;
+  }
+  ud_work = work;
+  ud_plan_ms = sp_ms_since(t0);
+  if (int rc = sparse_stage(0)) return rc;
+  char* base = d_sp_stage;
+  const double* dwv = w_dev ? wv : reinterpret_cast<const double*>(base + o_wv);
+  CK(cudaMemsetAsync(d_ud_stat, 0, UD_NSTAT * sizeof(int), stream));
+  const int npos = (int)vpos.size();
+  g_launches++;
+  k_ud_values<<<(npos + 255) / 256, 256, 0, stream>>>(npos, reinterpret_cast<const int*>(base + o_vpos),
+                                                       reinterpret_cast<const int*>(base + o_vptr),
+                                                       reinterpret_cast<const int*>(base + o_vc),
+                                                       reinterpret_cast<const double*>(base + o_sig), dwv, dev.vals);
+  for (const PassOff& o : po) {
+    UDPlanDev q;
+    q.ntask = o.ntask; q.n = n;
+    q.tasks = reinterpret_cast<const int4*>(base + o.tasks);
+    q.pend = reinterpret_cast<int*>(base + o.cnt);
+    q.rows_left = q.pend + o.nreached; q.done = q.rows_left + o.nreached; q.qhead = q.done + o.nreached;
+    q.alpha = reinterpret_cast<double*>(base + o.alpha);
+    q.w = d_ud_w; q.pb = d_ud_pb; q.stat = d_ud_stat;
+    g_launches += 3;
+    k_ud_zero<<<(o.nreached + 7) / 8, 256, 0, stream>>>(dev, o.nreached, reinterpret_cast<const int*>(base + o.reached),
+                                                       reinterpret_cast<const int*>(base + o.mask), n, d_ud_w);
+    k_ud_scatter<<<(o.nscat + 255) / 256, 256, 0, stream>>>(o.nscat, reinterpret_cast<const int*>(base + o.scat), dwv, n, d_ud_w);
+    k_updown<<<std::min(o.ntask, ud_grid), UD_NT, 0, stream>>>(dev, q);
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(h_ud_stat, d_ud_stat, UD_NSTAT * sizeof(int), cudaMemcpyDeviceToHost, stream));
+  return CLDL_OK;
+}
+
+// the verdict of the last update, its sign changes folded into the positive count (after the stream synchronised);
+// anything but 1 leaves the factor invalid until the next refactor
+int LDLObject::updown_verdict() {
+  positive_inertia = (uint64_t)((int64_t)ud_pos_base + h_ud_stat[UD_DPOS]);
+  const int v = (h_ud_stat[UD_ZERO] && !dev.reg_enable) ? CLDL_E_ZERO_PIVOT : h_ud_stat[UD_FAIL] ? 0 : 1;
+  factor_ok = v == 1;
+  if (v != 1) factored = false;
+  return v;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2750,6 +2941,26 @@ int cldl_sparse_stats(const cldl_t* h, double* out6) {
   const LDLObject& o = h->obj;
   const double v[6] = {o.sp_plan_ms, (double)o.sp_reached[0], (double)o.sp_reached[1], (double)o.sp_entries[0],
                        (double)o.sp_entries[1], (double)o.sp_work};
+  for (int i = 0; i < 6; i++) out6[i] = v[i];
+  return CLDL_OK;
+}
+
+int cldl_updown(cldl_t* h, uint64_t k, const uint64_t* w_colptr, const uint64_t* w_rowidx, const double* w_values,
+                const double* sigma) {
+  if (!h) return CLDL_E_ARG;
+  if (int rc = h->obj.updown_async(k, w_colptr, w_rowidx, w_values, false, sigma)) return rc;
+  return h->obj.sync_status();
+}
+int cldl_updown_dev(cldl_t* h, uint64_t k, const uint64_t* w_colptr, const uint64_t* w_rowidx, const double* d_w_values,
+                    const double* sigma) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.updown_async(k, w_colptr, w_rowidx, d_w_values, true, sigma);
+}
+int cldl_updown_stats(const cldl_t* h, double* out6) {
+  if (!h || !out6) return CLDL_E_ARG;
+  const LDLObject& o = h->obj;
+  const double v[6] = {o.ud_plan_ms, (double)o.ud_passes, (double)o.ud_fronts, (double)o.ud_tasks, (double)o.ud_entries,
+                       (double)o.ud_work};
   for (int i = 0; i < 6; i++) out6[i] = v[i];
   return CLDL_OK;
 }

@@ -149,6 +149,26 @@ class LDLObject {
   int solve_sparse_async(uint64_t nb, const uint64_t* b_index, const double* b_values, bool b_dev, uint64_t nx,
                          const uint64_t* x_index, double* x_values, bool x_dev);
   int inverse_entries(uint64_t nnz, const uint64_t* rows, const uint64_t* cols, double* out);
+  // rank-k updates (cldl_updown, ldl_updown.cuh): the payload goes through the pruned solves' stage; the rest is set
+  // up by the first call
+  bool ud_ready = false;
+  std::vector<int> ud_cp, ud_row, ud_src;   // the caller's pattern per column, rows ascending, with CSC positions
+  std::vector<unsigned> ud_seen;         // [n] duplicate check of a column's rows (stamps)
+  unsigned ud_seen_epoch = 0;
+  double* d_ud_w = nullptr;              // [UD_PASS n] permuted work vectors
+  double* d_ud_pb = nullptr;             // [ud_slots][CB_PB_MAXNS][UD_PASS] (p, beta)
+  int* d_ud_stat = nullptr;              // the last call's flags and sign-change count (UD_FAIL, ...)
+  int* h_ud_stat = nullptr;              // the same, pinned
+  int ud_slots = 0, ud_grid = 0;
+  bool ud_last = false;                  // the last factor change enqueued was an update: sync_status reads h_ud_stat
+  uint64_t ud_pos_base = 0;              // positive_inertia before it
+  UpdownPlan ud_plan;
+  double ud_plan_ms = 0.0;               // host time of the last call's checks and plans
+  long long ud_passes = 0, ud_fronts = 0, ud_tasks = 0, ud_entries = 0, ud_work = 0;   // its counts (diagnostics)
+  int updown_setup();
+  int updown_async(uint64_t k, const uint64_t* w_colptr, const uint64_t* w_rowidx, const double* w_values, bool w_dev,
+                   const double* sigma);
+  int updown_verdict();
   DFFactor dff;
   int *d_dff_init = nullptr, *d_dff_cnt = nullptr;
   std::vector<DFTask> h_dff_tasks;

@@ -588,6 +588,80 @@ void build_pruned_plan(const Symbolic& S, const SolvePlan& full, SolvePrune& X, 
   }
 }
 
+void build_updown_plan(const Symbolic& S, SolvePrune& X, const int* first, int k, UpdownPlan& P) {
+  P.reached.clear(); P.mask.clear(); P.tasks.clear(); P.cnt_init.clear();
+  P.nslots = 0; P.entries = 0; P.work = 0;
+  if (++X.epoch == 0) { std::fill(X.stamp.begin(), X.stamp.end(), 0u); X.epoch = 1; }   // once in 2^32 calls
+  const unsigned ep = X.epoch;
+  // each column's whole path: its mask bit is needed on every front up to the root
+  for (int r = 0; r < k; r++) {
+    P.work++;
+    for (int s = X.col2sn[first[r]]; s >= 0; s = S.sn_parent[s]) {
+      if (X.stamp[s] != ep) {
+        X.stamp[s] = ep;
+        X.ntf2t[s] = (int)P.reached.size();
+        P.reached.push_back(s);
+        P.mask.push_back(0);
+      }
+      P.mask[X.ntf2t[s]] |= 1 << r;
+      P.work++;
+    }
+  }
+  std::vector<int> ord(P.reached.size());
+  for (size_t i = 0; i < ord.size(); i++) ord[i] = (int)i;
+  std::sort(ord.begin(), ord.end(), [&](int a, int b) {
+    P.work++;
+    const int sa = P.reached[a], sb = P.reached[b];
+    return S.sn_level[sa] != S.sn_level[sb] ? S.sn_level[sa] < S.sn_level[sb] : sa < sb;
+  });
+  const size_t r = ord.size();
+  std::vector<int> reached(r), mask(r);
+  for (size_t i = 0; i < r; i++) {
+    reached[i] = P.reached[ord[i]];
+    mask[i] = P.mask[ord[i]];
+    X.ntf2t[reached[i]] = (int)i;
+  }
+  P.reached.swap(reached);
+  P.mask.swap(mask);
+  P.cnt_init.assign(3 * r, 0);
+  for (size_t i = 0; i < r; i++) {
+    const int s = P.reached[i], p = S.sn_parent[s];
+    const int ns = S.sn_first[s + 1] - S.sn_first[s], nr = (int)(S.sn_rowptr[s + 1] - S.sn_rowptr[s]);
+    const int pli = p >= 0 ? X.ntf2t[p] : -1;
+    if (pli >= 0) P.cnt_init[pli]++;
+    P.entries += (long long)(ns + nr) * ns;
+    UDTask t{};
+    t.s = s; t.li = (int)i; t.pli = pli; t.mask = P.mask[i]; t.r0 = 0; t.r1 = nr; t.slot = -1;
+    if (nr <= DF_RB) {
+      t.kind = 0;
+      P.tasks.push_back(t);
+    } else {
+      t.kind = 1; t.slot = P.nslots++;
+      P.tasks.push_back(t);
+      for (int a = 0; a < nr; a += DF_RB) {
+        t.kind = 2; t.r0 = a; t.r1 = std::min(nr, a + DF_RB);
+        P.tasks.push_back(t);
+        P.cnt_init[r + i]++;
+      }
+    }
+    P.work += 1 + P.cnt_init[r + i];
+  }
+}
+
+int updown_slot_bound(const Symbolic& S) {
+  const int nsup = S.nsup;
+  std::vector<int> ord(nsup), cnt(nsup, 0);
+  for (int s = 0; s < nsup; s++) ord[s] = s;
+  std::sort(ord.begin(), ord.end(), [&](int a, int b) { return S.sn_level[a] > S.sn_level[b]; });   // parents first
+  int most = 0;
+  for (int s : ord) {
+    const int p = S.sn_parent[s];
+    cnt[s] = (S.sn_rowptr[s + 1] - S.sn_rowptr[s] > DF_RB ? 1 : 0) + (p >= 0 ? cnt[p] : 0);
+    most = std::max(most, cnt[s]);
+  }
+  return UD_PASS * most;
+}
+
 // Selected inversion (k_selinv): the queue runs the levels from the root down, as the backward sweep does.  The
 // gather maps follow every front's rows up the tree: `cur` holds their positions in the current ancestor's front; the
 // rows that are pivots of that ancestor form the next segment (rows are ascending, so segments are contiguous and

@@ -149,6 +149,38 @@ struct PrunedPlan {
 void build_pruned_plan(const Symbolic& S, const SolvePlan& full, SolvePrune& X, const int* cols, size_t k,
                        PrunedPlan& P);
 
+// Rank-k updates of the factor (cldl_updown, k_updown in ldl_updown.cuh).  A column w of W whose first eliminated row
+// lies in front s0 changes only the fronts on the path from s0 to the root: its other rows are ancestors of that row
+// in the elimination tree (the pattern condition), and each step of the update fills w only along L's column
+// structure.  The columns go in passes of at most UD_PASS; a pass's plan is the upward closure of its columns' first
+// fronts, in the level order of the full factor queue, with per front the mask of the pass's columns whose path passes
+// through it.  A path is a chain, so sibling fronts never share a column: each column's alpha and work vector have one
+// owner at a time.  Tasks: kind 0, a whole front with at most DF_RB rows below the pivot block (the pivot block's
+// sequential recurrence, then its rows); kind 1, the pivot block of a front with more rows, which publishes (p, beta)
+// per (pivot, column) in the front's slot; kind 2, rows [r0, r1) of such a front, DF_RB at most, which wait for their
+// kind 1 task.  Kinds 0 and 1 wait for the reached children (pend); a front is complete when its kind 0 task or its
+// last row task ends.  Every wait is on a task queued earlier.
+#define UD_PASS 8           /* columns of W per pass of the factor update (bits of a front's mask) */
+struct UDTask {             // 32 bytes = 2 x int4
+  int kind, s, li, pli;     // li: the front's index in the plan (counters), pli: the parent's (-1: a root)
+  int mask, r0, r1, slot;   // mask: the pass's columns whose path passes through s; kinds 1, 2: rows and (p, beta) slot
+};
+static_assert(sizeof(UDTask) == 32, "UDTask is 2 x int4");
+struct UpdownPlan {
+  std::vector<int> reached;              // the closure, in queue order (level, then front)
+  std::vector<int> mask;                 // [reached]
+  std::vector<UDTask> tasks;
+  std::vector<int> cnt_init;             // [3 reached]: pend (reached children) | rows_left (row tasks) | done (0)
+  int nslots = 0;                        // fronts with row tasks
+  long long entries = 0;                 // panel entries (ns + nr) ns of the reached fronts
+  long long work = 0;                    // host steps: path visits, sort comparisons, records written
+};
+// first[r] (r < k <= UD_PASS): the first eliminated (permuted) row of column r.  Uses X's col2sn, stamps and scratch;
+// O(k r + r log r) in the r reached fronts, nothing proportional to n or nsup.
+void build_updown_plan(const Symbolic& S, SolvePrune& X, const int* first, int k, UpdownPlan& P);
+// an upper bound on the slots of any pass: UD_PASS times the most fronts with row tasks on one path to a root (O(nsup))
+int updown_slot_bound(const Symbolic& S);
+
 // One task of k_selinv (48 bytes = 3 x int4), queued root to leaves.  kind 0: a whole front with at most SI_RB rows
 // (its rows, then its pivot block); 1: rows [r0, r1) of Z_RS of a front with more rows; 2: the pivot block Z_SS of
 // such a front, after all of its row tasks.  Kinds 0 and 1 wait for the parent front's Z, kind 2 for its row tasks.

@@ -250,6 +250,50 @@ int cldl_null_space_dev(cldl_t *h, uint64_t r, double *d_V, double *resid);
  * backward, and the host steps the plan building took (summed over the column pairs of cldl_inverse_entries). */
 int cldl_sparse_stats(const cldl_t *h, double *out6);
 
+/* Rank-k updates and downdates (CHOLMOD's cholmod_updown): the handle's matrix K becomes K + sum_r sigma_r w_r w_r^T,
+ * its stored values and its factor both, without a refactor.  W is n x k in CSC (w_colptr[k + 1], w_rowidx, w_values,
+ * row indices in the caller's order), sigma k finite reals.
+ *   - Pattern: every pair (a, b) of stored rows of one column of W must be a stored entry of the upper triangle passed
+ *     to cldl_create (diagonal included): each column's pattern is a clique of K's graph.  Then every updated entry
+ *     lies in L's structure (the column's rows are ancestors of its first eliminated row in the elimination tree, so
+ *     only the fronts on the path from that row's front to the root change) and the supernodal storage stays as it is.
+ *     Explicit zeros in K's pattern at create make room for more.
+ *   - Values: per stored entry (i, j), i <= j, the contributions are added in ascending r, each operation rounded once:
+ *     v += (sigma_r * w_i) * w_j.
+ *   - Factor: Gill, Golub, Murray and Saunders' method C1 for L D L^T, per pivot column j on the paths in elimination
+ *     order and per column r whose path contains j in ascending r (alpha_r starts at sigma_r):
+ *         p = w[j];  dbar = d_j + alpha_r p^2;  beta = alpha_r p / dbar;  alpha_r <- alpha_r d_j / dbar;  d_j <- dbar
+ *         rows i of the front below j:  w[i] -= p L_ij;  L_ij += beta w[i]
+ *     then 1/D is rewritten, and wide pivot blocks (more than 8 pivots, which store L11^-1) are recovered, updated and
+ *     inverted again.  Every solve-type call then works on the updated factor unchanged.  The dynamic regularisation E
+ *     of the last refactor is kept: the result is the factor of (K + E) + W diag(sigma) W^T.  If values were changed
+ *     since the last refactor (cldl_update_values and the like) the call is not refused, and the factor stays exactly
+ *     as stale as it was.
+ *   - Verdict, as cldl_refactor's: 1 on success; 0 when an updated pivot is not finite, or with regularisation on fails
+ *     the refactor's sign test (dbar * dsign < regularize_eps), or with a null-pivot threshold set has |dbar| <= tol;
+ *     CLDL_E_ZERO_PIVOT for an exact zero pivot with regularisation off.  After 0 or an error from the factor update the
+ *     values are updated and the factor is invalid: solve-type calls return CLDL_E_NOT_FACTORED until cldl_refactor,
+ *     which factors the updated matrix.  regularize_count is unchanged; with regularisation off, positive_inertia,
+ *     cldl_inertia and the sign of cldl_logdet follow the pivots that change sign.
+ *   - Refused before anything changes: CLDL_E_NOT_FACTORED without a refactor that returned 1 (or with an update whose
+ *     verdict was not yet read by cldl_sync_status); CLDL_E_ARG on a Schur or sharded handle, after a refactor that
+ *     found null pivots, for an index >= n, a duplicate row in a column, a non-finite sigma, a pair outside the pattern,
+ *     and a NULL array that is needed.  k = 0, an empty column and sigma_r = 0 change nothing; the call returns 1.
+ *   - Cost: the columns go in passes of 8; each pass is one dataflow kernel over the fronts on its columns' paths.
+ *     Host work per call is O(r log r) in the r fronts reached plus the sum of the squared column counts (the pattern
+ *     check).  The first call sorts a copy of the caller's pattern on the host (8 nnzA bytes) and allocates 8 n doubles
+ *     of work vectors, the pruned solves' set-up and a few scalars per front; cldl_destroy frees them.
+ *   - No floating-point atomics: repeated calls on equal handles give the same bits.
+ * cldl_updown reads host arrays and synchronises.  cldl_updown_dev takes w_values in device memory (pattern and sigma
+ * on the host) and is only enqueued on the handle's stream; its verdict comes from cldl_sync_status, as for
+ * cldl_refactor_dev.  cldl_updown_stats gives the last call's host milliseconds, passes, fronts reached, tasks, panel
+ * entries of the fronts reached ((ns + nr) ns per front, summed over the passes) and host steps. */
+int cldl_updown(cldl_t *h, uint64_t k, const uint64_t *w_colptr, const uint64_t *w_rowidx, const double *w_values,
+                const double *sigma);
+int cldl_updown_dev(cldl_t *h, uint64_t k, const uint64_t *w_colptr, const uint64_t *w_rowidx,
+                    const double *d_w_values, const double *sigma);   /* pattern and sigma on the host */
+int cldl_updown_stats(const cldl_t *h, double *out6);
+
 /* Adjoint solve: the adjoint of x = K^-1 b.  For an output gradient g (n doubles):
  *     gb = (K + E)^-1 g
  * and, when gvals is not NULL, the gradient of <g, x> with respect to the stored values of the upper triangle passed

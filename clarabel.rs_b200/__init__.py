@@ -178,6 +178,11 @@ class RefineInfo:
     ferr: float
 
 
+# cldl_solve_part / cldl_mul_part sys codes (CHOLMOD's numbering) and cldl_sample forms
+PART_SYS = {"A": 0, "LDLt": 1, "LD": 2, "DLt": 3, "L": 4, "Lt": 5, "D": 6, "P": 7, "Pt": 8, "Dhalf": 9}
+SAMPLE_FORMS = {"precision": 0, "covariance": 1}
+
+
 # every symbol declared in include/clarabel_b200.h (checked by tests/test_abi.py)
 EXPORTED_SYMBOLS = [
     "cldl_default_opts", "cldl_create", "cldl_destroy", "cldl_update_values",
@@ -193,6 +198,8 @@ EXPORTED_SYMBOLS = [
     "cldl_solve_sparse", "cldl_solve_sparse_dev", "cldl_inverse_entries", "cldl_sparse_stats",
     "cldl_set_null_pivot_tol", "cldl_null_pivots", "cldl_inertia", "cldl_null_space", "cldl_null_space_dev",
     "cldl_updown", "cldl_updown_dev", "cldl_updown_stats",
+    "cldl_solve_part", "cldl_solve_part_dev", "cldl_mul_part", "cldl_mul_part_dev", "cldl_factor_csc_nnz",
+    "cldl_get_factor_csc", "cldl_get_factor_csc_dev", "cldl_sample", "cldl_sample_dev",
 ]
 
 
@@ -629,6 +636,116 @@ class CudaLDLSolver:
         resid = np.empty(int(r), np.float64)
         _check(f(self._h, int(r), C.c_void_p(d_V_ptr), _p(resid, C.c_double)), "null_space_dev")
         return resid
+
+    # --- the factor's parts (see cldl_solve_part in include/clarabel_b200.h) ---
+    def _sys(self, sys):
+        if sys not in PART_SYS:
+            raise BackendError(f"unknown sys {sys!r}: one of {', '.join(PART_SYS)}")
+        return PART_SYS[sys]
+
+    def _part(self, name, sys, v):
+        f = getattr(self._L, name)
+        f.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]
+        f.restype = C.c_int
+        code = self._sys(sys)
+        v = np.asarray(v, dtype=np.float64)
+        assert v.shape[:1] == (self.n,) and v.ndim in (1, 2)
+        cols = np.ascontiguousarray(v.reshape(self.n, -1).T)
+        out = np.empty_like(cols)
+        for j in range(cols.shape[0]):
+            _check(f(self._h, code, _p(out[j], C.c_double), _p(cols[j], C.c_double)), name[5:])
+        return out[0] if v.ndim == 1 else np.ascontiguousarray(out.T)
+
+    def solve_part(self, sys, b):
+        """x = op^-1 b for sys in "A" ((K + E)^-1, caller order: exactly ``solve``), "LDLt", "LD", "DLt", "L", "Lt",
+        "D" (D^+: 1/D, 0 at null pivots), "P" (x = P b), "Pt" (x = P^T b), "Dhalf" (|D|^-1/2, 0 at null pivots); every
+        sys but "A" in permuted order, (P b)[k] = b[perm()[k]].  ``b``: n values or n x k (column by column).
+        BackendError (NotFactored) before a refactor that returned True, (BadArgument) on a Schur or sharded handle."""
+        return self._part("cldl_solve_part", sys, b)
+
+    def mul_part(self, sys, x):
+        """y = op x for sys in "A" (P^T L D L^T P, caller order), "LDLt", "LD", "DLt", "L", "Lt", "D", "Dhalf"
+        (|D|^1/2), "P", "Pt", in permuted order as for ``solve_part``"""
+        return self._part("cldl_mul_part", sys, x)
+
+    def solve_part_dev(self, sys, d_x_ptr, d_b_ptr):
+        """device-pointer form of ``solve_part`` for one vector (cldl_solve_part_dev): only enqueued on the handle's
+        stream"""
+        f = self._L.cldl_solve_part_dev
+        f.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        f.restype = C.c_int
+        _check(f(self._h, self._sys(sys), C.c_void_p(d_x_ptr), C.c_void_p(d_b_ptr)), "solve_part_dev")
+
+    def mul_part_dev(self, sys, d_y_ptr, d_x_ptr):
+        """device-pointer form of ``mul_part`` for one vector (cldl_mul_part_dev): only enqueued"""
+        f = self._L.cldl_mul_part_dev
+        f.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+        f.restype = C.c_int
+        _check(f(self._h, self._sys(sys), C.c_void_p(d_y_ptr), C.c_void_p(d_x_ptr)), "mul_part_dev")
+
+    def factor_csc_nnz(self):
+        """entries of L strictly lower on the stored supernodal pattern (cldl_factor_csc_nnz)"""
+        f = self._L.cldl_factor_csc_nnz
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        f.restype = C.c_int
+        v = C.c_uint64()
+        _check(f(self._h, C.byref(v)), "factor_csc_nnz")
+        return int(v.value)
+
+    def factor_csc(self):
+        """(L, D, Dinv, perm): L (scipy.sparse.csc_matrix, n x n) strictly lower in permuted order, rows ascending, on
+        the stored supernodal pattern, with P (K + E) P^T = (I + L) diag(D) (I + L)^T, the layout of the reference's
+        qdldl factors; D and Dinv as stored (0 at null pivots); perm as ``perm()``.  Pivot blocks wider than 8 columns
+        are recovered from their stored inverse (within rounding of the factor's L11).  Synchronises."""
+        import scipy.sparse as sps
+        f = self._L.cldl_get_factor_csc
+        f.argtypes = [C.c_void_p] + [C.POINTER(C.c_uint64)] * 2 + [C.POINTER(C.c_double)] * 3
+        f.restype = C.c_int
+        nnz = self.factor_csc_nnz()
+        cp, ri = np.empty(self.n + 1, np.uint64), np.empty(nnz, np.uint64)
+        Lx, D, Dinv = np.empty(nnz), np.empty(self.n), np.empty(self.n)
+        _check(f(self._h, _p(cp, C.c_uint64), _p(ri, C.c_uint64), _p(Lx, C.c_double), _p(D, C.c_double),
+                 _p(Dinv, C.c_double)), "get_factor_csc")
+        L = sps.csc_matrix((Lx, ri.astype(np.int64), cp.astype(np.int64)), shape=(self.n, self.n))
+        return L, D, Dinv, self.perm()
+
+    def factor_csc_dev(self, d_colptr, d_rowval, d_Lx, d_D, d_Dinv):
+        """device-pointer form of ``factor_csc`` (cldl_get_factor_csc_dev; any pointer may be None): only enqueued"""
+        f = self._L.cldl_get_factor_csc_dev
+        f.argtypes = [C.c_void_p] * 6
+        f.restype = C.c_int
+        _check(f(self._h, *(C.c_void_p(p) if p else None for p in (d_colptr, d_rowval, d_Lx, d_D, d_Dinv))),
+               "get_factor_csc_dev")
+
+    def sample(self, k=1, seed=0, offset=0, mean=None, form="precision", return_z=False):
+        """k draws x ~ N(mean, (K + E)^-1) (form "precision": x = mean + P^T L^-T |D|^-1/2 z) or N(mean, K + E)
+        (form "covariance": x = mean + P^T L |D|^1/2 z), as an n x k array, in caller order.  z: standard normals from Philox4x64-10 with key (seed, 0), draw c at stream position
+        offset + c (see cldl_sample), returned in permuted order when ``return_z``.  BackendError (BadArgument) when a
+        pivot is negative, for an unknown form, on Schur and sharded handles; (NotFactored) as for ``solve``."""
+        f = self._L.cldl_sample
+        f.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64] + [C.POINTER(C.c_double)] * 3
+        f.restype = C.c_int
+        if form not in SAMPLE_FORMS:
+            raise BackendError(f"unknown form {form!r}: 'precision' or 'covariance'")
+        k = int(k)
+        mu = None if mean is None else _f64(np.asarray(mean, dtype=np.float64).ravel())
+        assert mu is None or mu.size == self.n
+        X = np.empty((self.n, k), np.float64, order="F")
+        Z = np.empty((self.n, k), np.float64, order="F") if return_z else None
+        _check(f(self._h, SAMPLE_FORMS[form], k, int(seed), int(offset), None if mu is None else _p(mu, C.c_double),
+                 _p(X, C.c_double), None if Z is None else _p(Z, C.c_double)), "sample")
+        return (X, Z) if return_z else X
+
+    def sample_dev(self, k, seed, offset, d_mu_ptr, d_X_ptr, d_Z_ptr=None, form="precision"):
+        """device-pointer form of ``sample`` (cldl_sample_dev): mean (n doubles) or None, X and Z (n x k, column-major)
+        at device addresses.  Only enqueued on the handle's stream."""
+        f = self._L.cldl_sample_dev
+        f.argtypes = [C.c_void_p, C.c_int, C.c_uint64, C.c_uint64, C.c_uint64] + [C.c_void_p] * 3
+        f.restype = C.c_int
+        if form not in SAMPLE_FORMS:
+            raise BackendError(f"unknown form {form!r}: 'precision' or 'covariance'")
+        _check(f(self._h, SAMPLE_FORMS[form], int(k), int(seed), int(offset),
+                 *(C.c_void_p(p) if p else None for p in (d_mu_ptr, d_X_ptr, d_Z_ptr))), "sample_dev")
 
     def adjoint_solve(self, g, x):
         """The adjoint of x = K^-1 b for an output gradient g: (gb, gvals) with gb = (K + E)^-1 g (n values) and gvals

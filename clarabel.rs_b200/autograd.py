@@ -22,6 +22,7 @@ The linear solve underneath, differentiable on its own (`SparseLDL`, one `CudaLD
     K = SparseLDL(n, colptr, rowval, dsigns)       # upper-triangular CSC pattern, diagonal included
     x = K.solve(values, b)                         # x = K^-1 b, differentiable in values and b
     sign, logabsdet = K.slogdet(values)            # differentiable in values
+    X = K.sample(values, k, seed, mean=mu)         # k draws of N(mu, K^-1), differentiable in mu
 
 `values` are the stored upper-triangle values (float64, the pattern's CSC order), b is (n,) or (n, k).  The backward
 pass of `solve` is one adjoint solve on the forward pass's factor (gb = K^-1 g, and -(gb_i x_j + x_i gb_j) on the
@@ -184,6 +185,32 @@ class SparseLDL:
     def slogdet(self, values):
         """(sign, logabsdet) of K, as float64 scalar tensors; logabsdet is differentiable in values."""
         return _LDLSlogdet.apply(self, values)
+
+    def sample(self, values, k, seed, mean=None, form="precision", offset=0):
+        """k Gaussian draws as an (n, k) tensor: x ~ N(mean, K^-1) (form "precision", K a sparse precision matrix) or
+        N(mean, K) (form "covariance"), from the handle's sampler (CudaLDLSolver.sample: Philox4x64-10 with key
+        (seed, 0), draw c at stream position offset + c).  K must be positive semidefinite.  Differentiable in mean
+        only: a reparameterised gradient in values would need the adjoint of the factorisation itself, so values that
+        require grad raise."""
+        if isinstance(values, torch.Tensor) and values.requires_grad:
+            raise RuntimeError("sample is not differentiable in values: pass values.detach()")
+        self._factor(values)
+        k = int(k)
+        X = torch.empty((k, self.n), dtype=torch.float64, device=self.device)    # column-major n x k
+        self._handle_waits_for_torch()                   # (1)
+        self.solver.sample_dev(k, int(seed), int(offset), None, X.data_ptr(), None, form=form)
+        self._torch_waits_for_handle()                   # (2)
+        X = X.t()
+        if mean is None:
+            return X
+        return self._check_mean(mean) + X
+
+    def _check_mean(self, mean):
+        if not isinstance(mean, torch.Tensor) or mean.dtype != torch.float64 or mean.device != self.device:
+            raise TypeError(f"mean must be a float64 tensor on {self.device}")
+        if tuple(mean.shape) != (self.n,):
+            raise ValueError(f"mean has shape {tuple(mean.shape)}, expected ({self.n},)")
+        return mean.reshape(self.n, 1)
 
 
 class _LDLSolve(torch.autograd.Function):

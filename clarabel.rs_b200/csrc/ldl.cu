@@ -1092,6 +1092,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
 #include "ldl_refine.cuh"
 #include "ldl_sparse.cuh"
 #include "ldl_updown.cuh"
+#include "ldl_parts.cuh"
 
 __global__ void k_update_values(double* __restrict__ vals, const int* __restrict__ idx,
                                 const double* __restrict__ v, long long len) {
@@ -2466,6 +2467,213 @@ int LDLObject::updown_verdict() {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// The factor's parts (cldl_solve_part, cldl_mul_part, cldl_get_factor_csc, cldl_sample; ldl_parts.cuh).  The partial
+// solves are the solve's own launches, one direction at a time.  The forward sweep leaves L^-1 b in the work vector
+// d_xp; the backward sweep leaves its result there too, in permuted order, besides storing it permuted out (to a
+// scratch vector here), so a permuted-order result is read back from d_xp.  L^-T is the backward sweep with 1/D read
+// from ones, as in null_space; precision draws read 1/D from sqrt|1/D|.  Products with L and L^T are the kernels of
+// ldl_parts.cuh; L x needs the row lists of FactorParts (ldl_plan.h), uploaded by the first call that needs them.
+
+int LDLObject::parts_check() {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  return CLDL_OK;
+}
+
+int LDLObject::parts_setup(bool lists) {
+  CK(cudaSetDevice(device));
+  if (!d_pt_work) {
+    const size_t mk = own.mark();
+    if (own.alloc(&d_pt_work, 3 * (size_t)n) != cudaSuccess) { own.release_since(mk); d_pt_work = nullptr; return CLDL_E_CUDA; }
+  }
+  if (lists && !d_pt_colptr) {
+    const FactorParts F = build_factor_parts(S);
+    const size_t mk = own.mark();
+    if (own.upload(&d_pt_rptr, F.row_ptr) != cudaSuccess || own.upload(&d_pt_rpos, F.row_pos) != cudaSuccess ||
+        own.upload(&d_pt_colptr, F.colptr) != cudaSuccess) {
+      own.release_since(mk);
+      d_pt_rptr = d_pt_rpos = nullptr;
+      d_pt_colptr = nullptr;
+      return CLDL_E_CUDA;
+    }
+    pt_nnz = F.colptr[n];
+  }
+  return CLDL_OK;
+}
+
+void LDLObject::pt_lmul(double* d_y, const double* d_x) {
+  g_launches += 2;
+  k_pt_lmul_front<<<S.nsup, PT_NT, 0, stream>>>(dev, d_x, d_y, dev.u);
+  k_pt_lmul_rows<<<(n + 255) / 256, 256, 0, stream>>>(n, d_pt_rptr, d_pt_rpos, dev.u, d_y);
+}
+void LDLObject::pt_ltmul(double* d_y, const double* d_x) {
+  g_launches++;
+  k_pt_ltmul<<<S.nsup, PT_NT, 0, stream>>>(dev, d_x, d_y);
+}
+// which: 0 1/D, 1 D, 2 sqrt|1/D|, 3 sqrt|D|
+void LDLObject::pt_diag(int which, double* d_y, const double* d_x) {
+  g_launches++;
+  k_pt_diag<<<(n + 255) / 256, 256, 0, stream>>>(n, which >> 1, (which & 1) ? dev.D : dev.Dinv, d_x, d_y);
+}
+
+int LDLObject::solve_part_async(int sys, double* d_x, const double* d_b) {
+  if (sys < CLDL_SYS_A || sys > CLDL_SYS_DHALF) return CLDL_E_ARG;
+  if (int rc = parts_check()) return rc;
+  if (sys == CLDL_SYS_A) return solve_async(d_x, d_b);
+  if (int rc = parts_setup(false)) return rc;
+  const size_t bytes = (size_t)n * sizeof(double);
+  double* const t = d_pt_work + n;
+  switch (sys) {
+    case CLDL_SYS_D: pt_diag(0, d_x, d_b); break;
+    case CLDL_SYS_DHALF: pt_diag(2, d_x, d_b); break;
+    case CLDL_SYS_P:
+    case CLDL_SYS_PT:
+      CK(cudaMemcpyAsync(t, d_b, bytes, cudaMemcpyDeviceToDevice, stream));
+      g_launches++;
+      if (sys == CLDL_SYS_P) k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, t, d_x);
+      else k_pt_permute_out<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, t, d_x);
+      break;
+    default: {
+      const bool fwd = sys == CLDL_SYS_LDLT || sys == CLDL_SYS_LD || sys == CLDL_SYS_L;
+      const bool bwd = sys == CLDL_SYS_LDLT || sys == CLDL_SYS_DLT || sys == CLDL_SYS_LT;
+      if (sys == CLDL_SYS_LT && !d_ns_ones) {
+        const size_t mk = own.mark();
+        if (own.alloc(&d_ns_ones, (size_t)n) != cudaSuccess) { own.release_since(mk); d_ns_ones = nullptr; return CLDL_E_CUDA; }
+        double* ones = d_ns_ones;
+        const int nn = n;
+        g_launches++;
+        k_map<<<(n + 255) / 256, 256, 0, stream>>>(nn, [=] __device__(int i) { ones[i] = 1.0; });
+      }
+      SVRhs r;
+      r.xp[0] = r.xp[1] = d_xp; r.u[0] = r.u[1] = dev.u; r.out[0] = r.out[1] = d_pt_work;
+      CK(cudaMemcpyAsync(d_xp, d_b, bytes, cudaMemcpyDeviceToDevice, stream));
+      if (int rc = sv_reset()) return rc;
+      if (fwd) {
+        sv_leaves(true, 1, r, sv_leaf_lists());
+        sv_sweep(true, 1, sv, r);
+      }
+      if (bwd) {
+        double* const dinv = dev.Dinv;
+        if (sys == CLDL_SYS_LT) dev.Dinv = d_ns_ones;     // the launches below take their own copy of dev
+        sv_sweep(false, 1, sv, r);
+        sv_leaves(false, 1, r, sv_leaf_lists());
+        dev.Dinv = dinv;
+      }
+      if (sys == CLDL_SYS_LD) pt_diag(0, d_x, d_xp);
+      else CK(cudaMemcpyAsync(d_x, d_xp, bytes, cudaMemcpyDeviceToDevice, stream));
+    }
+  }
+  CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+int LDLObject::mul_part_async(int sys, double* d_y, const double* d_x) {
+  if (sys < CLDL_SYS_A || sys > CLDL_SYS_DHALF) return CLDL_E_ARG;
+  if (int rc = parts_check()) return rc;
+  const bool tri = sys <= CLDL_SYS_LT;
+  if (int rc = parts_setup(tri)) return rc;
+  const size_t bytes = (size_t)n * sizeof(double);
+  double *const p1 = d_pt_work + n, *const p2 = p1 + n;
+  // the products read x while they write y: x is copied first, so y may be x
+  if (sys != CLDL_SYS_A && sys != CLDL_SYS_LD && sys != CLDL_SYS_D && sys != CLDL_SYS_DHALF)
+    CK(cudaMemcpyAsync(p1, d_x, bytes, cudaMemcpyDeviceToDevice, stream));
+  switch (sys) {
+    case CLDL_SYS_A:
+      g_launches++;
+      k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, d_x, p1);
+      pt_ltmul(p2, p1);
+      pt_diag(1, p2, p2);
+      pt_lmul(p1, p2);
+      g_launches++;
+      k_pt_permute_out<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, p1, d_y);
+      break;
+    case CLDL_SYS_LDLT: pt_ltmul(p2, p1); pt_diag(1, p2, p2); pt_lmul(d_y, p2); break;
+    case CLDL_SYS_LD: pt_diag(1, p1, d_x); pt_lmul(d_y, p1); break;
+    case CLDL_SYS_DLT: pt_ltmul(d_y, p1); pt_diag(1, d_y, d_y); break;
+    case CLDL_SYS_L: pt_lmul(d_y, p1); break;
+    case CLDL_SYS_LT: pt_ltmul(d_y, p1); break;
+    case CLDL_SYS_D: pt_diag(1, d_y, d_x); break;
+    case CLDL_SYS_DHALF: pt_diag(3, d_y, d_x); break;
+    case CLDL_SYS_P: g_launches++; k_permute_in<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, p1, d_y); break;
+    case CLDL_SYS_PT: g_launches++; k_pt_permute_out<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, p1, d_y); break;
+  }
+  CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+// any output may be NULL; the column pointers come from the host plan, uploaded once
+int LDLObject::factor_csc_async(unsigned long long* d_cp, unsigned long long* d_ri, double* d_Lx, double* d_D,
+                                double* d_Dinv) {
+  if (int rc = parts_check()) return rc;
+  if (int rc = parts_setup(true)) return rc;
+  const size_t bytes = (size_t)n * sizeof(double);
+  if (d_cp) CK(cudaMemcpyAsync(d_cp, d_pt_colptr, ((size_t)n + 1) * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
+  if (d_ri || d_Lx) {
+    g_launches++;
+    k_pt_csc<<<S.nsup, PT_NT, 0, stream>>>(dev, d_pt_colptr, d_ri, d_Lx);
+  }
+  if (d_D) CK(cudaMemcpyAsync(d_D, dev.D, bytes, cudaMemcpyDeviceToDevice, stream));
+  if (d_Dinv) CK(cudaMemcpyAsync(d_Dinv, dev.Dinv, bytes, cudaMemcpyDeviceToDevice, stream));
+  CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+// Draws.  Precision: the normals of two columns go into the two work vectors of the sweeps, the backward sweeps run
+// with 1/D read from sqrt|1/D| (0 at null pivots) and store the draws permuted out into X.  Covariance: per column,
+// sqrt|D| z, the product with L, P^T.  Then mu is added.
+int LDLObject::sample_async(int form, uint64_t k, uint64_t seed, uint64_t offset, const double* d_mu, double* d_X,
+                            double* d_Z) {
+  if (form != CLDL_SAMPLE_PRECISION && form != CLDL_SAMPLE_COVARIANCE) return CLDL_E_ARG;
+  if (int rc = parts_check()) return rc;
+  if (positive_inertia + null_count < (uint64_t)n) return CLDL_E_ARG;
+  if (k && !d_X) return CLDL_E_ARG;
+  if (k == 0) return CLDL_OK;
+  if (int rc = parts_setup(form == CLDL_SAMPLE_COVARIANCE)) return rc;
+  const size_t bytes = (size_t)n * sizeof(double);
+  const unsigned ng = (unsigned)(((n + 3) / 4 + 127) / 128);
+  double *const p0 = d_pt_work, *const p1 = p0 + n, *const p2 = p1 + n;
+  if (form == CLDL_SAMPLE_PRECISION) {
+    pt_diag(2, p2, nullptr);
+    for (uint64_t c = 0; c < k; c += 2) {
+      const int nrhs = c + 1 < k ? 2 : 1;
+      SVRhs r;
+      r.xp[0] = d_xp; r.u[0] = dev.u; r.out[0] = d_X + c * (size_t)n;
+      r.xp[1] = nrhs == 2 ? d_xp2 : d_xp; r.u[1] = nrhs == 2 ? d_u2 : dev.u;
+      r.out[1] = nrhs == 2 ? d_X + (c + 1) * (size_t)n : r.out[0];
+      for (int h = 0; h < nrhs; h++) {
+        g_launches++;
+        k_pt_normals<<<ng, 128, 0, stream>>>(n, seed, offset + c + h, r.xp[h]);
+        if (d_Z) CK(cudaMemcpyAsync(d_Z + (c + h) * (size_t)n, r.xp[h], bytes, cudaMemcpyDeviceToDevice, stream));
+      }
+      if (int rc = sv_reset()) return rc;
+      double* const dinv = dev.Dinv;
+      dev.Dinv = p2;                        // the launches below take their own copy of dev
+      sv_sweep(false, nrhs, sv, r);
+      sv_leaves(false, nrhs, r, sv_leaf_lists());
+      dev.Dinv = dinv;
+    }
+  } else {
+    for (uint64_t c = 0; c < k; c++) {
+      g_launches++;
+      k_pt_normals<<<ng, 128, 0, stream>>>(n, seed, offset + c, p1);
+      if (d_Z) CK(cudaMemcpyAsync(d_Z + c * (size_t)n, p1, bytes, cudaMemcpyDeviceToDevice, stream));
+      pt_diag(3, p1, p1);
+      pt_lmul(p0, p1);
+      g_launches++;
+      k_pt_permute_out<<<(n + 255) / 256, 256, 0, stream>>>(n, dev.perm, p0, d_X + c * (size_t)n);
+    }
+  }
+  if (d_mu) {
+    for (uint64_t c = 0; c < k; c++) {
+      g_launches++;
+      k_pt_add<<<(n + 255) / 256, 256, 0, stream>>>(n, d_mu, d_X + c * (size_t)n);
+    }
+  }
+  CK(cudaGetLastError());
+  return CLDL_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // One factorisation on several GPUs (SURVEY 8e).  This object is one rank: it owns some subtrees of the assembly tree
 // and replicates the top part above the cut.  Both dataflow queues list the owned tasks first, then the top tasks:
 //   refactor phase 0  level-0 kernel + k_factor_df over the owned tasks
@@ -2963,6 +3171,100 @@ int cldl_updown_stats(const cldl_t* h, double* out6) {
                        (double)o.ud_work};
   for (int i = 0; i < 6; i++) out6[i] = v[i];
   return CLDL_OK;
+}
+
+// the factor's parts: the host-pointer forms stage through device buffers and synchronise
+int cldl_solve_part_dev(cldl_t* h, int sys, double* d_x, const double* d_b) {
+  if (!h || !d_x || !d_b) return CLDL_E_ARG;
+  return h->obj.solve_part_async(sys, d_x, d_b);
+}
+int cldl_mul_part_dev(cldl_t* h, int sys, double* d_y, const double* d_x) {
+  if (!h || !d_y || !d_x) return CLDL_E_ARG;
+  return h->obj.mul_part_async(sys, d_y, d_x);
+}
+static int parts_host(cldl_t* h, int sys, double* y, const double* x, bool mul) {
+  if (!h || !y || !x) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (int rc = o.parts_check()) return rc;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t bytes = (size_t)o.n * sizeof(double);
+  if (cudaMemcpyAsync(o.d_bx, x, bytes, cudaMemcpyHostToDevice, o.stream) != cudaSuccess) return CLDL_E_CUDA;
+  int rc = mul ? o.mul_part_async(sys, o.d_bx + o.n, o.d_bx) : o.solve_part_async(sys, o.d_bx + o.n, o.d_bx);
+  if (rc) return rc;
+  if (cudaMemcpyAsync(y, o.d_bx + o.n, bytes, cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
+}
+int cldl_solve_part(cldl_t* h, int sys, double* x, const double* b) { return parts_host(h, sys, x, b, false); }
+int cldl_mul_part(cldl_t* h, int sys, double* y, const double* x) { return parts_host(h, sys, y, x, true); }
+int cldl_factor_csc_nnz(const cldl_t* h, uint64_t* nnz) {
+  if (!h || !nnz) return CLDL_E_ARG;
+  const LDLObject& o = h->obj;
+  uint64_t t = 0;
+  for (int s = 0; s < o.S.nsup; s++) {
+    const uint64_t ns = (uint64_t)(o.S.sn_first[s + 1] - o.S.sn_first[s]), nr = (uint64_t)(o.S.sn_rowptr[s + 1] - o.S.sn_rowptr[s]);
+    t += ns * (ns - 1) / 2 + ns * nr;
+  }
+  *nnz = t;
+  return CLDL_OK;
+}
+int cldl_get_factor_csc_dev(cldl_t* h, uint64_t* d_colptr, uint64_t* d_rowval, double* d_Lx, double* d_D, double* d_Dinv) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.factor_csc_async((unsigned long long*)d_colptr, (unsigned long long*)d_rowval, d_Lx, d_D, d_Dinv);
+}
+int cldl_get_factor_csc(cldl_t* h, uint64_t* colptr, uint64_t* rowval, double* Lx, double* D, double* Dinv) {
+  if (!h) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (int rc = o.parts_check()) return rc;
+  if (int rc = o.parts_setup(true)) return rc;
+  const size_t n = (size_t)o.n, nnz = (size_t)o.pt_nnz;
+  // rowval and Lx are staged through buffers of their own, freed before the return
+  unsigned long long* dri = nullptr;
+  double* dlx = nullptr;
+  auto done = [&](int rc) { if (dri) o.own.free(dri); if (dlx) o.own.free(dlx); return rc; };
+  if ((rowval && o.own.alloc(&dri, nnz) != cudaSuccess) || (Lx && o.own.alloc(&dlx, nnz) != cudaSuccess)) return done(CLDL_E_CUDA);
+  if (int rc = o.factor_csc_async(nullptr, dri, dlx, D ? o.d_bx : nullptr, Dinv ? o.d_bx + n : nullptr)) return done(rc);
+  if ((colptr && cudaMemcpyAsync(colptr, o.d_pt_colptr, (n + 1) * sizeof(uint64_t), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess) ||
+      (rowval && cudaMemcpyAsync(rowval, dri, nnz * sizeof(uint64_t), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess) ||
+      (Lx && cudaMemcpyAsync(Lx, dlx, nnz * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess) ||
+      (D && cudaMemcpyAsync(D, o.d_bx, n * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess) ||
+      (Dinv && cudaMemcpyAsync(Dinv, o.d_bx + n, n * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess) ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return done(CLDL_E_CUDA);
+  return done(CLDL_OK);
+}
+int cldl_sample_dev(cldl_t* h, int form, uint64_t k, uint64_t seed, uint64_t offset, const double* d_mu, double* d_X,
+                    double* d_Z) {
+  if (!h) return CLDL_E_ARG;
+  return h->obj.sample_async(form, k, seed, offset, d_mu, d_X, d_Z);
+}
+// the host-pointer form: two columns at a time through the staging buffer (mu in its second half)
+int cldl_sample(cldl_t* h, int form, uint64_t k, uint64_t seed, uint64_t offset, const double* mu, double* X, double* Z) {
+  if (!h) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (k && !X) return CLDL_E_ARG;
+  if (int rc = o.sample_async(form, 0, seed, offset, nullptr, nullptr, nullptr)) return rc;
+  if (k == 0) return CLDL_OK;
+  const size_t n = (size_t)o.n, bytes = n * sizeof(double);
+  if (int rc = o.parts_setup(form == CLDL_SAMPLE_COVARIANCE)) return rc;
+  double* dmu = nullptr;
+  double* dz = nullptr;
+  double* dx = nullptr;
+  auto done = [&](int rc) { if (dmu) o.own.free(dmu); if (dz) o.own.free(dz); if (dx) o.own.free(dx); return rc; };
+  if (o.own.alloc(&dx, 2 * n) != cudaSuccess || (Z && o.own.alloc(&dz, 2 * n) != cudaSuccess) ||
+      (mu && o.own.alloc(&dmu, n) != cudaSuccess))
+    return done(CLDL_E_CUDA);
+  if (mu && cudaMemcpyAsync(dmu, mu, bytes, cudaMemcpyHostToDevice, o.stream) != cudaSuccess) return done(CLDL_E_CUDA);
+  for (uint64_t c = 0; c < k; c += 2) {
+    const uint64_t kk = c + 1 < k ? 2 : 1;
+    if (int rc = o.sample_async(form, kk, seed, offset + c, dmu, dx, dz)) return done(rc);
+    if (cudaMemcpyAsync(X + c * n, dx, kk * bytes, cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+        (Z && cudaMemcpyAsync(Z + c * n, dz, kk * bytes, cudaMemcpyDeviceToHost, o.stream) != cudaSuccess) ||
+        cudaStreamSynchronize(o.stream) != cudaSuccess)
+      return done(CLDL_E_CUDA);
+  }
+  return done(CLDL_OK);
 }
 
 int cldl_adjoint_solve(cldl_t* h, const double* g, const double* x, double* gb, double* gvals) {

@@ -169,6 +169,21 @@ class LDLObject {
   int updown_async(uint64_t k, const uint64_t* w_colptr, const uint64_t* w_rowidx, const double* w_values, bool w_dev,
                    const double* sigma);
   int updown_verdict();
+  // the factor's parts (cldl_solve_part, cldl_mul_part, cldl_get_factor_csc, cldl_sample; ldl_parts.cuh): work vectors
+  // allocated by the first call, row lists and column pointers (FactorParts in ldl_plan.h) by the first that needs them
+  double* d_pt_work = nullptr;           // [3 n]: the sweeps' caller-order store, two temporaries
+  long long *d_pt_rptr = nullptr, *d_pt_rpos = nullptr;
+  unsigned long long* d_pt_colptr = nullptr;
+  uint64_t pt_nnz = 0;
+  int parts_check();
+  int parts_setup(bool lists);
+  void pt_lmul(double* d_y, const double* d_x);    // y = L x (x and y distinct, permuted order)
+  void pt_ltmul(double* d_y, const double* d_x);   // y = L^T x
+  void pt_diag(int which, double* d_y, const double* d_x);   // y = s(a) x per entry (k_pt_diag): which 0 1/D, 1 D, 2 sqrt|1/D|, 3 sqrt|D|
+  int solve_part_async(int sys, double* d_x, const double* d_b);
+  int mul_part_async(int sys, double* d_y, const double* d_x);
+  int factor_csc_async(unsigned long long* d_cp, unsigned long long* d_ri, double* d_Lx, double* d_D, double* d_Dinv);
+  int sample_async(int form, uint64_t k, uint64_t seed, uint64_t offset, const double* d_mu, double* d_X, double* d_Z);
   DFFactor dff;
   int *d_dff_init = nullptr, *d_dff_cnt = nullptr;
   std::vector<DFTask> h_dff_tasks;

@@ -820,4 +820,23 @@ SchurPlan build_schur_plan(const Symbolic& S, const std::vector<int>& schur, con
   return P;
 }
 
+FactorParts build_factor_parts(const Symbolic& S) {
+  FactorParts F;
+  const int n = S.n;
+  const int64_t nnz21 = S.sn_rowptr[S.nsup];
+  F.row_ptr.assign((size_t)n + 1, 0);
+  for (int64_t e = 0; e < nnz21; e++) F.row_ptr[S.sn_rows[e] + 1]++;
+  for (int i = 0; i < n; i++) F.row_ptr[i + 1] += F.row_ptr[i];
+  F.row_pos.resize(nnz21 ? (size_t)nnz21 : 1, 0);
+  std::vector<long long> next(F.row_ptr.begin(), F.row_ptr.end() - 1);
+  for (int64_t e = 0; e < nnz21; e++) F.row_pos[next[S.sn_rows[e]]++] = e;
+  F.colptr.assign((size_t)n + 1, 0);
+  for (int s = 0; s < S.nsup; s++) {
+    const int f = S.sn_first[s], ns = S.sn_first[s + 1] - f;
+    const int64_t nr = S.sn_rowptr[s + 1] - S.sn_rowptr[s];
+    for (int j = 0; j < ns; j++) F.colptr[f + j + 1] = F.colptr[f + j] + (uint64_t)(ns - 1 - j) + (uint64_t)nr;
+  }
+  return F;
+}
+
 }  // namespace cb

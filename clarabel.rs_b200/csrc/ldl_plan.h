@@ -234,4 +234,14 @@ SchurPlan build_schur_plan(const Symbolic& S, const std::vector<int>& schur, con
 // the owner vector above, for the plan builders (first: S.schur_first)
 std::vector<int> schur_owner(const Symbolic& S, int first);
 
+// The factor's parts (cldl_mul_part, cldl_get_factor_csc; ldl_parts.cuh).  L's entries below the pivot blocks by row:
+// for permuted row i, the positions e in sn_rows with sn_rows[e] == i, ascending (ptr: [n + 1], pos: [nnz of L21]);
+// and the compressed-column pointers of L strictly lower on the stored pattern, column f + j of front s holding
+// ns - 1 - j pivot-block entries and nr entries of L21 ([n + 1], ptr[n] = sum over the fronts of ns (ns - 1) / 2 + ns nr).
+struct FactorParts {
+  std::vector<long long> row_ptr, row_pos;
+  std::vector<uint64_t> colptr;
+};
+FactorParts build_factor_parts(const Symbolic& S);
+
 }  // namespace cb

@@ -294,6 +294,59 @@ int cldl_updown_dev(cldl_t *h, uint64_t k, const uint64_t *w_colptr, const uint6
                     const double *d_w_values, const double *sigma);   /* pattern and sigma on the host */
 int cldl_updown_stats(const cldl_t *h, double *out6);
 
+/* The factor's parts (CHOLMOD's cholmod_solve(sys, ...), PARDISO's phases 331 / 332 / 333).  With
+ * P (K + E) P^T = L D L^T (L unit lower triangular, E the dynamic regularisation of the last refactor), (P b)[k] =
+ * b[perm[k]] (cldl_get_perm) and D+ = D with 0 at null pivots (cldl_set_null_pivot_tol):
+ *   cldl_solve_part     x = op^-1 b.  sys CLDL_SYS_A is x = (K + E)^-1 b in caller order: cldl_solve's launches, bit
+ *                       for bit.  Every other sys works in permuted order: LDLT (L D L^T)^-1, LD (L D)^-1,
+ *                       DLT (D L^T)^-1, L L^-1, LT L^-T, D D+ (1/D, 0 at null pivots), P x = P b, PT x = P^T b,
+ *                       DHALF x = |D|^-1/2 b (0 at null pivots).  L^-1 is the forward sweep alone, (D L^T)^-1 the
+ *                       backward sweep alone, L^-T the backward sweep with 1/D read as ones.
+ *   cldl_mul_part       y = op x for op in A = P^T L D L^T P (caller order), LDLT, LD, DLT, L, LT, D, DHALF = |D|^1/2,
+ *                       P, PT (permuted order).  L x and L^T x are one pass over the fronts each (ldl_parts.cuh).
+ *   cldl_factor_csc_nnz / cldl_get_factor_csc
+ *                       L strictly lower in compressed-column form, permuted order, rows ascending in every column, on
+ *                       the stored supernodal pattern: nnz = sum over the fronts of ns (ns - 1) / 2 + ns nr.  Entries
+ *                       below the pivot blocks and in pivot blocks of at most 8 columns are the factor's bits; wider
+ *                       pivot blocks are recovered from their stored inverse and are within rounding of L11 (entries
+ *                       outside the simplicial pattern come back at rounding level).  D and Dinv as stored, 0 at null
+ *                       pivots.  colptr: n + 1, rowval and Lx: nnz, D and Dinv: n.  Any output may be NULL.
+ *   cldl_sample         k draws, X n x k column-major in caller order: form CLDL_SAMPLE_PRECISION
+ *                       x = mu + P^T L^-T |D|^-1/2 z (covariance (K + E)^-1; D+ at null pivots: draws in the range of
+ *                       the generalised inverse), form CLDL_SAMPLE_COVARIANCE x = mu + P^T L |D|^1/2 z (covariance
+ *                       K + E).  mu: n doubles or NULL (0).  Z: NULL or n x k, the standard normals used, in permuted
+ *                       order.  z[r] of column c is normal 4 j + q (j = r / 4, q = r % 4) of Philox4x64-10 with key
+ *                       (seed, 0) and counter (j, offset + c, 0, 0): four words w, u = (w >> 11) 2^-53, Box-Muller
+ *                       on (1 - u0, u1) and (1 - u2, u3): sqrt(-2 ln(1 - u0)) cos(2 pi u1), ... sin(2 pi u1), then
+ *                       the same on (u2, u3).  So draw c of a call equals draw 0 of a call at offset + c, bit for bit.
+ *                       Precision draws go two per pair of backward sweeps; a draw has the same bits either way.
+ *   - Valid after a refactor that returned 1 and after an update that returned 1; otherwise CLDL_E_NOT_FACTORED.
+ *   - CLDL_E_ARG on Schur and sharded handles, for an unknown sys or form, a NULL array that is needed, and (sampling)
+ *     when a pivot is negative: the matrix must be semidefinite.
+ *   - The factor, D, 1/D and later solves are unchanged.  The host-pointer forms synchronise; the _dev forms take
+ *     device pointers and are only enqueued on the handle's stream.  The first call allocates 3 n doubles of work
+ *     vectors, the first product with L or export (n + 1) + nnz(L21) int64s of row lists and n + 1 of column
+ *     pointers, the first L^-T solve n doubles of ones (shared with cldl_null_space); they stay until cldl_destroy.
+ *     cldl_get_factor_csc stages rowval and Lx through nnz int64s and doubles, cldl_sample through at most 5 n
+ *     doubles, allocated and freed by the call. */
+enum {
+  CLDL_SYS_A = 0, CLDL_SYS_LDLT = 1, CLDL_SYS_LD = 2, CLDL_SYS_DLT = 3, CLDL_SYS_L = 4, CLDL_SYS_LT = 5,
+  CLDL_SYS_D = 6, CLDL_SYS_P = 7, CLDL_SYS_PT = 8, CLDL_SYS_DHALF = 9
+};
+enum { CLDL_SAMPLE_PRECISION = 0, CLDL_SAMPLE_COVARIANCE = 1 };
+int cldl_solve_part(cldl_t *h, int sys, double *x, const double *b);
+int cldl_solve_part_dev(cldl_t *h, int sys, double *d_x, const double *d_b);
+int cldl_mul_part(cldl_t *h, int sys, double *y, const double *x);
+int cldl_mul_part_dev(cldl_t *h, int sys, double *d_y, const double *d_x);
+int cldl_factor_csc_nnz(const cldl_t *h, uint64_t *nnz);
+int cldl_get_factor_csc(cldl_t *h, uint64_t *colptr, uint64_t *rowval, double *Lx, double *D, double *Dinv);
+int cldl_get_factor_csc_dev(cldl_t *h, uint64_t *d_colptr, uint64_t *d_rowval, double *d_Lx, double *d_D,
+                            double *d_Dinv);
+int cldl_sample(cldl_t *h, int form, uint64_t k, uint64_t seed, uint64_t offset, const double *mu, double *X,
+                double *Z);
+int cldl_sample_dev(cldl_t *h, int form, uint64_t k, uint64_t seed, uint64_t offset, const double *d_mu, double *d_X,
+                    double *d_Z);
+
 /* Adjoint solve: the adjoint of x = K^-1 b.  For an output gradient g (n doubles):
  *     gb = (K + E)^-1 g
  * and, when gvals is not NULL, the gradient of <g, x> with respect to the stored values of the upper triangle passed

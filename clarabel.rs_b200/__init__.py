@@ -178,6 +178,41 @@ class RefineInfo:
     ferr: float
 
 
+class cldl_eig_opts(C.Structure):
+    _fields_ = [
+        ("ncv", C.c_int32),
+        ("max_restarts", C.c_int32),
+        ("tol", C.c_double),
+        ("seed", C.c_uint64),
+    ]
+
+
+class cldl_eig_info(C.Structure):
+    _fields_ = [
+        ("status", C.c_int32),
+        ("nconv", C.c_int32),
+        ("restarts", C.c_int32),
+        ("solves", C.c_uint32),
+        ("m_products", C.c_uint32),
+        ("n_below", C.c_uint64),
+        ("max_resid", C.c_double),
+    ]
+
+
+@dataclass
+class EigInfo:
+    """Mirror of cldl_eig_info: status 1 converged, 0 not within max_restarts, -1 M not positive definite; resid the
+    per-pair scaled residuals (None for eigsh_dev without them)."""
+    status: int
+    nconv: int
+    restarts: int
+    solves: int
+    m_products: int
+    n_below: int
+    max_resid: float
+    resid: object = None
+
+
 # cldl_solve_part / cldl_mul_part sys codes (CHOLMOD's numbering) and cldl_sample forms
 PART_SYS = {"A": 0, "LDLt": 1, "LD": 2, "DLt": 3, "L": 4, "Lt": 5, "D": 6, "P": 7, "Pt": 8, "Dhalf": 9}
 SAMPLE_FORMS = {"precision": 0, "covariance": 1}
@@ -200,6 +235,7 @@ EXPORTED_SYMBOLS = [
     "cldl_updown", "cldl_updown_dev", "cldl_updown_stats",
     "cldl_solve_part", "cldl_solve_part_dev", "cldl_mul_part", "cldl_mul_part_dev", "cldl_factor_csc_nnz",
     "cldl_get_factor_csc", "cldl_get_factor_csc_dev", "cldl_sample", "cldl_sample_dev",
+    "cldl_default_eig_opts", "cldl_eig_abi_sizes", "cldl_eigsh", "cldl_eigsh_dev",
 ]
 
 
@@ -812,6 +848,89 @@ class CudaLDLSolver:
         o, i = self._refine_opts(max_iter, tol, stop_ratio, error_analysis), cldl_refine_info()
         _check(f(self._h, C.c_void_p(d_x_ptr), C.c_void_p(d_b_ptr), C.byref(o), C.byref(i)), "solve_refined_dev")
         return self._refine_info(i)
+
+    # --- eigenvalues nearest a shift (see cldl_eigsh) ---
+    def _eig_opts(self, ncv, tol, max_restarts, seed):
+        o = cldl_eig_opts()
+        o.ncv, o.max_restarts, o.tol, o.seed = int(ncv), int(max_restarts), float(tol), int(seed)
+        return o
+
+    def _m_values(self, M):
+        if M is None:
+            return None
+        m = _f64(np.asarray(M, dtype=np.float64).ravel())
+        assert m.size == self._pattern[1].size, "M: one value per stored entry of the handle's pattern"
+        return m
+
+    def eigsh(self, k, sigma, M=None, *, ncv=0, tol=0.0, max_restarts=300, seed=0, vectors=True):
+        """The k eigenpairs of A x = lambda M x nearest sigma: (lam, X, EigInfo).  The handle must hold the values
+        A - sigma M, factored with regularisation off (``factor_shifted`` does both).  ``M``: None (the identity) or
+        the values of a positive definite M on the handle's pattern (caller order).  Thick-restart Lanczos on
+        (A - sigma M)^-1 M with one solve per step: lam ascending, X (n x k, None unless ``vectors``) M-orthonormal with
+        each column's entry of largest magnitude positive; ``info.resid`` the residuals ||A x - lam M x||_inf scaled as
+        in cldl_eigsh, from the values; ``info.n_below`` the number of eigenvalues below sigma.  Convergence is
+        ``info.status`` (1), not an exception.  Repeated eigenvalues: not every copy is guaranteed, check with
+        n_below.  Synchronises once per Lanczos step.  BackendError (NotFactored) before a refactor that returned True,
+        (BadArgument) for the refusals of cldl_eigsh."""
+        f = self._L.cldl_eigsh
+        f.argtypes = [C.c_void_p, C.c_double, C.POINTER(C.c_double), C.c_uint64, C.POINTER(cldl_eig_opts)] + \
+            [C.POINTER(C.c_double)] * 3 + [C.POINTER(cldl_eig_info)]
+        f.restype = C.c_int
+        k = int(k)
+        m = self._m_values(M)
+        lam, resid = np.empty(max(k, 0), np.float64), np.empty(max(k, 0), np.float64)
+        X = np.empty((self.n, max(k, 0)), np.float64, order="F") if vectors else None
+        o, i = self._eig_opts(ncv, tol, max_restarts, seed), cldl_eig_info()
+        _check(f(self._h, float(sigma), None if m is None else _p(m, C.c_double), k, C.byref(o), _p(lam, C.c_double),
+                 None if X is None else _p(X, C.c_double), _p(resid, C.c_double), C.byref(i)), "eigsh")
+        return lam, X, EigInfo(int(i.status), int(i.nconv), int(i.restarts), int(i.solves), int(i.m_products),
+                               int(i.n_below), float(i.max_resid), resid)
+
+    def eigsh_dev(self, k, sigma, d_M_ptr=None, d_X_ptr=None, *, ncv=0, tol=0.0, max_restarts=300, seed=0):
+        """``eigsh`` with M's values (nnzA doubles, or None) and X (n x k doubles, column-major, or None) in device
+        memory: returns (lam, EigInfo).  Synchronises once per Lanczos step, as ``eigsh``."""
+        f = self._L.cldl_eigsh_dev
+        f.argtypes = [C.c_void_p, C.c_double, C.c_void_p, C.c_uint64, C.POINTER(cldl_eig_opts), C.POINTER(C.c_double),
+                      C.c_void_p, C.POINTER(C.c_double), C.POINTER(cldl_eig_info)]
+        f.restype = C.c_int
+        k = int(k)
+        lam, resid = np.empty(max(k, 0), np.float64), np.empty(max(k, 0), np.float64)
+        o, i = self._eig_opts(ncv, tol, max_restarts, seed), cldl_eig_info()
+        _check(f(self._h, float(sigma), C.c_void_p(d_M_ptr) if d_M_ptr else None, k, C.byref(o), _p(lam, C.c_double),
+                 C.c_void_p(d_X_ptr) if d_X_ptr else None, _p(resid, C.c_double), C.byref(i)), "eigsh_dev")
+        return lam, EigInfo(int(i.status), int(i.nconv), int(i.restarts), int(i.solves), int(i.m_products),
+                            int(i.n_below), float(i.max_resid), resid)
+
+    def factor_shifted(self, A, sigma, M=None):
+        """Put A - sigma M in the handle (``update_values`` of every stored entry), refactor, and return n-, the number
+        of eigenvalues of (A, M) below sigma (Sylvester's law).  ``A``, ``M``: values on the handle's pattern (M None:
+        the identity, which needs every diagonal entry stored).  The number of eigenvalues in [a, b) is
+        factor_shifted(A, b) - factor_shifted(A, a).  The count is that of A - sigma M only when nothing was
+        regularised, so the handle should be built with ``regularize_enable=False``.  BackendError when the refactor
+        fails or returns False, when it regularised a pivot (``regularize_count`` > 0: the inertia would be that of
+        A - sigma M + E), and when the factor has null pivots (sigma is then numerically an eigenvalue)."""
+        cp, rv = self._pattern
+        a = _f64(np.asarray(A, dtype=np.float64).ravel())
+        assert a.size == rv.size
+        if M is None:
+            cols = np.repeat(np.arange(self.n), np.diff(cp.astype(np.int64)))
+            diag = rv.astype(np.int64) == cols
+            if np.count_nonzero(diag) != self.n:
+                raise BackendError("factor_shifted with M = I needs every diagonal entry in the pattern")
+            vals = a - float(sigma) * diag
+        else:
+            vals = a - float(sigma) * self._m_values(M)
+        self.update_values(np.arange(rv.size), vals)
+        if not self.refactor():
+            raise BackendError("factor_shifted: the refactor of A - sigma M returned False")
+        nreg = self.linear_solver_info().regularize_count
+        if nreg:
+            raise BackendError(f"factor_shifted: {nreg} pivots regularised, the inertia is not that of A - sigma M "
+                               "(build the handle with regularize_enable=False)")
+        npos, nneg, nzero = self.inertia()
+        if nzero:
+            raise BackendError("factor_shifted: null pivots, sigma is numerically an eigenvalue")
+        return nneg
 
     # --- Schur complement handles (constructed with schur=...) ---
     def _schur_call(self, name, *args):

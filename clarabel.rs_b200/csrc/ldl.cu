@@ -32,6 +32,7 @@
 
 #include "../../include/clarabel_b200.h"
 #include "ldl_device.h"
+#include "ldl_eig.h"
 #include "problem_setup.h"
 #include "symbolic.h"
 #include "vec.cuh"
@@ -1093,6 +1094,7 @@ __global__ void __launch_bounds__(DF_NT, 2) k_factor_df(LDLDev d, DFFactor q) {
 #include "ldl_sparse.cuh"
 #include "ldl_updown.cuh"
 #include "ldl_parts.cuh"
+#include "ldl_eig.cuh"
 
 __global__ void k_update_values(double* __restrict__ vals, const int* __restrict__ idx,
                                 const double* __restrict__ v, long long len) {
@@ -2674,6 +2676,245 @@ int LDLObject::sample_async(int form, uint64_t k, uint64_t seed, uint64_t offset
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Eigenvalues nearest a shift (cldl_eigsh): the EigOps of lanczos_run (ldl_eig.cpp) on the device.  T v = F^-1 (M v)
+// is a solve of the column MV[:, j] (V[:, j] when M = I); z = M w is kept beside w, so a Lanczos step needs one product
+// with M (k_refine_residual at b = 0 gives -M w), and the Gram-Schmidt passes update z with MV h.  The h and s slots
+// live in `sc`; fetch() reads them to pinned memory and waits: the one synchronisation of a step.
+namespace {
+struct DevEigOps final : EigOps {
+  LDLObject& o;
+  int n, ncv;
+  bool ident;
+  uint64_t seed;
+  const double* Mv;            // M's values, caller order (NULL: M = I)
+  double *V, *MV, *Y, *w, *z, *part, *sc, *dS;        // MV = V and z = w when M = I
+  double *hS, *hsc;                                    // pinned: S of combine(), the scalars of fetch()
+  double *zero, *tmp, *kx, *rmax;                      // k_refine_residual's b = 0 and outputs (refine work vectors)
+  unsigned* cnt;
+  uint32_t m_products = 0;
+  DevEigOps(LDLObject& obj) : o(obj) {}
+
+  double* col(double* B, int j) const { return B + (size_t)j * n; }
+  double* hslot(int slot) const { return sc + (size_t)slot * (ncv + 1); }
+  double* sslot(int slot) const { return sc + 2 * (size_t)(ncv + 1) + slot; }
+  void mprod(const double* x) {     // z = M x
+    const int nn = n;
+    double *zz = z, *t = tmp;
+    g_launches += 2;
+    k_refine_residual<<<(unsigned)((n + RF_NT / 32 - 1) / (RF_NT / 32)), RF_NT, 0, o.stream>>>(
+        n, o.d_rf_rowptr, o.d_rf_col, o.d_rf_src, Mv, x, zero, t, kx, rmax, nullptr);
+    k_map<<<(n + 255) / 256, 256, 0, o.stream>>>(nn, [=] __device__(int i) { zz[i] = -t[i]; });
+    m_products++;
+  }
+  int apply(int j) override {
+    if (int rc = o.solve_async(w, col(MV, j))) return rc;
+    if (!ident) mprod(w);
+    return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA;
+  }
+  int random(uint64_t draw) override {
+    g_launches++;
+    k_pt_normals<<<(unsigned)(((n + 3) / 4 + 127) / 128), 128, 0, o.stream>>>(n, seed, draw, w);
+    if (!ident) mprod(w);
+    return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA;
+  }
+  int mdots(int j, int slot) override {
+    g_launches++;
+    k_eig_dots<<<red_grid(n), RED_THREADS, 0, o.stream>>>(n, j, V, z, part, cnt, hslot(slot));
+    return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA;
+  }
+  int update(int j, int slot) override {
+    g_launches++;
+    k_eig_update<<<(n + 255) / 256, 256, 0, o.stream>>>(n, j, V, MV, hslot(slot), w, ident ? nullptr : z);
+    return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA;
+  }
+  int mnorm2(int slot) override {
+    const double *ww = w, *zz = z;
+    g_launches++;
+    k_sum<<<red_grid(n), RED_THREADS, 0, o.stream>>>(n, [=] __device__(int i) { return ww[i] * zz[i]; },
+                                                     ReduceWS{part, cnt}, sslot(slot));
+    return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA;
+  }
+  int store(int j, int slot) override {
+    const double *ww = w, *zz = z, *s = sslot(slot);
+    double *v = col(V, j), *mv = ident ? nullptr : col(MV, j);
+    g_launches++;
+    k_map<<<(n + 255) / 256, 256, 0, o.stream>>>(n, [=] __device__(int i) {
+      const double sv = *s, d = sv > 0.0 ? sqrt(sv) : 0.0;
+      v[i] = d > 0.0 ? ww[i] / d : 0.0;
+      if (mv) mv[i] = d > 0.0 ? zz[i] / d : 0.0;
+    });
+    return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA;
+  }
+  int combine(int m, int k, const double* Sh) override {
+    std::memcpy(hS, Sh, (size_t)m * k * sizeof(double));    // the previous copy out of hS finished at the last fetch
+    if (cudaMemcpyAsync(dS, hS, (size_t)m * k * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess)
+      return CLDL_E_CUDA;
+    const dim3 grid((unsigned)((n + EIG_CB_NT - 1) / EIG_CB_NT), (unsigned)((k + EIG_CB_COLS - 1) / EIG_CB_COLS));
+    for (int b = 0; b < (ident ? 1 : 2); b++) {
+      double* B = b ? MV : V;
+      g_launches++;
+      k_eig_combine<<<grid, EIG_CB_NT, 0, o.stream>>>(n, m, k, B, dS, Y);
+      if (cudaMemcpyAsync(B, Y, (size_t)n * k * sizeof(double), cudaMemcpyDeviceToDevice, o.stream) != cudaSuccess)
+        return CLDL_E_CUDA;
+    }
+    return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA;
+  }
+  int copy(int dst, int src) override {
+    for (int b = 0; b < (ident ? 1 : 2); b++) {
+      double* B = b ? MV : V;
+      if (cudaMemcpyAsync(col(B, dst), col(B, src), (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, o.stream) != cudaSuccess)
+        return CLDL_E_CUDA;
+    }
+    return 0;
+  }
+  int fetch(int j, double out[5]) override {
+    if (cudaMemcpyAsync(hsc, sc, (2 * (size_t)(ncv + 1) + 3) * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+        cudaStreamSynchronize(o.stream) != cudaSuccess)
+      return CLDL_E_CUDA;
+    out[0] = hsc[j];
+    out[1] = hsc[ncv + 1 + j];
+    for (int q = 0; q < 3; q++) out[2 + q] = hsc[2 * (ncv + 1) + q];
+    return 0;
+  }
+};
+}  // namespace
+
+int LDLObject::eigsh(double sigma, const double* M, bool m_dev, uint64_t nev, const cldl_eig_opts& op, double* evals,
+                     double* X, bool x_dev, double* resid, cldl_eig_info* info) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  const uint64_t ncv_max = std::min<uint64_t>((uint64_t)n, EIG_MAX_NCV);
+  if (!evals || nev == 0 || nev >= (uint64_t)n) return CLDL_E_ARG;
+  if (op.ncv != 0 && !((uint64_t)op.ncv > nev && (uint64_t)op.ncv <= ncv_max)) return CLDL_E_ARG;
+  if (op.max_restarts < 0 || !(op.tol >= 0.0) || !std::isfinite(sigma)) return CLDL_E_ARG;
+  if (2 * nnzA - n > 0x7fffffff) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if (regularize_count > 0 || null_count > 0) return CLDL_E_ARG;
+  const int ncv = op.ncv ? op.ncv : (int)std::min<uint64_t>(ncv_max, std::max<uint64_t>(2 * nev + 1, 20));
+  if ((uint64_t)ncv <= nev) return CLDL_E_ARG;
+  const int k = (int)nev, nn = n;
+  CK(cudaSetDevice(device));
+  if (!d_rf_work) {
+    const size_t mk = own.mark();
+    if (int rc = refine_setup()) { own.release_since(mk); d_rf_work = nullptr; cudaGetLastError(); return rc; }
+  }
+  // The call's own buffers, all released on the way out.  A failed allocation leaves its error as the runtime's last
+  // error, which the handle's next call would report: it is cleared here (every launch of the call was checked).
+  const size_t mk = own.mark();
+  struct Release {
+    DevOwner& own;
+    size_t mk;
+    ~Release() { own.release_since(mk); cudaGetLastError(); }
+  } rel{own, mk};
+  DevEigOps E(*this);
+  E.n = n; E.ncv = ncv; E.ident = M == nullptr; E.seed = op.seed;
+  const size_t nb = (size_t)n * (ncv + 1);
+  CK(own.alloc(&E.V, nb));
+  if (!E.ident) CK(own.alloc(&E.MV, nb)); else E.MV = E.V;
+  CK(own.alloc(&E.Y, (size_t)n * ncv));
+  CK(own.alloc(&E.w, (size_t)n));
+  if (!E.ident) CK(own.alloc(&E.z, (size_t)n)); else E.z = E.w;
+  CK(own.alloc(&E.part, (size_t)(ncv + 1) * RED_BLOCKS));
+  CK(own.alloc(&E.cnt, 1));
+  CK(own.alloc(&E.sc, 2 * (size_t)(ncv + 1) + 3 + 2 * (size_t)k + 2 + RF_NS));
+  CK(own.alloc(&E.dS, (size_t)ncv * ncv));
+  CK(own.alloc_host(&E.hS, (size_t)ncv * ncv));
+  CK(own.alloc_host(&E.hsc, 2 * (size_t)(ncv + 1) + 3 + 2 * (size_t)k + 2));
+  if (!E.ident && !m_dev) {
+    double* dM = nullptr;
+    CK(own.alloc(&dM, (size_t)nnzA));
+    CK(cudaMemcpyAsync(dM, M, (size_t)nnzA * sizeof(double), cudaMemcpyHostToDevice, stream));
+    E.Mv = dM;
+  } else {
+    E.Mv = M;
+  }
+  E.zero = d_rf_work; E.tmp = d_rf_work + (size_t)n; E.kx = d_rf_work + 3 * (size_t)n; E.rmax = d_rf_work + 4 * (size_t)n;
+  CK(cudaMemsetAsync(E.zero, 0, (size_t)n * sizeof(double), stream));
+  CK(cudaMemsetAsync(E.cnt, 0, sizeof(unsigned), stream));
+  CK(cudaMemsetAsync(E.sc, 0, (2 * (size_t)(ncv + 1) + 3) * sizeof(double), stream));
+  EigResult R;
+  if (int rc = lanczos_run(E, n, k, ncv, op.max_restarts, op.tol, E.ident, R)) return rc;
+
+  cldl_eig_info in{};
+  in.status = R.status;
+  in.nconv = R.nconv;
+  in.restarts = R.restarts;
+  in.solves = R.applies;
+  in.n_below = (uint64_t)n - positive_inertia - null_count;
+  const size_t bytes = (size_t)n * sizeof(double);
+  if (R.theta.empty()) {           // stopped before a basis existed (M-norm <= 0, or a non-finite value)
+    for (int c = 0; c < k; c++) { evals[c] = NAN; if (resid) resid[c] = NAN; }
+    in.max_resid = NAN;
+    if (X) {
+      const double qnan = NAN;
+      for (int c = 0; c < k; c++) {      // a column at a time: n k may exceed int
+        double* Xo = (x_dev ? X : E.Y) + (size_t)c * n;
+        g_launches++;
+        k_map<<<(n + 255) / 256, 256, 0, stream>>>(nn, [=] __device__(int i) { Xo[i] = qnan; });
+      }
+      if (!x_dev) CK(cudaMemcpyAsync(X, E.Y, bytes * k, cudaMemcpyDeviceToHost, stream));
+    }
+    in.m_products = E.m_products;
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(stream));
+    if (info) *info = in;
+    return CLDL_OK;
+  }
+  // per column c of V[:, 0, k): its sign (the entry of largest magnitude positive), then the residual from the values
+  double* st = E.sc + 2 * (size_t)(ncv + 1) + 3;   // ||x_c||_inf, ||r_c||_inf per column, then ||F||_inf, ||M||_inf
+  double* rsc = st + 2 * (size_t)k + 2;            // k_refine_argmax's scalars (out[RF_J], out[RF_VJ])
+  double *r = d_rf_work + (size_t)n, *rsum = d_rf_work + 2 * (size_t)n, *r2 = d_rf_work + 5 * (size_t)n;
+  const ReduceWS ws{E.part, E.cnt};
+  CK(cudaMemsetAsync(st, 0, (2 * (size_t)k + 2) * sizeof(double), stream));
+  const unsigned rgrid = (unsigned)((n + RF_NT / 32 - 1) / (RF_NT / 32));
+  for (int c = 0; c < k; c++) {
+    double* x = E.V + (size_t)c * n;
+    double* sg = rsc + RF_NS - 1;
+    const double ls = 1.0 / R.theta[c];     // lambda - sigma
+    g_launches += 3;
+    k_refine_argmax<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, x, ws, rsc);
+    k_map<<<1, 32, 0, stream>>>(1, [=] __device__(int) {
+      const int j = (int)rsc[RF_J];
+      *sg = j >= 0 && j < nn && x[j] < 0.0 ? -1.0 : 1.0;
+    });
+    k_map<<<(n + 255) / 256, 256, 0, stream>>>(nn, [=] __device__(int i) { if (*sg < 0.0) x[i] = -x[i]; });
+    const bool first = c == 0;
+    g_launches += 3;
+    k_refine_residual<<<rgrid, RF_NT, 0, stream>>>(n, d_rf_rowptr, d_rf_col, d_rf_src, dev.vals, x, E.zero, r, E.kx,
+                                                   E.rmax, first ? rsum : nullptr);
+    if (first) k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return rsum[i]; }, st + 2 * k);
+    k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return x[i]; }, st + 2 * c);
+    if (E.ident) {
+      g_launches++;
+      k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return r[i] + ls * x[i]; }, st + 2 * c + 1);
+    } else {
+      g_launches += first ? 3 : 2;
+      k_refine_residual<<<rgrid, RF_NT, 0, stream>>>(n, d_rf_rowptr, d_rf_col, d_rf_src, E.Mv, x, E.zero, r2, E.kx,
+                                                     E.rmax, first ? rsum : nullptr);
+      if (first) k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return rsum[i]; }, st + 2 * k + 1);
+      k_max_nonneg<<<red_grid(n), RED_THREADS, 0, stream>>>(nn, [=] __device__(int i) { return r[i] - ls * r2[i]; }, st + 2 * c + 1);
+      E.m_products++;
+    }
+    CK(cudaGetLastError());
+  }
+  if (X) CK(cudaMemcpyAsync(X, E.V, bytes * k, x_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, stream));
+  CK(cudaMemcpyAsync(E.hsc, st, (2 * (size_t)k + 2) * sizeof(double), cudaMemcpyDeviceToHost, stream));
+  CK(cudaStreamSynchronize(stream));
+  const double nF = E.hsc[2 * k], nM = E.ident ? 1.0 : E.hsc[2 * k + 1];
+  in.max_resid = 0.0;
+  for (int c = 0; c < k; c++) {
+    const double lam = sigma + 1.0 / R.theta[c];
+    const double num = E.hsc[2 * c + 1], den = (nF + std::fabs(sigma) * nM + std::fabs(lam) * nM) * E.hsc[2 * c];
+    const double rs = num == 0.0 ? 0.0 : num / den;
+    evals[c] = lam;
+    if (resid) resid[c] = rs;
+    in.max_resid = std::isnan(rs) || rs > in.max_resid ? rs : in.max_resid;
+  }
+  in.m_products = E.m_products;
+  if (info) *info = in;
+  return CLDL_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // One factorisation on several GPUs (SURVEY 8e).  This object is one rank: it owns some subtrees of the assembly tree
 // and replicates the top part above the cut.  Both dataflow queues list the owned tasks first, then the top tasks:
 //   refactor phase 0  level-0 kernel + k_factor_df over the owned tasks
@@ -3324,6 +3565,33 @@ int cldl_solve_refined(cldl_t* h, double* x, const double* b, const cldl_refine_
       cudaStreamSynchronize(o.stream) != cudaSuccess)
     return CLDL_E_CUDA;
   return CLDL_OK;
+}
+
+void cldl_default_eig_opts(cldl_eig_opts* o) {
+  std::memset(o, 0, sizeof(*o));
+  o->ncv = 0;
+  o->max_restarts = 300;
+  o->tol = 0.0;
+  o->seed = 0;
+}
+void cldl_eig_abi_sizes(uint64_t* out2) {
+  out2[0] = sizeof(cldl_eig_opts);
+  out2[1] = sizeof(cldl_eig_info);
+}
+static int eigsh_entry(cldl_t* h, double sigma, const double* M, bool dev, uint64_t nev, const cldl_eig_opts* opts,
+                       double* evals, double* X, double* resid, cldl_eig_info* info) {
+  if (!h) return CLDL_E_ARG;
+  cldl_eig_opts o;
+  if (opts) o = *opts; else cldl_default_eig_opts(&o);
+  return h->obj.eigsh(sigma, M, dev, nev, o, evals, X, dev, resid, info);
+}
+int cldl_eigsh(cldl_t* h, double sigma, const double* M_nzval, uint64_t nev, const cldl_eig_opts* o, double* evals,
+               double* X, double* resid, cldl_eig_info* info) {
+  return eigsh_entry(h, sigma, M_nzval, false, nev, o, evals, X, resid, info);
+}
+int cldl_eigsh_dev(cldl_t* h, double sigma, const double* d_M_nzval, uint64_t nev, const cldl_eig_opts* o,
+                   double* evals, double* d_X, double* resid, cldl_eig_info* info) {
+  return eigsh_entry(h, sigma, d_M_nzval, true, nev, o, evals, d_X, resid, info);
 }
 
 int cldl_create_schur(cldl_t** out, uint64_t n, const uint64_t* colptr, const uint64_t* rowval,

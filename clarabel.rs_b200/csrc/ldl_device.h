@@ -250,6 +250,9 @@ class LDLObject {
   int refine_analyse(const double* d_xv, const double* d_b, bool first);
   int condest(int which, const double* d_b, double* est, uint32_t* solves);
   int solve_refined(double* d_x, const double* d_b, const cldl_refine_opts& o, cldl_refine_info* info);
+  // eigenvalues nearest a shift (cldl_eigsh; ldl_eig.cpp, ldl_eig.cuh): buffers allocated and freed by each call
+  int eigsh(double sigma, const double* M, bool m_dev, uint64_t nev, const cldl_eig_opts& o, double* evals, double* X,
+            bool x_dev, double* resid, cldl_eig_info* info);
   // Schur complement handle (cldl_create_schur; SchurPlan in ldl_plan.h): B's fronts are factored, S's never
   std::vector<int> schur_set;            // non-empty: a Schur complement handle
   bool schur = false;

@@ -428,6 +428,71 @@ int cldl_solve_refined_dev(cldl_t *h, double *d_x, const double *d_b, const cldl
                            cldl_refine_info *info);
 void cldl_refine_abi_sizes(uint64_t *out2);   /* sizeof cldl_refine_opts, cldl_refine_info */
 
+/* Eigenvalues nearest a shift (scipy.sparse.linalg.eigsh(sigma=), SLEPc's shift-and-invert).  The caller puts the
+ * values F = A - sigma M in the handle (A its matrix, M positive definite, both on the handle's pattern) and refactors
+ * with regularize_enable = 0.  cldl_eigsh returns the nev eigenpairs (lambda, x) of A x = lambda M x nearest sigma:
+ *   - Method: thick-restart Lanczos (Wu and Simon 2000) on T = F^-1 M, self-adjoint in <x, y>_M = x^T M y.  Its
+ *     eigenvalues theta give lambda = sigma + 1 / theta; the nev of largest |theta| are wanted.  Each step is one solve
+ *     with the factor, one product with M (none when M_nzval is NULL: M = I), and classical Gram-Schmidt against the
+ *     whole basis, twice, in the M-inner product.  An invariant subspace (the second pass removes more than 30% of what
+ *     the first left, or leaves less than 2^-40 ||T v_j||_M) sets beta = 0 and continues with a fresh random vector
+ *     orthogonalised against the basis.  A
+ *     restart keeps the nev wanted Ritz vectors and up to (ncv - nev) / 2 more, as more have converged.
+ *   - Converged: |beta_m y_{m,i}| <= tol |theta_i| (ARPACK's test, y_i the eigenvector of the projected matrix).
+ *   - Single-vector Lanczos finds every eigenvalue but not necessarily every copy of a repeated one.  info.n_below is n-
+ *     of the factor, which by Sylvester's law is the number of eigenvalues of (A, M) below sigma: the number of lambda
+ *     in [a, b) is n_below at b minus n_below at a, the completeness check.
+ *   - Output: evals ascending; X (n x nev column-major, or NULL) M-orthonormal, each column's entry of largest
+ *     magnitude positive (the smallest index on a tie).  With status 0 the nconv converged pairs come first, then the
+ *     other wanted Ritz pairs, each group ascending.
+ *   - resid[i] (nev doubles, or NULL) = ||A x - lambda M x||_inf / ((||F||_inf + |sigma| ||M||_inf + |lambda| ||M||_inf)
+ *     ||x||_inf), with A x - lambda M x = F x - (lambda - sigma) M x formed from the handle's values, not the factor:
+ *     an inaccurate factor (it is taken without pivoting) shows in the residuals.  info.max_resid is their maximum.
+ *   - The start vector is Philox draw 0 of `seed` (the normals of cldl_sample at offset 0), the k-th fresh vector draw k.
+ *   - status: 1 all nev converged; 0 not within max_restarts (or a non-finite value met: evals, X and resid are then
+ *     NaN when nconv = 0); -1 a zero or negative M-norm was met, M is not positive definite (evals, X and resid NaN).
+ *     All return CLDL_OK.  The M-norms checked are those of the random draws and of T v_j, and that of a fresh vector
+ *     after orthogonalisation: an indefinite M whose negative directions none of them meets is not detected, and the
+ *     run then ends with status 0 or with pairs that are not eigenpairs of a definite pencil.  M must be positive
+ *     definite; the check is a safeguard, not a test of definiteness.
+ *   - CLDL_E_NOT_FACTORED without a refactor that returned 1.  CLDL_E_ARG on Schur and sharded handles, for nev = 0 or
+ *     nev >= n, an ncv that is nonzero and outside (nev, min(n, 512)], ncv = 0 with nev >= min(n, 512) (the default
+ *     basis would not exceed nev), max_restarts < 0, tol < 0 or NaN, NULL evals,
+ *     when 2 nnzA - n does not fit int32 (the mirrored pattern of cldl_solve_refined), and for a factor with
+ *     regularize_count > 0 (it would be the factor of F + E) or with null pivots (sigma is then numerically an
+ *     eigenvalue: move it).  CLDL_E_CUDA when an allocation fails; the handle stays usable.
+ *   - Synchronisation: BOTH forms synchronise the handle's stream once per Lanczos step (the iteration runs on the
+ *     host), as cldl_solve_refined_dev does.  cldl_eigsh_dev reads M's values and writes X in device memory.
+ *   - Memory: the call allocates (ncv + 1) n doubles of basis (twice that with M), ncv n of restart scratch, 2 n of
+ *     work vectors and (ncv + 1) 296 of reduction partials (plus nnzA for a host M), and frees them before it returns;
+ *     the first call also sets up cldl_solve_refined's mirrored pattern, which stays.
+ *   - No floating-point atomics and fixed reduction orders: two calls give the same bits.  The call reads the factor and
+ *     the values and writes only its own buffers: the factor and later solves are bit for bit unchanged.
+ * opts == NULL means the defaults of cldl_default_eig_opts; resid and info may be NULL. */
+typedef struct {
+  int32_t ncv;             /* basis size; 0 = min(n, 512, max(2 nev + 1, 20))                   (default 0) */
+  int32_t max_restarts;    /* thick restarts at most                                             (default 300) */
+  double tol;              /* convergence tolerance; 0 = DBL_EPSILON                             (default 0) */
+  uint64_t seed;           /* Philox key of the start vector and of fresh vectors                (default 0) */
+} cldl_eig_opts;
+
+typedef struct {
+  int32_t status;          /* 1 converged, 0 not converged, -1 M not positive definite */
+  int32_t nconv;           /* converged pairs among the nev returned (they come first) */
+  int32_t restarts;        /* thick restarts made */
+  uint32_t solves;         /* solves with the factor (one per Lanczos step) */
+  uint32_t m_products;     /* products with M, residuals included (0 when M = I) */
+  uint64_t n_below;        /* n- of the factor: eigenvalues of (A, M) below sigma */
+  double max_resid;        /* max of resid */
+} cldl_eig_info;
+
+void cldl_default_eig_opts(cldl_eig_opts *o);
+void cldl_eig_abi_sizes(uint64_t *out2);       /* sizeof cldl_eig_opts, cldl_eig_info */
+int cldl_eigsh(cldl_t *h, double sigma, const double *M_nzval, uint64_t nev, const cldl_eig_opts *o, double *evals,
+               double *X, double *resid, cldl_eig_info *info);
+int cldl_eigsh_dev(cldl_t *h, double sigma, const double *d_M_nzval, uint64_t nev, const cldl_eig_opts *o,
+                   double *evals, double *d_X, double *resid, cldl_eig_info *info);
+
 /* ---- device-pointer twins (asynchronous on the handle's stream) ---- */
 int cldl_update_values_dev(cldl_t *h, const int32_t *d_index, const double *d_values, uint64_t len);
 int cldl_set_values_dev(cldl_t *h, const double *d_nzval);   /* whole array, caller order */

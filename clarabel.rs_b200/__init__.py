@@ -213,6 +213,53 @@ class EigInfo:
     resid: object = None
 
 
+class cldl_gmres_opts(C.Structure):
+    _fields_ = [
+        ("restart", C.c_int32),
+        ("max_iter", C.c_int32),
+        ("tol", C.c_double),
+        ("error_analysis", C.c_int32),
+    ]
+
+
+class cldl_gmres_info(C.Structure):
+    _fields_ = [
+        ("iterations", C.c_uint32),
+        ("cycles", C.c_uint32),
+        ("solves", C.c_uint32),
+        ("products", C.c_uint32),
+        ("converged", C.c_int32),
+        ("norm_K_inf", C.c_double),
+        ("norm_x_inf", C.c_double),
+        ("resid_inf", C.c_double),
+        ("scaled_resid", C.c_double),
+        ("omega1", C.c_double),
+        ("omega2", C.c_double),
+        ("cond1", C.c_double),
+        ("cond2", C.c_double),
+        ("ferr", C.c_double),
+    ]
+
+
+@dataclass
+class GmresInfo:
+    """Mirror of cldl_gmres_info: the steps taken and the analysis of the x a preconditioned solve returned."""
+    iterations: int
+    cycles: int
+    solves: int
+    products: int
+    converged: bool
+    norm_K_inf: float
+    norm_x_inf: float
+    resid_inf: float
+    scaled_resid: float
+    omega1: float
+    omega2: float
+    cond1: float
+    cond2: float
+    ferr: float
+
+
 # cldl_solve_part / cldl_mul_part sys codes (CHOLMOD's numbering) and cldl_sample forms
 PART_SYS = {"A": 0, "LDLt": 1, "LD": 2, "DLt": 3, "L": 4, "Lt": 5, "D": 6, "P": 7, "Pt": 8, "Dhalf": 9}
 SAMPLE_FORMS = {"precision": 0, "covariance": 1}
@@ -236,6 +283,7 @@ EXPORTED_SYMBOLS = [
     "cldl_solve_part", "cldl_solve_part_dev", "cldl_mul_part", "cldl_mul_part_dev", "cldl_factor_csc_nnz",
     "cldl_get_factor_csc", "cldl_get_factor_csc_dev", "cldl_sample", "cldl_sample_dev",
     "cldl_default_eig_opts", "cldl_eig_abi_sizes", "cldl_eigsh", "cldl_eigsh_dev",
+    "cldl_default_gmres_opts", "cldl_gmres_abi_sizes", "cldl_solve_gmres", "cldl_solve_gmres_dev",
 ]
 
 
@@ -848,6 +896,53 @@ class CudaLDLSolver:
         o, i = self._refine_opts(max_iter, tol, stop_ratio, error_analysis), cldl_refine_info()
         _check(f(self._h, C.c_void_p(d_x_ptr), C.c_void_p(d_b_ptr), C.byref(o), C.byref(i)), "solve_refined_dev")
         return self._refine_info(i)
+
+    # --- solves preconditioned by the factor (see cldl_solve_gmres) ---
+    @staticmethod
+    def _gmres_opts(restart, max_iter, tol, error_analysis):
+        o = cldl_gmres_opts()
+        o.restart, o.max_iter, o.tol = int(restart), int(max_iter), float(tol)
+        o.error_analysis = 1 if error_analysis else 0
+        return o
+
+    @staticmethod
+    def _gmres_info(i):
+        return GmresInfo(int(i.iterations), int(i.cycles), int(i.solves), int(i.products), bool(i.converged),
+                         i.norm_K_inf, i.norm_x_inf, i.resid_inf, i.scaled_resid, i.omega1, i.omega2, i.cond1, i.cond2,
+                         i.ferr)
+
+    def solve_gmres(self, b, *, restart=20, max_iter=100, tol=float(np.finfo(np.float64).eps), error_analysis=False):
+        """Solve of K x = b by restarted flexible GMRES preconditioned by the factor: (x, GmresInfo).  K is the matrix
+        of the handle's CURRENT values, as in ``solve_refined``; the preconditioner is the factor of the last
+        ``refactor()``, regularised pivots and older values included.  Use it where ``solve_refined`` stalls: after
+        dynamic regularisation or a large value change it converges in about rank(change) + 1 steps.  x0 is bitwise
+        ``solve(b)``; each cycle of at most ``restart`` Arnoldi steps ends with an analysis, and the call stops at
+        omega1 + omega2 <= tol, after max_iter steps in all, or when a cycle did not lower omega1 + omega2; the iterate
+        with the smallest omega1 + omega2 is returned.  ``error_analysis``: also cond1, cond2 and ferr.  Convergence is
+        ``info.converged``, not an exception.  Synchronises once per Arnoldi step.  BackendError (NotFactored) before a
+        refactor that returned True, (BadArgument) for the refusals of cldl_solve_gmres."""
+        f = self._L.cldl_solve_gmres
+        f.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(cldl_gmres_opts),
+                      C.POINTER(cldl_gmres_info)]
+        f.restype = C.c_int
+        b = _f64(b)
+        assert b.size == self.n
+        x = np.empty_like(b)
+        o, i = self._gmres_opts(restart, max_iter, tol, error_analysis), cldl_gmres_info()
+        _check(f(self._h, _p(x, C.c_double), _p(b, C.c_double), C.byref(o), C.byref(i)), "solve_gmres")
+        return x, self._gmres_info(i)
+
+    def solve_gmres_dev(self, d_x_ptr, d_b_ptr, *, restart=20, max_iter=100, tol=float(np.finfo(np.float64).eps),
+                        error_analysis=False):
+        """``solve_gmres`` on device buffers (n doubles each, not overlapping): writes x to d_x_ptr and returns the
+        GmresInfo.  Synchronises the handle's stream once per Arnoldi step, as ``solve_gmres``; no vector is copied to
+        the host."""
+        f = self._L.cldl_solve_gmres_dev
+        f.argtypes = [C.c_void_p] * 3 + [C.POINTER(cldl_gmres_opts), C.POINTER(cldl_gmres_info)]
+        f.restype = C.c_int
+        o, i = self._gmres_opts(restart, max_iter, tol, error_analysis), cldl_gmres_info()
+        _check(f(self._h, C.c_void_p(d_x_ptr), C.c_void_p(d_b_ptr), C.byref(o), C.byref(i)), "solve_gmres_dev")
+        return self._gmres_info(i)
 
     # --- eigenvalues nearest a shift (see cldl_eigsh) ---
     def _eig_opts(self, ncv, tol, max_restarts, seed):

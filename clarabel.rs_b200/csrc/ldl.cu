@@ -33,6 +33,7 @@
 #include "../../include/clarabel_b200.h"
 #include "ldl_device.h"
 #include "ldl_eig.h"
+#include "ldl_krylov.h"
 #include "problem_setup.h"
 #include "symbolic.h"
 #include "vec.cuh"
@@ -2915,6 +2916,191 @@ int LDLObject::eigsh(double sigma, const double* M, bool m_dev, uint64_t nev, co
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Solves preconditioned by the factor (cldl_solve_gmres): the KrylovOps of fgmres_run (ldl_krylov.cpp) on the device,
+// with the basis kernels of cldl_eigsh (k_eig_dots at z = w, k_eig_update without MV) and the products and analyses of
+// the refined solves.  K z is k_refine_residual at b = 0 on the current values, which writes -K z to the work vector of
+// the residual (and |K||z|, the rows' maxima to kx, rmax): a cycle's v_0 = r / beta is stored before its first
+// product, and an analysis after the last product precedes the estimator.  The h and s slots live in `sc`; fetch()
+// reads them to pinned memory and waits: the one synchronisation of a step.
+static_assert(KRYLOV_MAX_RESTART <= EIG_MAX_NCV, "k_eig_update holds up to EIG_MAX_NCV + 1 coefficients");
+namespace {
+struct DevKrylovOps final : KrylovOps {
+  LDLObject& o;
+  int n, m;
+  const double* b;
+  double *xbest, *xc, *cur;    // the output, the iterate being formed, the one analysed next
+  double *V, *Z, *part, *sc, *dy;
+  double* hsc;                 // pinned: the scalars of fetch(), then -y of correct()
+  double *w, *zero, *r, *kx, *rmax;   // refine work vectors
+  unsigned* cnt;
+  bool first = true;
+  uint32_t products = 0;
+  double norm_K = 0.0, rec[4] = {0.0, 0.0, 0.0, 0.0}, best[4] = {0.0, 0.0, 0.0, 0.0};   // ||x||, ||r||, omega1, omega2
+  DevKrylovOps(LDLObject& obj) : o(obj) {}
+
+  double* col(double* B, int j) const { return B + (size_t)j * n; }
+  double* hslot(int slot) const { return sc + (size_t)slot * (m + 1); }
+  double* sslot(int slot) const { return sc + 2 * (size_t)(m + 1) + slot; }
+  static int ok() { return cudaGetLastError() == cudaSuccess ? 0 : CLDL_E_CUDA; }
+
+  int residual() override {
+    return cudaMemcpyAsync(w, r, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, o.stream) == cudaSuccess
+               ? 0 : CLDL_E_CUDA;
+  }
+  int precondition(int j) override { return o.solve_async(col(Z, j), col(V, j)); }
+  int apply(int j) override {
+    const double* t = r;
+    double* ww = w;
+    g_launches += 2;
+    k_refine_residual<<<(unsigned)((n + RF_NT / 32 - 1) / (RF_NT / 32)), RF_NT, 0, o.stream>>>(
+        n, o.d_rf_rowptr, o.d_rf_col, o.d_rf_src, o.dev.vals, col(Z, j), zero, r, kx, rmax, nullptr);
+    k_map<<<(n + 255) / 256, 256, 0, o.stream>>>(n, [=] __device__(int i) { ww[i] = -t[i]; });
+    products++;
+    return ok();
+  }
+  int dots(int j, int slot) override {
+    g_launches++;
+    k_eig_dots<<<red_grid(n), RED_THREADS, 0, o.stream>>>(n, j, V, w, part, cnt, hslot(slot));
+    return ok();
+  }
+  int update(int j, int slot) override {
+    g_launches++;
+    k_eig_update<<<(n + 255) / 256, 256, 0, o.stream>>>(n, j, V, nullptr, hslot(slot), w, nullptr);
+    return ok();
+  }
+  int norm2(int slot) override {
+    const double* ww = w;
+    g_launches++;
+    k_sum<<<red_grid(n), RED_THREADS, 0, o.stream>>>(n, [=] __device__(int i) { return ww[i] * ww[i]; },
+                                                     ReduceWS{part, cnt}, sslot(slot));
+    return ok();
+  }
+  int store(int j, int slot) override {
+    const double *ww = w, *s = sslot(slot);
+    double* v = col(V, j);
+    g_launches++;
+    k_map<<<(n + 255) / 256, 256, 0, o.stream>>>(n, [=] __device__(int i) {
+      const double sv = *s, d = sv > 0.0 ? sqrt(sv) : 0.0;
+      v[i] = d > 0.0 ? ww[i] / d : 0.0;
+    });
+    return ok();
+  }
+  int correct(int k, const double* y) override {
+    double* ny = hsc + 2 * (size_t)(m + 1) + 4;     // the last copy out of it finished at the last analysis
+    for (int i = 0; i < k; i++) ny[i] = -y[i];
+    if (cudaMemcpyAsync(dy, ny, (size_t)k * sizeof(double), cudaMemcpyHostToDevice, o.stream) != cudaSuccess ||
+        cudaMemcpyAsync(xc, xbest, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, o.stream) != cudaSuccess)
+      return CLDL_E_CUDA;
+    g_launches++;
+    k_eig_update<<<(n + 255) / 256, 256, 0, o.stream>>>(n, k, Z, nullptr, dy, xc, nullptr);   // x -= Z (-y)
+    cur = xc;
+    return ok();
+  }
+  int keep() override {
+    if (cur != xbest &&
+        cudaMemcpyAsync(xbest, cur, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, o.stream) != cudaSuccess)
+      return CLDL_E_CUDA;
+    for (int q = 0; q < 4; q++) best[q] = rec[q];
+    return 0;
+  }
+  int analyse(double om[2]) override {
+    if (int rc = o.refine_analyse(cur, b, first)) return rc;
+    products++;
+    if (first) {
+      norm_K = o.h_rf[RF_KN];
+      first = false;   // the first analysis left ||K||'s row sums in the vector that becomes the products' b = 0
+      if (cudaMemsetAsync(zero, 0, (size_t)n * sizeof(double), o.stream) != cudaSuccess) return CLDL_E_CUDA;
+    }
+    rec[0] = o.h_rf[RF_XN]; rec[1] = o.h_rf[RF_RINF]; rec[2] = o.h_rf[RF_W1]; rec[3] = o.h_rf[RF_W2];
+    om[0] = rec[2];
+    om[1] = rec[3];
+    return 0;
+  }
+  int fetch(int j, double* h0, double* h1, double s[4]) override {
+    if (cudaMemcpyAsync(hsc, sc, (2 * (size_t)(m + 1) + 4) * sizeof(double), cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+        cudaStreamSynchronize(o.stream) != cudaSuccess)
+      return CLDL_E_CUDA;
+    for (int i = 0; i < j; i++) { h0[i] = hsc[i]; h1[i] = hsc[m + 1 + i]; }
+    for (int q = 0; q < 4; q++) s[q] = hsc[2 * (m + 1) + q];
+    return 0;
+  }
+};
+}  // namespace
+
+// x0 = the plain solve into d_x, then fgmres_run; the kept iterate is d_x.  Work vectors of the refined solves: xc in
+// the first, the residual in the second (the products' -K z too), b = 0 in the third (after the first analysis), kx and
+// rmax in the fourth and fifth, w in the sixth.
+int LDLObject::solve_gmres(double* d_x, const double* d_b, const cldl_gmres_opts& op, cldl_gmres_info* info) {
+  if (sharded() || schur) return CLDL_E_ARG;
+  if (!(op.restart >= 1 && op.restart <= std::min(n, KRYLOV_MAX_RESTART))) return CLDL_E_ARG;
+  if (op.max_iter < 0 || !(op.tol >= 0.0)) return CLDL_E_ARG;
+  if (2 * nnzA - n > 0x7fffffff) return CLDL_E_ARG;
+  if (!factor_ok) return CLDL_E_NOT_FACTORED;
+  if (null_count > 0) return CLDL_E_ARG;
+  const int m = op.restart;
+  CK(cudaSetDevice(device));
+  if (!d_rf_work) {
+    const size_t mk = own.mark();
+    if (int rc = refine_setup()) { own.release_since(mk); d_rf_work = nullptr; cudaGetLastError(); return rc; }
+  }
+  // The call's own buffers, all released on the way out.  A failed allocation leaves its error as the runtime's last
+  // error, which the handle's next call would report: it is cleared here (every launch of the call was checked).
+  const size_t mk = own.mark();
+  struct Release {
+    DevOwner& own;
+    size_t mk;
+    ~Release() { own.release_since(mk); cudaGetLastError(); }
+  } rel{own, mk};
+  DevKrylovOps G(*this);
+  G.n = n; G.m = m; G.b = d_b; G.xbest = G.cur = d_x;
+  CK(own.alloc(&G.V, (size_t)n * (m + 1)));
+  CK(own.alloc(&G.Z, (size_t)n * m));
+  CK(own.alloc(&G.part, (size_t)(m + 1) * RED_BLOCKS));
+  CK(own.alloc(&G.cnt, 1));
+  CK(own.alloc(&G.sc, 2 * (size_t)(m + 1) + 4));
+  CK(own.alloc(&G.dy, (size_t)m));
+  CK(own.alloc_host(&G.hsc, 2 * (size_t)(m + 1) + 4 + m));
+  G.xc = d_rf_work; G.r = d_rf_work + (size_t)n; G.zero = d_rf_work + 2 * (size_t)n;
+  G.kx = d_rf_work + 3 * (size_t)n; G.rmax = d_rf_work + 4 * (size_t)n; G.w = d_rf_work + 5 * (size_t)n;
+  CK(cudaMemsetAsync(G.cnt, 0, sizeof(unsigned), stream));
+  CK(cudaMemsetAsync(G.sc, 0, (2 * (size_t)(m + 1) + 4) * sizeof(double), stream));
+  if (int rc = solve_async(d_x, d_b)) return rc;
+  KrylovResult R;
+  if (int rc = fgmres_run(G, m, op.max_iter, op.tol, R)) return rc;
+
+  cldl_gmres_info in{};
+  in.iterations = R.iterations;
+  in.cycles = R.cycles;
+  in.solves = 1 + R.iterations;
+  in.products = G.products;
+  in.norm_K_inf = G.norm_K;
+  in.norm_x_inf = G.best[0];
+  in.resid_inf = G.best[1];
+  in.omega1 = G.best[2];
+  in.omega2 = G.best[3];
+  in.converged = in.omega1 + in.omega2 <= op.tol ? 1 : 0;
+  const double den = in.norm_K_inf * in.norm_x_inf;
+  in.scaled_resid = in.resid_inf == 0.0 ? 0.0 : in.resid_inf / den;
+  if (op.error_analysis) {
+    // den1, den2 and the sets of the returned x: the products overwrote kx and rmax since its analysis
+    if (int rc = refine_analyse(d_x, d_b, false)) return rc;
+    in.products++;
+    const bool has[2] = {h_rf[RF_HAS1] != 0.0, h_rf[RF_HAS2] != 0.0};
+    double est[2] = {0.0, 0.0};
+    for (int c = 0; c < 2; c++)
+      if (has[c] && in.norm_x_inf > 0.0)
+        if (int rc = condest(c + 1, d_b, est + c, &in.solves)) return rc;
+    if (in.norm_x_inf > 0.0) {
+      in.cond1 = est[0] / in.norm_x_inf;
+      in.cond2 = est[1] / in.norm_x_inf;
+    }
+    in.ferr = in.omega1 * in.cond1 + in.omega2 * in.cond2;
+  }
+  if (info) *info = in;
+  return CLDL_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // One factorisation on several GPUs (SURVEY 8e).  This object is one rank: it owns some subtrees of the assembly tree
 // and replicates the top part above the cut.  Both dataflow queues list the owned tasks first, then the top tasks:
 //   refactor phase 0  level-0 kernel + k_factor_df over the owned tasks
@@ -3592,6 +3778,39 @@ int cldl_eigsh(cldl_t* h, double sigma, const double* M_nzval, uint64_t nev, con
 int cldl_eigsh_dev(cldl_t* h, double sigma, const double* d_M_nzval, uint64_t nev, const cldl_eig_opts* o,
                    double* evals, double* d_X, double* resid, cldl_eig_info* info) {
   return eigsh_entry(h, sigma, d_M_nzval, true, nev, o, evals, d_X, resid, info);
+}
+
+void cldl_default_gmres_opts(cldl_gmres_opts* o) {
+  std::memset(o, 0, sizeof(*o));
+  o->restart = 20;
+  o->max_iter = 100;
+  o->tol = DBL_EPSILON;
+  o->error_analysis = 0;
+}
+void cldl_gmres_abi_sizes(uint64_t* out2) {
+  out2[0] = sizeof(cldl_gmres_opts);
+  out2[1] = sizeof(cldl_gmres_info);
+}
+int cldl_solve_gmres_dev(cldl_t* h, double* d_x, const double* d_b, const cldl_gmres_opts* opts, cldl_gmres_info* info) {
+  if (!h || !d_x || !d_b) return CLDL_E_ARG;
+  cldl_gmres_opts o;
+  if (opts) o = *opts; else cldl_default_gmres_opts(&o);
+  return h->obj.solve_gmres(d_x, d_b, o, info);
+}
+int cldl_solve_gmres(cldl_t* h, double* x, const double* b, const cldl_gmres_opts* opts, cldl_gmres_info* info) {
+  if (!h || !x || !b) return CLDL_E_ARG;
+  LDLObject& o = h->obj;
+  if (o.sharded() || o.schur) return CLDL_E_ARG;
+  if (!o.factor_ok) return CLDL_E_NOT_FACTORED;
+  if (cudaSetDevice(o.device) != cudaSuccess) return CLDL_E_CUDA;
+  const size_t bytes = (size_t)o.n * sizeof(double);
+  if (cudaMemcpyAsync(o.d_bx, b, bytes, cudaMemcpyHostToDevice, o.stream) != cudaSuccess) return CLDL_E_CUDA;
+  int rc = cldl_solve_gmres_dev(h, o.d_bx + o.n, o.d_bx, opts, info);
+  if (rc) return rc;
+  if (cudaMemcpyAsync(x, o.d_bx + o.n, bytes, cudaMemcpyDeviceToHost, o.stream) != cudaSuccess ||
+      cudaStreamSynchronize(o.stream) != cudaSuccess)
+    return CLDL_E_CUDA;
+  return CLDL_OK;
 }
 
 int cldl_create_schur(cldl_t** out, uint64_t n, const uint64_t* colptr, const uint64_t* rowval,

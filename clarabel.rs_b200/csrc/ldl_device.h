@@ -253,6 +253,9 @@ class LDLObject {
   // eigenvalues nearest a shift (cldl_eigsh; ldl_eig.cpp, ldl_eig.cuh): buffers allocated and freed by each call
   int eigsh(double sigma, const double* M, bool m_dev, uint64_t nev, const cldl_eig_opts& o, double* evals, double* X,
             bool x_dev, double* resid, cldl_eig_info* info);
+  // FGMRES preconditioned by the factor (cldl_solve_gmres; ldl_krylov.cpp): basis buffers allocated and freed by each
+  // call, the refined solves' mirrored pattern and work vectors shared
+  int solve_gmres(double* d_x, const double* d_b, const cldl_gmres_opts& o, cldl_gmres_info* info);
   // Schur complement handle (cldl_create_schur; SchurPlan in ldl_plan.h): B's fronts are factored, S's never
   std::vector<int> schur_set;            // non-empty: a Schur complement handle
   bool schur = false;

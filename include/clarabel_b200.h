@@ -493,6 +493,68 @@ int cldl_eigsh(cldl_t *h, double sigma, const double *M_nzval, uint64_t nev, con
 int cldl_eigsh_dev(cldl_t *h, double sigma, const double *d_M_nzval, uint64_t nev, const cldl_eig_opts *o,
                    double *evals, double *d_X, double *resid, cldl_eig_info *info);
 
+/* Solves preconditioned by the factor: restarted right-preconditioned flexible GMRES (Saad 1993), the remedy for
+ * static pivoting of Arioli, Duff, Gratton and Pralet (2007) and Arioli and Duff (2009); PARDISO's iparm(4) for a
+ * factor reused on new values.  K is the matrix of the handle's CURRENT values, as in cldl_solve_refined; the
+ * preconditioner K~ is the factor of the last refactor, which is K + E when pivots were regularised
+ * (cldl_info.regularize_count) and that of older values when values changed since.  Where refinement stalls (a
+ * regularised pivot, a large value change) FGMRES still converges: K~^-1 K is the identity plus a matrix of rank
+ * regularize_count, or of rank at most 2 r for values changed in r columns, and GMRES needs about that many steps plus
+ * one.
+ *   - x0 is the plain solve, bitwise cldl_solve(b), analysed with omega1 / omega2 exactly as in cldl_solve_refined.
+ *   - A cycle starts from r = b - K x of the last analysis, beta = ||r||_2, v_0 = r / beta.  Step j: z_j = K~^-1 v_j
+ *     (kept as column j of Z), w = K z_j, classical Gram-Schmidt twice against v_0 .. v_j, giving h_{0..j,j} and
+ *     h_{j+1,j} = ||w||_2, and v_{j+1} = w / h_{j+1,j}.  The Givens rotations and the least-squares solve run on the
+ *     host in double precision, in a fixed order.
+ *   - A cycle ends after `restart` steps, when the call has made max_iter steps, at a breakdown (h_{j+1,j} <=
+ *     2^-40 ||K z_j||_2: the solution lies in the space), at a non-finite value (that step is not used), or when the
+ *     estimated residual |g_{j+1}| <= (tol / omega_c) beta, omega_c = omega1 + omega2 at the cycle's start.  Then
+ *     x = x + Z y (y the least-squares solution) is analysed.
+ *   - The call stops at omega1 + omega2 <= tol, at max_iter steps, at a non-finite omega1 + omega2, or when a cycle
+ *     did not lower omega1 + omega2 below omega_c.  The iterate with the smallest omega1 + omega2 is returned (the
+ *     earlier one on a tie), with its analysis in info.  max_iter = 0 returns x0 and its analysis; tol = 0 runs until
+ *     max_iter steps or stagnation.
+ *   - Error analysis (error_analysis = 1): cond1, cond2 and ferr at the returned x, as in cldl_solve_refined (K^-1
+ *     there is K~^-1, the inverse of the factored matrix).  The returned x is analysed once more first.
+ *   - Returns CLDL_OK or a negative code; convergence is info.converged, not the return value.  CLDL_E_NOT_FACTORED
+ *     without a refactor that returned 1.  CLDL_E_ARG on Schur and sharded handles, for restart outside
+ *     [1, min(n, 512)], max_iter < 0, tol < 0 or NaN, when 2 nnzA - n does not fit int32 (the mirrored pattern), and
+ *     for a factor with null pivots.  CLDL_E_CUDA when an allocation fails: the call's buffers are freed, the runtime's
+ *     last error is cleared and the handle stays usable.
+ *   - No floating-point atomics and fixed reduction orders: two calls give the same bits.  The factor, D, 1/D, the
+ *     values and every later solve are left bit for bit unchanged.
+ *   - Synchronisation: BOTH forms synchronise the handle's stream once per Arnoldi step and once per analysis (and
+ *     after each solve of the estimator).  cldl_solve_gmres_dev takes device buffers (d_x and d_b must not overlap)
+ *     and never copies a vector to the host.
+ *   - Memory: the call allocates (restart + 1) n doubles for V, restart n for Z and (restart + 1) 296 of reduction
+ *     partials plus a few scalars, and frees them before it returns.  The first call also sets up
+ *     cldl_solve_refined's mirrored pattern and work vectors, which stay.
+ * opts == NULL means the defaults of cldl_default_gmres_opts; info may be NULL. */
+typedef struct {
+  int32_t restart;         /* Arnoldi steps per cycle, 1 .. min(n, 512)                         (default 20) */
+  int32_t max_iter;        /* Arnoldi steps in all; 0 = the plain solve, analysed only          (default 100) */
+  double tol;              /* stop once omega1 + omega2 <= tol                                  (default DBL_EPSILON) */
+  int32_t error_analysis;  /* 1: also estimate cond1, cond2 and ferr (extra solves)             (default 0) */
+} cldl_gmres_opts;
+
+typedef struct {
+  uint32_t iterations;     /* Arnoldi steps taken */
+  uint32_t cycles;         /* cycles begun */
+  uint32_t solves;         /* LDL solves made by the call: x0, one per step, the estimator's */
+  uint32_t products;       /* products with K: one per step and one per analysis */
+  int32_t converged;       /* 1 when the returned x has omega1 + omega2 <= tol */
+  double norm_K_inf, norm_x_inf, resid_inf;   /* ||K||_inf (current values), ||x||_inf, ||b - K x||_inf */
+  double scaled_resid;     /* resid_inf / (norm_K_inf * norm_x_inf); 0 when resid_inf = 0 */
+  double omega1, omega2;   /* componentwise backward errors of the returned x */
+  double cond1, cond2, ferr;   /* error_analysis only, else 0 */
+} cldl_gmres_info;
+
+void cldl_default_gmres_opts(cldl_gmres_opts *o);
+void cldl_gmres_abi_sizes(uint64_t *out2);     /* sizeof cldl_gmres_opts, cldl_gmres_info */
+int cldl_solve_gmres(cldl_t *h, double *x, const double *b, const cldl_gmres_opts *opts, cldl_gmres_info *info);
+int cldl_solve_gmres_dev(cldl_t *h, double *d_x, const double *d_b, const cldl_gmres_opts *opts,
+                         cldl_gmres_info *info);
+
 /* ---- device-pointer twins (asynchronous on the handle's stream) ---- */
 int cldl_update_values_dev(cldl_t *h, const int32_t *d_index, const double *d_values, uint64_t len);
 int cldl_set_values_dev(cldl_t *h, const double *d_nzval);   /* whole array, caller order */
